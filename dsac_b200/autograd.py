@@ -1,0 +1,104 @@
+"""The engine's losses as differentiable PyTorch functions, for training the coordinate CNN end to end.
+
+    loss = softam_loss(engine, prediction, pix, gt_jp)              # soft-argmax pipeline, [n]
+    loss = dsac_expected_loss(engine, prediction, pix, gt_jp)       # DSAC / RANSAC variant, [n]
+    loss.sum().backward()                                           # prediction.grad
+
+`prediction` is the coordinate CNN's output: float32 [n][1600][3] scene coordinates in metres on the engine's device,
+cell y*40+x.  It is the only input that receives a gradient.  The gradient is the one the reference hands to
+model:backward (lua/train_obj_softam.lua:101-105): dLoss/dObj clamped to +-clamp, scaled by the incoming gradient, per
+millimetre of the int16 grid, straight through the rounding to millimetres (DESIGN.md quirk Q12).
+
+Everything stays on the device, on torch.cuda.current_stream().  The engine holds one pass: a forward on the same engine
+between a loss and its backward() makes that backward() raise.
+"""
+import torch
+
+from . import engine as _E
+
+
+def _check_inputs(engine, prediction, pix, gt_jp):
+    dev = torch.device("cuda", engine.cfg.device)
+    if gt_jp is None:
+        raise ValueError("the loss needs the ground-truth poses gt_jp [n][12]")
+    n = prediction.shape[0] if prediction.dim() == 3 else -1
+    if prediction.dtype != torch.float32 or tuple(prediction.shape[1:]) != (_E.N, 3) or prediction.dim() != 3:
+        raise ValueError("prediction must be float32 [n][%d][3], got %s %s" % (_E.N, prediction.dtype, tuple(prediction.shape)))
+    if not 1 <= n <= engine.cfg.max_frames:
+        raise ValueError("%d frames, the engine holds 1..%d" % (n, engine.cfg.max_frames))
+    for name, t in (("prediction", prediction), ("pix", pix), ("gt_jp", gt_jp)):
+        if t.device != dev:
+            raise ValueError("%s is on %s, the engine on %s" % (name, t.device, dev))
+    if pix.dtype != torch.int32 or pix.numel() not in (_E.N * 2, n * _E.N * 2):
+        raise ValueError("pix must be int32 [N][2] (shared) or [n][N][2]")
+    if gt_jp.dtype != torch.float64 or gt_jp.numel() != n * 12:
+        raise ValueError("gt_jp must be float64 [n][12]")
+    return n, pix.contiguous(), gt_jp.contiguous(), (1 if pix.numel() == _E.N * 2 else 0)
+
+
+def _coords(engine, prediction, stream):
+    n = prediction.shape[0]
+    coords = torch.empty((n, _E.N, 3), dtype=torch.int16, device=prediction.device)
+    engine.coords_from_prediction_device(n, prediction.data_ptr(), coords.data_ptr(), stream)
+    return coords
+
+
+def _grad_input(ctx, grad_loss):
+    if ctx.engine.passes != ctx.pass_id:
+        raise RuntimeError("the engine ran another forward pass after this loss was computed: its backward() would "
+                           "differentiate that pass; call backward() before the next forward, or use a second engine")
+    g = grad_loss.detach().to(torch.float64).contiguous()
+    return g, torch.empty((ctx.n, _E.N, 3), dtype=torch.float32, device=g.device)
+
+
+class _SoftamLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, prediction, engine, pix, gt_jp, frame0, clamp):
+        n, pix, gt_jp, shared = _check_inputs(engine, prediction, pix, gt_jp)
+        stream = torch.cuda.current_stream(prediction.device).cuda_stream
+        pred = prediction.detach().contiguous()
+        coords = _coords(engine, pred, stream)
+        engine.forward_device(n, coords.data_ptr(), pix.data_ptr(), shared, gt_jp.data_ptr(), frame0, stream)
+        loss = torch.empty(n, dtype=torch.float64, device=prediction.device)
+        engine.fetch_device(n, stream, loss=loss.data_ptr())
+        ctx.engine, ctx.pass_id, ctx.n, ctx.clamp = engine, engine.passes, n, clamp
+        ctx.keep = (coords, pix, gt_jp)   # the engine's backward reads the pass's inputs
+        return loss
+
+    @staticmethod
+    def backward(ctx, grad_loss):
+        g, grad = _grad_input(ctx, grad_loss)
+        ctx.engine.backward_device(ctx.n, g.data_ptr(), None, grad.data_ptr(), ctx.clamp, torch.cuda.current_stream(g.device).cuda_stream)
+        return grad, None, None, None, None, None
+
+
+class _DsacExpectedLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, prediction, engine, pix, gt_jp, frame0, random_draw, clamp):
+        n, pix, gt_jp, shared = _check_inputs(engine, prediction, pix, gt_jp)
+        stream = torch.cuda.current_stream(prediction.device).cuda_stream
+        coords = _coords(engine, prediction.detach().contiguous(), stream)
+        loss = torch.empty(n, dtype=torch.float64, device=prediction.device)
+        engine.forward_dsac_device(n, coords.data_ptr(), pix.data_ptr(), shared, gt_jp.data_ptr(), random_draw, frame0, stream,
+                                   expected_loss=loss.data_ptr())
+        ctx.engine, ctx.pass_id, ctx.n, ctx.clamp = engine, engine.passes, n, clamp
+        ctx.keep = (coords, pix, gt_jp)
+        return loss
+
+    @staticmethod
+    def backward(ctx, grad_loss):
+        g, grad = _grad_input(ctx, grad_loss)
+        ctx.engine.backward_dsac_device(ctx.n, g.data_ptr(), grad.data_ptr(), ctx.clamp, torch.cuda.current_stream(g.device).cuda_stream)
+        return grad, None, None, None, None, None, None
+
+
+def softam_loss(engine, prediction, pix, gt_jp, frame0=0, clamp=0.1):
+    """Per-frame loss of the soft-argmax pipeline (train_ransac_softam.cpp) on `prediction`, float64 [n]; differentiable
+    with respect to `prediction`.  frame0: global index of the first frame (keys the sampler streams)."""
+    return _SoftamLoss.apply(prediction, engine, pix, gt_jp, int(frame0), float(clamp))
+
+
+def dsac_expected_loss(engine, prediction, pix, gt_jp, frame0=0, random_draw=True, clamp=0.1):
+    """Per-frame expected loss of the DSAC / RANSAC variant (train_ransac.cpp) on `prediction`, float64 [n];
+    differentiable with respect to `prediction`."""
+    return _DsacExpectedLoss.apply(prediction, engine, pix, gt_jp, int(frame0), bool(random_draw), float(clamp))

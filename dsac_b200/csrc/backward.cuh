@@ -732,6 +732,9 @@ __global__ void k_kabsch(int n, int m, const double* __restrict__ a, const doubl
 
 int backward_run(dsac_engine* e, int32_t n, const int16_t* coords, const int32_t* pix, int32_t pix_shared,
                  const double* gt_jp, dsac_backward_out* out);
+int backward_device_run(dsac_engine* e, int32_t n, const double* d_loss_grad, double* d_dloss_dobj, float* d_dloss_dpred,
+                        float clamp, cudaStream_t stream);
 int kabsch_run(dsac_engine* e, int32_t n, int32_t m, const double* a, const double* b, double* R, double* t);
 struct dsac_backward_dsac_out;
-int backward_dsac_run(dsac_engine* e, int32_t n, dsac_backward_dsac_out* out);
+int backward_dsac_run(dsac_engine* e, int32_t n, const double* d_loss_grad, const dsac_backward_dsac_out* out, bool out_on_host,
+                      float* d_dloss_dpred, float clamp, cudaStream_t stream);

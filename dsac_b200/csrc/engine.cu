@@ -21,6 +21,7 @@
 #include "kernels.cuh"
 #include "refine.cuh"
 #include "sampler_split.cuh"
+#include "train.cuh"
 #include "upstream.cuh"
 
 using namespace dsac;
@@ -67,6 +68,10 @@ struct dsac_engine {
     int32_t* d_ra_frame = nullptr; double* d_ra_pose = nullptr; double* d_ra_loss = nullptr; double* d_ra_rot = nullptr;
     double* d_ra_t = nullptr; int32_t* d_ra_correct = nullptr; int32_t* d_ra_steps = nullptr; int32_t* d_ra_imap = nullptr;
     size_t ra_jobs = 0, ra_imap_jobs = 0;
+    // per-frame results of k_dsac_draw: drawn hypothesis, expected loss, its errors
+    int32_t* d_dsac_pick = nullptr; double* d_dsac_exp = nullptr; double* d_dsac_rot = nullptr; double* d_dsac_terr = nullptr;
+    int32_t* d_dsac_correct = nullptr;
+    int32_t* h_totals = nullptr;    // pinned [2]: selected hypotheses and refinement jobs of dsac_backward_dsac_device
     uint32_t* d_status = nullptr;
     unsigned long long* d_fragile = nullptr;
     unsigned long long* d_phase = nullptr;   // K1 per-phase cycle counters (DSAC_K1_TIMERS=1), else null
@@ -266,10 +271,12 @@ void dsac_engine_destroy(dsac_engine* e) {
                     e->d_stream_ncand, e->d_stream_endpos, e->d_ra_frame, e->d_ra_pose, e->d_ra_loss, e->d_ra_rot, e->d_ra_t,
                     e->d_ra_correct, e->d_ra_steps, e->d_ra_imap, e->d_status, e->d_fragile, e->d_diffmaps, e->d_scores, e->d_sf, e->d_entropy,
                     e->d_avg, e->d_ref, e->d_inlier_map, e->d_steps_done, e->d_n_perm, e->d_loss, e->d_rot_err,
-                    e->d_t_err, e->d_correct, e->d_frame_counter};
+                    e->d_t_err, e->d_correct, e->d_frame_counter, e->d_dsac_pick, e->d_dsac_exp, e->d_dsac_rot, e->d_dsac_terr,
+                    e->d_dsac_correct};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     if (e->h_stream_ncand) cudaFreeHost(e->h_stream_ncand);
+    if (e->h_totals) cudaFreeHost(e->h_totals);
     backward_scratch_free(&e->bw);
     for (auto& slot : e->bw_pool)
         if (slot.first) cudaFree(slot.first);
@@ -338,6 +345,12 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
     CUC(cudaMalloc(&e->d_t_err, n * sizeof(double)));
     CUC(cudaMalloc(&e->d_correct, n * sizeof(int32_t)));
     CUC(cudaMalloc(&e->d_frame_counter, n * sizeof(unsigned int)));
+    CUC(cudaMalloc(&e->d_dsac_pick, n * sizeof(int32_t)));
+    CUC(cudaMalloc(&e->d_dsac_exp, n * sizeof(double)));
+    CUC(cudaMalloc(&e->d_dsac_rot, n * sizeof(double)));
+    CUC(cudaMalloc(&e->d_dsac_terr, n * sizeof(double)));
+    CUC(cudaMalloc(&e->d_dsac_correct, n * sizeof(int32_t)));
+    CUC(cudaMallocHost(&e->h_totals, 2 * sizeof(int32_t)));
     CUC(cudaMemset(e->d_frame_counter, 0, n * sizeof(unsigned int)));
     CUC(cudaMemset(e->d_fragile, 0, sizeof(unsigned long long)));
     if (getenv("DSAC_K1_TIMERS")) {
@@ -944,13 +957,14 @@ int dsac_forward_device(dsac_engine* e, int32_t n, int64_t frame0, const int16_t
     return DSAC_OK;
 }
 
-// Queues the device->host copies of frames [off, off+n) into the caller's buffers (no synchronisation).
+// Queues the copies of frames [off, off+n) into the caller's buffers (no synchronisation).  cudaMemcpyDefault: a
+// destination may be host or device memory; n_candidates goes through the pinned per-stream counts (summed on the host).
 static int fetch_range(dsac_engine* e, int32_t off, int32_t n, dsac_forward_out* o, cudaStream_t stream) {
     const size_t H = e->cfg.n_hyps, N = DSAC_N, T = e->cfg.n_streams, nn = (size_t)n, f = (size_t)off;
 #define D2H(dst, src, per)                                                                                          \
     do {                                                                                                            \
         if ((dst) && (src))                                                                                         \
-            CU(cudaMemcpyAsync((dst) + f * (per), (src) + f * (per), nn * (per) * sizeof(*(dst)), cudaMemcpyDeviceToHost, stream)); \
+            CU(cudaMemcpyAsync((dst) + f * (per), (src) + f * (per), nn * (per) * sizeof(*(dst)), cudaMemcpyDefault, stream)); \
     } while (0)
     D2H(o->hyp_pose, e->d_hyp_pose, H * 6);
     D2H(o->img_idx, e->d_img_idx, H * 4);
@@ -1119,16 +1133,17 @@ int dsac_forward(dsac_engine* e, int32_t n, int64_t frame0, const int16_t* coord
     return dsac_forward_wait(e);
 }
 
-int dsac_forward_dsac(dsac_engine* e, int32_t n, int64_t frame0, const int16_t* coords, const int32_t* pix,
-                      int32_t pix_shared, const double* gt_jp, int32_t random_draw, dsac_dsac_out* out) {
-    if (!e || !out) return DSAC_ERR_ARG;
+// The DSAC variant's forward over device-resident inputs into the engine's buffers: sampling and scoring, refinement of
+// every hypothesis from its own pose (cnn.h:1155-1218), then the draw and the expected loss (k_dsac_draw).  Nothing is
+// copied to the host.  want_imaps: keep the inlier maps of every hypothesis.
+static int forward_dsac_run(dsac_engine* e, int32_t n, int64_t frame0, const int16_t* d_coords, const int32_t* d_pix,
+                            int32_t pix_shared, const double* d_gt, int32_t random_draw, bool want_imaps, cudaStream_t stream) {
     if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_forward_dsac: a submitted pass has not been awaited (dsac_forward_wait)");
     if (n < 1 || n > e->cfg.max_frames) return fail(e, DSAC_ERR_CAPACITY, "n_frames %d exceeds engine capacity %d", n, e->cfg.max_frames);
-    if (!coords || !pix) return fail(e, DSAC_ERR_ARG, "null input");
+    if (!d_coords || !d_pix) return fail(e, DSAC_ERR_ARG, "null input");
     const dsac_config& c = e->cfg;
     CU(cudaSetDevice(c.device));
-    cudaStream_t stream = e->pipe[0];
-    const size_t N = DSAC_N, nn = (size_t)n, H = c.n_hyps, jobs = nn * H, T = c.n_streams;
+    const size_t N = DSAC_N, nn = (size_t)n, H = c.n_hyps, jobs = nn * H;
     // refine-all buffers
     if (jobs > e->ra_jobs) {
         void* old[] = {e->d_ra_frame, e->d_ra_pose, e->d_ra_loss, e->d_ra_rot, e->d_ra_t, e->d_ra_correct, e->d_ra_steps};
@@ -1149,29 +1164,32 @@ int dsac_forward_dsac(dsac_engine* e, int32_t n, int64_t frame0, const int16_t* 
         CU(cudaMemcpy(e->d_ra_frame, jf.data(), jobs * sizeof(int32_t), cudaMemcpyHostToDevice));
         e->ra_jobs = jobs;
     }
-    if (out->inlier_maps && jobs > e->ra_imap_jobs) {
+    if (want_imaps && jobs > e->ra_imap_jobs) {
         if (e->d_ra_imap) cudaFree(e->d_ra_imap);
         e->d_ra_imap = nullptr;
         e->ra_imap_jobs = 0;
         CU(cudaMalloc(&e->d_ra_imap, jobs * N * sizeof(int32_t)));
         e->ra_imap_jobs = jobs;
     }
-    CU(cudaMemcpyAsync(e->d_coords, coords, nn * N * 3 * sizeof(int16_t), cudaMemcpyHostToDevice, stream));
-    CU(cudaMemcpyAsync(e->d_pix, pix, (pix_shared ? 1 : nn) * N * 2 * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
-    if (gt_jp) CU(cudaMemcpyAsync(e->d_gt, gt_jp, nn * 12 * sizeof(double), cudaMemcpyHostToDevice, stream));
-    e->cur_coords = e->d_coords; e->cur_pix = e->d_pix; e->cur_pix_shared = pix_shared; e->cur_gt = gt_jp ? e->d_gt : nullptr;
+    e->cur_coords = d_coords; e->cur_pix = d_pix; e->cur_pix_shared = pix_shared; e->cur_gt = d_gt;
     e->cur_n = 0;   // the soft-argmax backward does not apply to this pass
     e->dsac_n = 0;
     e->cur_frame0 = frame0;
     const uint32_t saved = e->stages;
     e->stages = DSAC_STAGE_SAMPLE | DSAC_STAGE_SCORE;
-    int rc = forward_range(e, 0, n, frame0, e->d_coords, e->d_pix, pix_shared, e->cur_gt, stream);
+    int rc = forward_range(e, 0, n, frame0, d_coords, d_pix, pix_shared, d_gt, stream);
     e->stages = saved;
     if (rc != DSAC_OK) return rc;
+    if (!d_gt) {   // no ground truth: losses and errors are zero
+        CU(cudaMemsetAsync(e->d_ra_loss, 0, jobs * sizeof(double), stream));
+        CU(cudaMemsetAsync(e->d_ra_rot, 0, jobs * sizeof(double), stream));
+        CU(cudaMemsetAsync(e->d_ra_t, 0, jobs * sizeof(double), stream));
+        CU(cudaMemsetAsync(e->d_ra_correct, 0, jobs * sizeof(int32_t), stream));
+    }
     {   // every hypothesis is a refinement job starting from its own pose (cnn.h:1155-1218)
         RefineParams rp;
         memset(&rp, 0, sizeof(rp));
-        rp.coords = e->d_coords; rp.pix = e->d_pix; rp.pix_stride = pix_shared ? 0 : DSAC_N * 2;
+        rp.coords = d_coords; rp.pix = d_pix; rp.pix_stride = pix_shared ? 0 : DSAC_N * 2;
         rp.perm = e->d_perm;
         rp.f = c.focal; rp.cx = c.cx; rp.cy = c.cy;
         rp.thr = c.thr2d; rp.inlier_count = c.inlier_count; rp.ref_steps = c.ref_steps;
@@ -1180,86 +1198,85 @@ int dsac_forward_dsac(dsac_engine* e, int32_t n, int64_t frame0, const int16_t* 
         rp.job_init = e->d_hyp_pose;
         rp.out_pose = e->d_ra_pose;
         rp.steps_done = e->d_ra_steps;
-        rp.inlier_map = out->inlier_maps ? e->d_ra_imap : nullptr;
-        if (e->cur_gt) {
-            rp.gt_jp = e->cur_gt;
+        rp.inlier_map = want_imaps ? e->d_ra_imap : nullptr;
+        if (d_gt) {
+            rp.gt_jp = d_gt;
             rp.loss = e->d_ra_loss; rp.rot_err = e->d_ra_rot; rp.t_err = e->d_ra_t; rp.correct = e->d_ra_correct;
         }
         k_refine<<<(unsigned)jobs, K4_THREADS, 0, stream>>>(rp);
         e->launches++;
         CU(cudaGetLastError());
     }
-    std::vector<double> sf(nn * H), loss(jobs, 0.0), rot(jobs, 0.0), terr(jobs, 0.0);
-    std::vector<int32_t> correct(jobs, 0), idx(nn * H * 4);
-    std::vector<unsigned long long> endpos(nn * T);
-    CU(cudaMemcpyAsync(sf.data(), e->d_sf, nn * H * sizeof(double), cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(idx.data(), e->d_img_idx, nn * H * 4 * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(endpos.data(), e->d_stream_endpos, nn * T * sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
-    if (e->cur_gt) {
-        CU(cudaMemcpyAsync(loss.data(), e->d_ra_loss, jobs * sizeof(double), cudaMemcpyDeviceToHost, stream));
-        CU(cudaMemcpyAsync(rot.data(), e->d_ra_rot, jobs * sizeof(double), cudaMemcpyDeviceToHost, stream));
-        CU(cudaMemcpyAsync(terr.data(), e->d_ra_t, jobs * sizeof(double), cudaMemcpyDeviceToHost, stream));
-        CU(cudaMemcpyAsync(correct.data(), e->d_ra_correct, jobs * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
+    {
+        DrawParams dp;
+        dp.H = c.n_hyps; dp.T = c.n_streams; dp.random_draw = random_draw ? 1 : 0;
+        dp.seed = c.seed; dp.frame0 = frame0;
+        dp.sf = e->d_sf; dp.img_idx = e->d_img_idx; dp.stream_endpos = e->d_stream_endpos;
+        dp.loss = e->d_ra_loss; dp.rot_err = e->d_ra_rot; dp.t_err = e->d_ra_t; dp.correct = e->d_ra_correct;
+        dp.inlier_maps = want_imaps ? e->d_ra_imap : nullptr;
+        dp.hyp_idx = e->d_dsac_pick; dp.expected_loss = e->d_dsac_exp;
+        dp.out_rot_err = e->d_dsac_rot; dp.out_t_err = e->d_dsac_terr; dp.out_correct = e->d_dsac_correct;
+        k_dsac_draw<<<n, DRAW_THREADS, 0, stream>>>(dp);
+        e->launches++;
+        CU(cudaGetLastError());
     }
-#define D2H(dst, src, bytes)                                                                    \
-    do {                                                                                        \
-        if ((dst) && (src)) CU(cudaMemcpyAsync((dst), (src), (bytes), cudaMemcpyDeviceToHost, stream)); \
-    } while (0)
-    D2H(out->hyp_pose, e->d_hyp_pose, nn * H * 6 * sizeof(double));
-    D2H(out->entropy, e->d_entropy, nn * sizeof(double));
-    D2H(out->ref_pose, e->d_ra_pose, jobs * 6 * sizeof(double));
-    D2H(out->steps_done, e->d_ra_steps, jobs * sizeof(int32_t));
-    D2H(out->inlier_maps, e->d_ra_imap, jobs * N * sizeof(int32_t));
-    D2H(out->status, e->d_status, nn * sizeof(uint32_t));
-#undef D2H
-    CU(cudaStreamSynchronize(stream));
-    if (out->sf) memcpy(out->sf, sf.data(), nn * H * sizeof(double));
-    if (out->img_idx) memcpy(out->img_idx, idx.data(), nn * H * 4 * sizeof(int32_t));
-    if (out->losses) memcpy(out->losses, loss.data(), jobs * sizeof(double));
-    for (size_t f = 0; f < nn; f++) {
-        const double* p = &sf[f * H];
-        // draw(), cnn.h:102-126
-        double probSum = 0, maxProb = -1;
-        int maxIdx = 0, pick = 0;
-        for (size_t i = 0; i < H; i++) {
-            if (p[i] < 1e-8) continue;
-            probSum += p[i];
-            if (maxProb < 0 || p[i] > maxProb) { maxProb = p[i]; maxIdx = (int)i; }
-        }
-        if (random_draw) {
-            // thread 0's generator continues after the sampling loop: same libstdc++ calls as drand (thread_rand.cpp:71-81)
-            std::mt19937 gen;
-            gen.seed(c.seed + (uint32_t)((frame0 + (long long)f) * (long long)T));
-            gen.discard(endpos[f * T]);
-            std::uniform_real_distribution<double> dist(0, probSum);
-            const double u = dist(gen);
-            double cum = 0;
-            bool found = false;
-            for (size_t i = 0; i < H; i++) {
-                if (p[i] < 1e-8) continue;
-                cum += p[i];
-                pick = (int)i;
-                if (cum > u) { found = true; break; }   // std::map::upper_bound on the cumulative sums
-            }
-            (void)found;
-        } else {
-            pick = maxIdx;
-        }
-        double expected = 0;
-        for (size_t h = 0; h < H; h++) expected += p[h] * loss[f * H + h];   // expectedMaxLoss, cnn.h:137-151
-        if (out->expected_loss) out->expected_loss[f] = expected;
-        if (out->hyp_idx) out->hyp_idx[f] = pick;
-        if (out->rot_err) out->rot_err[f] = rot[f * H + pick];
-        if (out->t_err) out->t_err[f] = terr[f * H + pick];
-        if (out->correct) out->correct[f] = correct[f * H + pick];
-        if (out->inlier_maps)   // the minimal set is excluded from its own inlier map (cnn.h:1221-1227)
-            for (size_t h = 0; h < H; h++)
-                for (int j = 0; j < 4; j++) {
-                    int cidx = idx[(f * H + h) * 4 + j];
-                    if (cidx >= 0) out->inlier_maps[(f * H + h) * N + cidx] = 0;
-                }
-    }
+    CU(cudaEventRecord(e->ev_fwd, stream));   // the backward waits on this
     e->dsac_n = n;
+    return DSAC_OK;
+}
+
+// Queues the copies of the outputs `out` asks for; destinations may be host or device memory (cudaMemcpyDefault).
+static int forward_dsac_copy(dsac_engine* e, int32_t n, const dsac_dsac_out* out, cudaStream_t stream) {
+    const size_t N = DSAC_N, nn = (size_t)n, H = e->cfg.n_hyps, jobs = nn * H;
+#define CP(dst, src, bytes)                                                                     \
+    do {                                                                                        \
+        if (dst) CU(cudaMemcpyAsync((dst), (src), (bytes), cudaMemcpyDefault, stream));        \
+    } while (0)
+    CP(out->hyp_pose, e->d_hyp_pose, jobs * 6 * sizeof(double));
+    CP(out->img_idx, e->d_img_idx, jobs * 4 * sizeof(int32_t));
+    CP(out->sf, e->d_sf, jobs * sizeof(double));
+    CP(out->entropy, e->d_entropy, nn * sizeof(double));
+    CP(out->ref_pose, e->d_ra_pose, jobs * 6 * sizeof(double));
+    CP(out->losses, e->d_ra_loss, jobs * sizeof(double));
+    CP(out->inlier_maps, e->d_ra_imap, jobs * N * sizeof(int32_t));
+    CP(out->steps_done, e->d_ra_steps, jobs * sizeof(int32_t));
+    CP(out->expected_loss, e->d_dsac_exp, nn * sizeof(double));
+    CP(out->hyp_idx, e->d_dsac_pick, nn * sizeof(int32_t));
+    CP(out->rot_err, e->d_dsac_rot, nn * sizeof(double));
+    CP(out->t_err, e->d_dsac_terr, nn * sizeof(double));
+    CP(out->correct, e->d_dsac_correct, nn * sizeof(int32_t));
+    CP(out->status, e->d_status, nn * sizeof(uint32_t));
+#undef CP
+    return DSAC_OK;
+}
+
+int dsac_forward_dsac_device(dsac_engine* e, int32_t n, int64_t frame0, const int16_t* d_coords, const int32_t* d_pix,
+                             int32_t pix_shared, const double* d_gt_jp, int32_t random_draw, const dsac_dsac_out* d_out, void* stream_v) {
+    if (!e || !d_out) return DSAC_ERR_ARG;
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    int rc = forward_dsac_run(e, n, frame0, d_coords, d_pix, pix_shared, d_gt_jp, random_draw, d_out->inlier_maps != nullptr, stream);
+    if (rc != DSAC_OK) return rc;
+    return forward_dsac_copy(e, n, d_out, stream);
+}
+
+int dsac_forward_dsac(dsac_engine* e, int32_t n, int64_t frame0, const int16_t* coords, const int32_t* pix,
+                      int32_t pix_shared, const double* gt_jp, int32_t random_draw, dsac_dsac_out* out) {
+    if (!e || !out) return DSAC_ERR_ARG;
+    if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_forward_dsac: a submitted pass has not been awaited (dsac_forward_wait)");
+    if (n < 1 || n > e->cfg.max_frames) return fail(e, DSAC_ERR_CAPACITY, "n_frames %d exceeds engine capacity %d", n, e->cfg.max_frames);
+    if (!coords || !pix) return fail(e, DSAC_ERR_ARG, "null input");
+    CU(cudaSetDevice(e->cfg.device));
+    cudaStream_t stream = e->pipe[0];
+    const size_t N = DSAC_N, nn = (size_t)n;
+    CU(cudaMemcpyAsync(e->d_coords, coords, nn * N * 3 * sizeof(int16_t), cudaMemcpyHostToDevice, stream));
+    CU(cudaMemcpyAsync(e->d_pix, pix, (pix_shared ? 1 : nn) * N * 2 * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+    if (gt_jp) CU(cudaMemcpyAsync(e->d_gt, gt_jp, nn * 12 * sizeof(double), cudaMemcpyHostToDevice, stream));
+    int rc = forward_dsac_run(e, n, frame0, e->d_coords, e->d_pix, pix_shared, gt_jp ? e->d_gt : nullptr, random_draw,
+                              out->inlier_maps != nullptr, stream);
+    if (rc == DSAC_OK) rc = forward_dsac_copy(e, n, out, stream);
+    const cudaError_t st = cudaStreamSynchronize(stream);   // also before an error return: copies from the caller's buffers may be queued
+    if (rc != DSAC_OK) return rc;
+    if (st != cudaSuccess) return fail(e, DSAC_ERR_CUDA, "dsac_forward_dsac: %s", cudaGetErrorString(st));
     return DSAC_OK;
 }
 
@@ -1270,10 +1287,30 @@ int dsac_backward(dsac_engine* e, int32_t n, const int16_t* coords, const int32_
     return backward_run(e, n, coords, pix, pix_shared, gt_jp, out);
 }
 
+int dsac_backward_device(dsac_engine* e, int32_t n, const double* d_loss_grad, double* d_dloss_dobj, float* d_dloss_dpred,
+                         float clamp, void* stream) {
+    if (!e) return DSAC_ERR_ARG;
+    if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_backward_device: a submitted pass has not been awaited (dsac_forward_wait)");
+    return backward_device_run(e, n, d_loss_grad, d_dloss_dobj, d_dloss_dpred, clamp, (cudaStream_t)stream);
+}
+
 int dsac_backward_dsac(dsac_engine* e, int32_t n, dsac_backward_dsac_out* out) {
     if (!e || !out) return DSAC_ERR_ARG;
     if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_backward_dsac: a submitted pass has not been awaited (dsac_forward_wait)");
-    return backward_dsac_run(e, n, out);
+    cudaStream_t stream = e->pipe[0];
+    int rc = backward_dsac_run(e, n, nullptr, out, true, nullptr, 0.f, stream);
+    const cudaError_t st = cudaStreamSynchronize(stream);
+    if (rc != DSAC_OK) return rc;
+    if (st != cudaSuccess) return fail(e, DSAC_ERR_CUDA, "dsac_backward_dsac: %s", cudaGetErrorString(st));
+    return DSAC_OK;
+}
+
+int dsac_backward_dsac_device(dsac_engine* e, int32_t n, const double* d_loss_grad, const dsac_backward_dsac_out* d_out,
+                              float* d_dloss_dpred, float clamp, void* stream) {
+    if (!e) return DSAC_ERR_ARG;
+    if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_backward_dsac_device: a submitted pass has not been awaited (dsac_forward_wait)");
+    const dsac_backward_dsac_out none = {};
+    return backward_dsac_run(e, n, d_loss_grad, d_out ? d_out : &none, false, d_dloss_dpred, clamp, (cudaStream_t)stream);
 }
 
 int dsac_gather_patches_device(dsac_engine* e, int32_t n, const uint8_t* d_frames, int32_t width, int32_t height,

@@ -20,7 +20,8 @@ ST_SAMPLER_EXHAUSTED, ST_REFINE_ABORTED = 1, 2
 EXPORTS = [
     "dsac_default_config", "dsac_engine_create", "dsac_engine_destroy", "dsac_last_error", "dsac_engine_config",
     "dsac_forward", "dsac_forward_submit", "dsac_forward_wait", "dsac_forward_device", "dsac_fetch", "dsac_device_view_get", "dsac_set_stages",
-    "dsac_set_tail_split", "dsac_launch_count", "dsac_sampler_profile", "dsac_sampler_profile_read", "dsac_debug_spec_result", "dsac_set_score_hook", "dsac_set_score_backward_hook", "dsac_backward", "dsac_forward_dsac", "dsac_backward_dsac", "dsac_gather_patches_device", "dsac_coords_from_prediction_device", "dsac_kabsch",
+    "dsac_set_tail_split", "dsac_launch_count", "dsac_sampler_profile", "dsac_sampler_profile_read", "dsac_debug_spec_result", "dsac_set_score_hook", "dsac_set_score_backward_hook", "dsac_backward", "dsac_backward_device", "dsac_forward_dsac", "dsac_forward_dsac_device",
+    "dsac_backward_dsac", "dsac_backward_dsac_device", "dsac_gather_patches_device", "dsac_coords_from_prediction_device", "dsac_kabsch",
     "dsac_stochastic_subsample",
     "dsac_synth_frames", "dsac_version",
 ]
@@ -117,6 +118,11 @@ def load(build_if_missing=True):
     lib.dsac_forward_dsac.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
                                       C.POINTER(DsacOut)]
     lib.dsac_backward_dsac.argtypes = [C.c_void_p, C.c_int32, C.POINTER(BackwardDsacOut)]
+    lib.dsac_backward_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]
+    lib.dsac_forward_dsac_device.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                             C.c_int32, C.POINTER(DsacOut), C.c_void_p]
+    lib.dsac_backward_dsac_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(BackwardDsacOut), C.c_void_p, C.c_float,
+                                              C.c_void_p]
     lib.dsac_gather_patches_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
                                                C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.dsac_coords_from_prediction_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -250,6 +256,7 @@ class Engine:
             raise RuntimeError("dsac_engine_create failed (%d): %s" % (rc, self.lib.dsac_last_error(None).decode()))
         self.h = h
         self._hook = None
+        self.passes = 0   # forward passes started on this engine: the engine holds one pass, autograd.py checks it is still its own
 
     def close(self):
         if getattr(self, "h", None):
@@ -303,6 +310,7 @@ class Engine:
         assert shared or pix.size == n * N * 2
         gt = np.ascontiguousarray(gt_jp, np.float64).reshape(n, 12) if gt_jp is not None else None
         res = out if out is not None else ForwardResult(n, self.cfg.n_hyps, want_diffmaps)
+        self.passes += 1
         self._check(self.lib.dsac_forward(self.h, n, frame0, _p(coords), _p(pix), shared, _p(gt), C.byref(res.raw)))
         return res
 
@@ -315,6 +323,7 @@ class Engine:
         gt = np.ascontiguousarray(gt_jp, np.float64).reshape(n, 12) if gt_jp is not None else None
         res = out if out is not None else ForwardResult(n, self.cfg.n_hyps, want_diffmaps)
         self._pending = (coords, pix, gt, res)
+        self.passes += 1
         self._check(self.lib.dsac_forward_submit(self.h, n, frame0, _p(coords), _p(pix), shared, _p(gt), C.byref(res.raw)))
         return res
 
@@ -326,6 +335,7 @@ class Engine:
 
     def forward_device(self, n, d_coords, d_pix, pix_shared=0, d_gt=None, frame0=0, stream=None):
         """dsac_forward_device with raw device pointers (ints)."""
+        self.passes += 1
         self._check(self.lib.dsac_forward_device(self.h, n, frame0, C.c_void_p(d_coords), C.c_void_p(d_pix), pix_shared,
                                                  C.c_void_p(d_gt) if d_gt else None, C.c_void_p(stream) if stream else None))
 
@@ -333,6 +343,16 @@ class Engine:
         res = out if out is not None else ForwardResult(n, self.cfg.n_hyps, want_diffmaps)
         self._check(self.lib.dsac_fetch(self.h, n, C.byref(res.raw), C.c_void_p(stream) if stream else None))
         return res
+
+    def fetch_device(self, n, stream=None, **ptrs):
+        """dsac_fetch into the given device pointers (ints; fields of dsac_forward_out except n_candidates); synchronises
+        `stream`."""
+        raw = ForwardOut()
+        for k, v in ptrs.items():
+            if k not in _OUT_FIELDS or k == "n_candidates":
+                raise KeyError(k)
+            setattr(raw, k, v)
+        self._check(self.lib.dsac_fetch(self.h, n, C.byref(raw), C.c_void_p(stream) if stream else None))
 
     def device_view(self):
         v = DeviceView()
@@ -374,6 +394,7 @@ class Engine:
         shared = 1 if pix.size == N * 2 else 0
         gt = np.ascontiguousarray(gt_jp, np.float64).reshape(n, 12) if gt_jp is not None else None
         res = DsacResult(n, self.cfg.n_hyps, want_inlier_maps)
+        self.passes += 1
         self._check(self.lib.dsac_forward_dsac(self.h, n, frame0, _p(coords), _p(pix), shared, _p(gt), int(random_draw),
                                                C.byref(res.raw)))
         return res
@@ -393,6 +414,36 @@ class Engine:
         res = BackwardDsacResult(n, self.cfg.n_hyps)
         self._check(self.lib.dsac_backward_dsac(self.h, n, C.byref(res.raw)))
         return res
+
+    def backward_device(self, n, d_loss_grad=None, d_dloss_dobj=None, d_dloss_dpred=None, clamp=0.0, stream=None):
+        """dsac_backward_device (raw device pointers as ints): soft-argmax backward of the preceding forward pass."""
+        self._check(self.lib.dsac_backward_device(self.h, n, C.c_void_p(d_loss_grad) if d_loss_grad else None,
+                                                  C.c_void_p(d_dloss_dobj) if d_dloss_dobj else None,
+                                                  C.c_void_p(d_dloss_dpred) if d_dloss_dpred else None, C.c_float(clamp),
+                                                  C.c_void_p(stream) if stream else None))
+
+    def forward_dsac_device(self, n, d_coords, d_pix, pix_shared=0, d_gt=None, random_draw=True, frame0=0, stream=None, **ptrs):
+        """dsac_forward_dsac_device (raw device pointers as ints); ptrs: device destinations of dsac_dsac_out fields."""
+        raw = DsacOut()
+        for k, v in ptrs.items():
+            if k not in _DSAC_FIELDS:
+                raise KeyError(k)
+            setattr(raw, k, v)
+        self.passes += 1
+        self._check(self.lib.dsac_forward_dsac_device(self.h, n, frame0, C.c_void_p(d_coords), C.c_void_p(d_pix), pix_shared,
+                                                      C.c_void_p(d_gt) if d_gt else None, int(random_draw), C.byref(raw),
+                                                      C.c_void_p(stream) if stream else None))
+
+    def backward_dsac_device(self, n, d_loss_grad=None, d_dloss_dpred=None, clamp=0.0, stream=None, **ptrs):
+        """dsac_backward_dsac_device (raw device pointers as ints); ptrs: device destinations of dsac_backward_dsac_out fields."""
+        raw = BackwardDsacOut()
+        for k, v in ptrs.items():
+            if k not in _BWD_FIELDS:
+                raise KeyError(k)
+            setattr(raw, k, v)
+        self._check(self.lib.dsac_backward_dsac_device(self.h, n, C.c_void_p(d_loss_grad) if d_loss_grad else None, C.byref(raw),
+                                                       C.c_void_p(d_dloss_dpred) if d_dloss_dpred else None, C.c_float(clamp),
+                                                       C.c_void_p(stream) if stream else None))
 
     def gather_patches_device(self, n, d_frames, width, height, d_pix, pix_shared, d_patches, mean=127.0, d_status=None, stream=None):
         """dsac_gather_patches_device (raw device pointers as ints): BGR frames -> normalised 3x42x42 CNN patches."""

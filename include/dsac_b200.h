@@ -139,6 +139,8 @@ int dsac_forward_wait(dsac_engine* e);
  * (dsac_fetch copies them out).  stream: a cudaStream_t cast to void* (NULL = default). */
 int dsac_forward_device(dsac_engine* e, int32_t n_frames, int64_t frame0, const int16_t* d_coords,
                         const int32_t* d_pix, int32_t pix_shared, const double* d_gt_jp, void* stream);
+/* dsac_fetch copies with cudaMemcpyDefault on `stream` and synchronises it: every destination may be host or device
+ * memory, except n_candidates, which is summed on the host and must be host memory. */
 int dsac_fetch(dsac_engine* e, int32_t n_frames, dsac_forward_out* out, void* stream);
 int dsac_device_view_get(dsac_engine* e, dsac_device_view* view);
 
@@ -206,6 +208,19 @@ typedef struct dsac_backward_out {
 int dsac_backward(dsac_engine* e, int32_t n_frames, const int16_t* coords, const int32_t* pix, int32_t pix_shared,
                   const double* gt_jp, dsac_backward_out* out);
 
+/* Soft-argmax backward of the preceding dsac_forward / dsac_forward_device / dsac_forward_submit pass over the same
+ * n_frames, on the caller's `stream` (a cudaStream_t; ordered after that pass by an event), with the inputs that pass
+ * read (they must still be valid).  All pointers are DEVICE pointers; nothing is synchronised.
+ *   d_loss_grad   [n] dOuter/dLoss_f, the gradient arriving at the per-frame losses; NULL = 1
+ *   d_dloss_dobj  [n][N][3] dLoss/dObj, exactly what dsac_backward returns; NULL = not written
+ *   d_dloss_dpred [n][N][3] the coordinate CNN's gradient as lua/train_obj_softam.lua:101-105 hands it to model:backward:
+ *                 float(d_loss_grad[f] * clamp(dLoss/dObj, +-clamp)), clamp before the scale, row y*40+x; NULL = not
+ *                 written.  clamp <= 0: no clamp.  Like the reference it is per millimetre of the int16 grid (the network
+ *                 predicts metres) and passes straight through the rounding and saturation of
+ *                 dsac_coords_from_prediction_device (DESIGN.md quirk Q12). */
+int dsac_backward_device(dsac_engine* e, int32_t n_frames, const double* d_loss_grad, double* d_dloss_dobj,
+                         float* d_dloss_dpred, float clamp, void* stream);
+
 /* Forward of the DSAC / RANSAC variant (SURVEY.md section 8f row N1): processImage of core/cnn.h:1028-1257 -- same sampling and
  * scoring, then draw() of the winning hypothesis (cnn.h:102-126), refinement of ALL hypotheses, per-hypothesis
  * losses and the expectation of the loss (cnn.h:137-151).  random_draw != 0 draws with the stream-0 generator
@@ -228,6 +243,11 @@ typedef struct dsac_dsac_out {
 } dsac_dsac_out;
 int dsac_forward_dsac(dsac_engine* e, int32_t n_frames, int64_t frame0, const int16_t* coords, const int32_t* pix,
                       int32_t pix_shared, const double* gt_jp, int32_t random_draw, dsac_dsac_out* out);
+/* The same forward on device-resident inputs, on the caller's `stream`: every non-NULL field of d_out is a DEVICE pointer,
+ * nothing is copied to the host or synchronised.  The inputs must stay valid until dsac_backward_dsac_device. */
+int dsac_forward_dsac_device(dsac_engine* e, int32_t n_frames, int64_t frame0, const int16_t* d_coords, const int32_t* d_pix,
+                             int32_t pix_shared, const double* d_gt_jp, int32_t random_draw, const dsac_dsac_out* d_out,
+                             void* stream);
 
 /* Backward of the DSAC / RANSAC variant (replaces the gradient block of train_ransac.cpp:304-381; must follow a
  * dsac_forward_dsac over the same n_frames with ground truth):
@@ -246,6 +266,13 @@ typedef struct dsac_backward_dsac_out {
     int32_t* n_refine_jobs;   /* [n]        refine() evaluations of path I, nullable */
 } dsac_backward_dsac_out;
 int dsac_backward_dsac(dsac_engine* e, int32_t n_frames, dsac_backward_dsac_out* out);
+/* The same backward after a dsac_forward_dsac(_device), on the caller's `stream` (ordered after that forward by an event):
+ * every non-NULL field of d_out (NULL: none) is a DEVICE pointer.  d_loss_grad, d_dloss_dpred and clamp as in
+ * dsac_backward_device, with dLoss/dObj = path I + path II.  The call reads back one pair of totals -- selected
+ * hypotheses and refinement jobs, which size the finite-difference k_refine launch -- and so synchronises `stream` once
+ * in the middle; no per-hypothesis or per-cell array crosses to the host. */
+int dsac_backward_dsac_device(dsac_engine* e, int32_t n_frames, const double* d_loss_grad, const dsac_backward_dsac_out* d_out,
+                              float* d_dloss_dpred, float clamp, void* stream);
 
 /* Upstream step on the device (SURVEY.md section 8f row N3), so that frames never leave HBM between the image and the
  * hypothesis engine.  All pointers are DEVICE pointers; `stream` is a cudaStream_t (NULL: default stream).
