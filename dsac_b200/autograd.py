@@ -1,13 +1,22 @@
-"""The engine's losses as differentiable PyTorch functions, for training the coordinate CNN end to end.
+"""The engine's losses and refined poses as differentiable PyTorch functions, for training the coordinate CNN end to end.
 
     loss = softam_loss(engine, prediction, pix, gt_jp)              # soft-argmax pipeline, [n]
     loss = dsac_expected_loss(engine, prediction, pix, gt_jp)       # DSAC / RANSAC variant, [n]
     loss.sum().backward()                                           # prediction.grad
 
+    pose = softam_pose(engine, prediction, pix)                     # refined jp 6-vector per frame, [n][6]
+    sf, ref = dsac_hypotheses(engine, prediction, pix)              # softmax [n][H], refined jp 6-vectors [n][H][6]
+    my_loss(pose).backward()                                        # prediction.grad, no ground truth needed
+
 `prediction` is the coordinate CNN's output: float32 [n][1600][3] scene coordinates in metres on the engine's device,
 cell y*40+x.  It is the only input that receives a gradient.  The gradient is the one the reference hands to
 model:backward (lua/train_obj_softam.lua:101-105): dLoss/dObj clamped to +-clamp, scaled by the incoming gradient, per
 millimetre of the int16 grid, straight through the rounding to millimetres (DESIGN.md quirk Q12).
+
+The pose outputs are jp 6-vectors [rodrigues(R); t in mm], the vector the reference's refine() and dLossMax work on.
+Their backward is the reference's chain with the incoming gradient in place of dLossMax (INTEGRATION.md, "Pose-valued
+outputs"): it inherits the reference's finite differences and quirks, and the clamp applies to the total dLoss/dObj,
+since the incoming gradient is already inside it.
 
 Everything stays on the device, on torch.cuda.current_stream().  The engine holds one pass: a forward on the same engine
 between a loss and its backward() makes that backward() raise.
@@ -17,9 +26,9 @@ import torch
 from . import engine as _E
 
 
-def _check_inputs(engine, prediction, pix, gt_jp):
+def _check_inputs(engine, prediction, pix, gt_jp, need_gt=True):
     dev = torch.device("cuda", engine.cfg.device)
-    if gt_jp is None:
+    if gt_jp is None and need_gt:
         raise ValueError("the loss needs the ground-truth poses gt_jp [n][12]")
     n = prediction.shape[0] if prediction.dim() == 3 else -1
     if prediction.dtype != torch.float32 or tuple(prediction.shape[1:]) != (_E.N, 3) or prediction.dim() != 3:
@@ -27,13 +36,13 @@ def _check_inputs(engine, prediction, pix, gt_jp):
     if not 1 <= n <= engine.cfg.max_frames:
         raise ValueError("%d frames, the engine holds 1..%d" % (n, engine.cfg.max_frames))
     for name, t in (("prediction", prediction), ("pix", pix), ("gt_jp", gt_jp)):
-        if t.device != dev:
+        if t is not None and t.device != dev:
             raise ValueError("%s is on %s, the engine on %s" % (name, t.device, dev))
     if pix.dtype != torch.int32 or pix.numel() not in (_E.N * 2, n * _E.N * 2):
         raise ValueError("pix must be int32 [N][2] (shared) or [n][N][2]")
-    if gt_jp.dtype != torch.float64 or gt_jp.numel() != n * 12:
+    if gt_jp is not None and (gt_jp.dtype != torch.float64 or gt_jp.numel() != n * 12):
         raise ValueError("gt_jp must be float64 [n][12]")
-    return n, pix.contiguous(), gt_jp.contiguous(), (1 if pix.numel() == _E.N * 2 else 0)
+    return n, pix.contiguous(), gt_jp.contiguous() if gt_jp is not None else None, (1 if pix.numel() == _E.N * 2 else 0)
 
 
 def _coords(engine, prediction, stream):
@@ -92,6 +101,57 @@ class _DsacExpectedLoss(torch.autograd.Function):
         return grad, None, None, None, None, None, None
 
 
+class _SoftamPose(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, prediction, engine, pix, frame0, clamp):
+        n, pix, _, shared = _check_inputs(engine, prediction, pix, None, need_gt=False)
+        stream = torch.cuda.current_stream(prediction.device).cuda_stream
+        coords = _coords(engine, prediction.detach().contiguous(), stream)
+        engine.forward_device(n, coords.data_ptr(), pix.data_ptr(), shared, None, frame0, stream)
+        pose = torch.empty((n, 6), dtype=torch.float64, device=prediction.device)
+        engine.refined_jp6_device(n, pose.data_ptr(), stream)
+        ctx.engine, ctx.pass_id, ctx.n, ctx.clamp = engine, engine.passes, n, clamp
+        ctx.keep = (coords, pix)
+        return pose
+
+    @staticmethod
+    def backward(ctx, grad_pose):
+        seed, grad = _grad_input(ctx, grad_pose)
+        ctx.engine.backward_pose_device(ctx.n, seed.data_ptr(), None, grad.data_ptr(), ctx.clamp,
+                                        torch.cuda.current_stream(seed.device).cuda_stream)
+        return grad, None, None, None, None
+
+
+class _DsacHypotheses(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, prediction, engine, pix, frame0, random_draw, clamp):
+        n, pix, _, shared = _check_inputs(engine, prediction, pix, None, need_gt=False)
+        stream = torch.cuda.current_stream(prediction.device).cuda_stream
+        coords = _coords(engine, prediction.detach().contiguous(), stream)
+        H = engine.cfg.n_hyps
+        sf = torch.empty((n, H), dtype=torch.float64, device=prediction.device)
+        engine.forward_dsac_device(n, coords.data_ptr(), pix.data_ptr(), shared, None, random_draw, frame0, stream,
+                                   sf=sf.data_ptr())
+        ref = torch.empty((n, H, 6), dtype=torch.float64, device=prediction.device)
+        engine.refined_jp6_device(n, ref.data_ptr(), stream)
+        ctx.engine, ctx.pass_id, ctx.n, ctx.clamp = engine, engine.passes, n, clamp
+        ctx.keep = (coords, pix)
+        ctx.set_materialize_grads(False)   # an unused output skips its path of the backward
+        return sf, ref
+
+    @staticmethod
+    def backward(ctx, grad_sf, grad_ref):
+        seeds = [g for g in (grad_sf, grad_ref) if g is not None]
+        if not seeds:
+            return None, None, None, None, None, None
+        _, grad = _grad_input(ctx, seeds[0])
+        ptr = [g.detach().to(torch.float64).contiguous() if g is not None else None for g in (grad_sf, grad_ref)]
+        ctx.engine.backward_dsac_pose_device(ctx.n, ptr[1].data_ptr() if ptr[1] is not None else None,
+                                             ptr[0].data_ptr() if ptr[0] is not None else None, grad.data_ptr(), ctx.clamp,
+                                             torch.cuda.current_stream(grad.device).cuda_stream)
+        return grad, None, None, None, None, None
+
+
 def softam_loss(engine, prediction, pix, gt_jp, frame0=0, clamp=0.1):
     """Per-frame loss of the soft-argmax pipeline (train_ransac_softam.cpp) on `prediction`, float64 [n]; differentiable
     with respect to `prediction`.  frame0: global index of the first frame (keys the sampler streams)."""
@@ -102,3 +162,16 @@ def dsac_expected_loss(engine, prediction, pix, gt_jp, frame0=0, random_draw=Tru
     """Per-frame expected loss of the DSAC / RANSAC variant (train_ransac.cpp) on `prediction`, float64 [n];
     differentiable with respect to `prediction`."""
     return _DsacExpectedLoss.apply(prediction, engine, pix, gt_jp, int(frame0), bool(random_draw), float(clamp))
+
+
+def softam_pose(engine, prediction, pix, frame0=0, clamp=0.1):
+    """Refined pose of every frame of the soft-argmax pipeline as a jp 6-vector [rodrigues(R); t in mm], float64 [n][6];
+    differentiable with respect to `prediction`.  Needs no ground truth."""
+    return _SoftamPose.apply(prediction, engine, pix, int(frame0), float(clamp))
+
+
+def dsac_hypotheses(engine, prediction, pix, frame0=0, random_draw=True, clamp=0.1):
+    """(sf [n][H], refined jp 6-vectors [n][H][6]) of the DSAC / RANSAC variant, both float64 and differentiable with
+    respect to `prediction`.  The gradient through the poses covers the hypotheses with sf > 1e-4 whose incoming
+    gradient is nonzero; an output that receives no gradient costs nothing in the backward."""
+    return _DsacHypotheses.apply(prediction, engine, pix, int(frame0), bool(random_draw), float(clamp))

@@ -59,6 +59,16 @@ __device__ __forceinline__ void jp6_from_cv_dev(const double pose[6], double out
     out[3] = t[0]; out[4] = t[1]; out[5] = t[2];
 }
 
+// jp 6-vectors of `count` refined cv poses (dsac_refined_jp6_device): the vector refine(), dLossMax and the
+// finite-difference jobs (job_jp6) work on, so the seed of a pose backward is the gradient with respect to it
+__global__ void k_pose_jp6(const double* __restrict__ pose, size_t count, double* __restrict__ jp6) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    double o[6];
+    jp6_from_cv_dev(pose + i * 6, o);
+    for (int k = 0; k < 6; k++) jp6[i * 6 + k] = o[k];
+}
+
 // dLossMax, maxloss.h:87-198
 __device__ void dloss_max_dev(const double est[6], const double gt[6], double jac[6]) {
     for (int i = 0; i < 6; i++) jac[i] = 0;
@@ -116,6 +126,7 @@ struct BwParams {
     const int32_t* pix;
     int pix_stride;
     const double* gt_jp;        // [n][12]
+    const double* seed;         // [n][6] dOuter/d(refined jp6) in place of dLossMax against gt_jp; null: dLossMax
     double f, cx, cy;
     int H, thr, skip, fix_q4;
     double alpha, beta, grad_clamp;
@@ -150,6 +161,7 @@ struct DsacBwParams {
     const double* ref_pose;     // [n*H][6] refined cv pose of every hypothesis (forward_dsac)
     const double* sf;           // [n*H]
     const double* gt_jp;        // [n][12]
+    const double* seed;         // [n*H][6] dOuter/d(refined jp6) in place of sf_h dLossMax_h; null: sf_h dLossMax_h
     // jobs
     int n_jobs;
     const int32_t* job_frame;   // [n_jobs]
@@ -200,7 +212,8 @@ __global__ void k_dsac_job_p3p(DsacBwParams p) {
 // central-difference pairs of a frame, in pair order (pairs are sorted by hypothesis; a hypothesis touches a column at
 // most once, so within one hypothesis' run the additions are independent, and the runs are applied one after the other).
 // One warp per frame: first the lanes evaluate dLossMax of the frame's selected hypotheses in parallel, then the runs
-// are walked in order with the lanes spread over a run's pairs.
+// are walked in order with the lanes spread over a run's pairs.  A seeded backward takes seed_h with weight 1 in place
+// of dLossMax_h with weight sf_h, and reads no ground truth.
 constexpr int DSAC_COMBINE_MAX_HYPS = 1024;   // = DSAC_MAX_HYPS
 __global__ void __launch_bounds__(32) k_dsac_combine(DsacBwParams p) {
     __shared__ int s_run_begin[DSAC_COMBINE_MAX_HYPS + 1];
@@ -225,18 +238,25 @@ __global__ void __launch_bounds__(32) k_dsac_combine(DsacBwParams p) {
     if (lane == 0) s_run_begin[n_runs] = q_end;
     __syncwarp();
     // dLossMax of every run's hypothesis
-    const double* g = p.gt_jp + (size_t)frame * 12;
     double gt6[6];
-    rodrigues_m2v(g, gt6);
-    gt6[3] = g[9]; gt6[4] = g[10]; gt6[5] = g[11];
+    if (!p.seed) {
+        const double* g = p.gt_jp + (size_t)frame * 12;
+        rodrigues_m2v(g, gt6);
+        gt6[3] = g[9]; gt6[4] = g[10]; gt6[5] = g[11];
+    }
     for (int r0 = 0; r0 < n_runs; r0 += 32) {
         if (r0 + lane < n_runs) {
             const int hyp = p.pair_hyp[s_run_begin[r0 + lane]];
-            double ref6[6], dl[6];
-            jp6_from_cv_dev(p.ref_pose + (size_t)hyp * 6, ref6);
-            dloss_max_dev(ref6, gt6, dl);
-            for (int k = 0; k < 6; k++) s_dl[lane][k] = dl[k];
-            s_dl[lane][6] = p.sf[hyp];
+            if (p.seed) {
+                for (int k = 0; k < 6; k++) s_dl[lane][k] = p.seed[(size_t)hyp * 6 + k];
+                s_dl[lane][6] = 1.0;
+            } else {
+                double ref6[6], dl[6];
+                jp6_from_cv_dev(p.ref_pose + (size_t)hyp * 6, ref6);
+                dloss_max_dev(ref6, gt6, dl);
+                for (int k = 0; k < 6; k++) s_dl[lane][k] = dl[k];
+                s_dl[lane][6] = p.sf[hyp];
+            }
         }
         __syncwarp();
         for (int r = r0; r < min(n_runs, r0 + 32); r++) {
@@ -255,18 +275,22 @@ __global__ void __launch_bounds__(32) k_dsac_combine(DsacBwParams p) {
 }
 
 
-// ---- per frame: dLossMax and the refine job list (one warp, lane 0 does the serial scan)
+// ---- per frame: dLossMax (or the caller's seed) and the refine job list (one warp, lane 0 does the serial scan)
 __global__ void k_bw_prep(BwParams p, int n) {
     const int frame = blockIdx.x * blockDim.x + threadIdx.x;
     if (frame >= n) return;
     // dLoss/dRefinedPose
-    double ref6[6], gt6[6], dl[6];
-    jp6_from_cv_dev(p.ref_pose + (size_t)frame * 6, ref6);
-    const double* g = p.gt_jp + (size_t)frame * 12;
-    rodrigues_m2v(g, gt6);  // poseGT.getRodVecAndTrans()
-    gt6[3] = g[9]; gt6[4] = g[10]; gt6[5] = g[11];
-    dloss_max_dev(ref6, gt6, dl);
-    for (int k = 0; k < 6; k++) p.s.dl[(size_t)frame * 6 + k] = dl[k];
+    if (p.seed) {
+        for (int k = 0; k < 6; k++) p.s.dl[(size_t)frame * 6 + k] = p.seed[(size_t)frame * 6 + k];
+    } else {
+        double ref6[6], gt6[6], dl[6];
+        jp6_from_cv_dev(p.ref_pose + (size_t)frame * 6, ref6);
+        const double* g = p.gt_jp + (size_t)frame * 12;
+        rodrigues_m2v(g, gt6);  // poseGT.getRodVecAndTrans()
+        gt6[3] = g[9]; gt6[4] = g[10]; gt6[5] = g[11];
+        dloss_max_dev(ref6, gt6, dl);
+        for (int k = 0; k < 6; k++) p.s.dl[(size_t)frame * 6 + k] = dl[k];
+    }
     // jobs 0..11: dRefineHyp (cnn_softam.h:756-833): +-eps on the cv rvec (eps = 0.001f) / cv tvec (eps*1000)
     int32_t* jf = p.s.job_frame + (size_t)frame * BW_JOBS;
     double* ji = p.s.job_init + (size_t)frame * BW_JOBS * 6;
@@ -732,9 +756,13 @@ __global__ void k_kabsch(int n, int m, const double* __restrict__ a, const doubl
 
 int backward_run(dsac_engine* e, int32_t n, const int16_t* coords, const int32_t* pix, int32_t pix_shared,
                  const double* gt_jp, dsac_backward_out* out);
+// d_seed: [n][6] dOuter/d(refined jp6) in place of dLossMax (the ground truth is then not needed); null: dLossMax
 int backward_device_run(dsac_engine* e, int32_t n, const double* d_loss_grad, double* d_dloss_dobj, float* d_dloss_dpred,
-                        float clamp, cudaStream_t stream);
+                        float clamp, cudaStream_t stream, const double* d_seed = nullptr);
 int kabsch_run(dsac_engine* e, int32_t n, int32_t m, const double* a, const double* b, double* R, double* t);
 struct dsac_backward_dsac_out;
+// seeded: path I from d_seed [n][H][6] in place of sf_h dLossMax_h, path II from d_grad_sf [n][H] in place of the
+// losses; a null seed skips its path, and the ground truth is not needed
 int backward_dsac_run(dsac_engine* e, int32_t n, const double* d_loss_grad, const dsac_backward_dsac_out* out, bool out_on_host,
-                      float* d_dloss_dpred, float clamp, cudaStream_t stream);
+                      float* d_dloss_dpred, float clamp, cudaStream_t stream, bool seeded = false,
+                      const double* d_seed = nullptr, const double* d_grad_sf = nullptr);

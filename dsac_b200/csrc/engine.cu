@@ -1313,6 +1313,45 @@ int dsac_backward_dsac_device(dsac_engine* e, int32_t n, const double* d_loss_gr
     return backward_dsac_run(e, n, d_loss_grad, d_out ? d_out : &none, false, d_dloss_dpred, clamp, (cudaStream_t)stream);
 }
 
+int dsac_refined_jp6_device(dsac_engine* e, int32_t n, double* d_jp6, void* stream_v) {
+    if (!e) return DSAC_ERR_ARG;
+    if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_refined_jp6_device: a submitted pass has not been awaited (dsac_forward_wait)");
+    if (!d_jp6) return fail(e, DSAC_ERR_ARG, "dsac_refined_jp6_device: null output");
+    const double* pose;
+    size_t count;
+    if (n >= 1 && e->cur_n == n && e->cur_coords) {   // soft-argmax pass: one refined pose per frame
+        pose = e->d_ref; count = (size_t)n;
+    } else if (n >= 1 && e->dsac_n == n) {            // DSAC-variant pass: every hypothesis refined
+        pose = e->d_ra_pose; count = (size_t)n * e->cfg.n_hyps;
+    } else {
+        return fail(e, DSAC_ERR_ARG, "dsac_refined_jp6_device must follow a forward pass over the same %d frames", n);
+    }
+    CU(cudaSetDevice(e->cfg.device));
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    CU(cudaStreamWaitEvent(stream, e->ev_fwd, 0));
+    k_pose_jp6<<<(unsigned)((count + 127) / 128), 128, 0, stream>>>(pose, count, d_jp6);
+    e->launches++;
+    CU(cudaGetLastError());
+    return DSAC_OK;
+}
+
+int dsac_backward_pose_device(dsac_engine* e, int32_t n, const double* d_grad_ref, double* d_dloss_dobj, float* d_dloss_dpred,
+                              float clamp, void* stream) {
+    if (!e) return DSAC_ERR_ARG;
+    if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_backward_pose_device: a submitted pass has not been awaited (dsac_forward_wait)");
+    if (!d_grad_ref) return fail(e, DSAC_ERR_ARG, "dsac_backward_pose_device: null d_grad_ref");
+    return backward_device_run(e, n, nullptr, d_dloss_dobj, d_dloss_dpred, clamp, (cudaStream_t)stream, d_grad_ref);
+}
+
+int dsac_backward_dsac_pose_device(dsac_engine* e, int32_t n, const double* d_grad_ref, const double* d_grad_sf,
+                                   const dsac_backward_dsac_out* d_out, float* d_dloss_dpred, float clamp, void* stream) {
+    if (!e) return DSAC_ERR_ARG;
+    if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_backward_dsac_pose_device: a submitted pass has not been awaited (dsac_forward_wait)");
+    const dsac_backward_dsac_out none = {};
+    return backward_dsac_run(e, n, nullptr, d_out ? d_out : &none, false, d_dloss_dpred, clamp, (cudaStream_t)stream, true,
+                             d_grad_ref, d_grad_sf);
+}
+
 int dsac_gather_patches_device(dsac_engine* e, int32_t n, const uint8_t* d_frames, int32_t width, int32_t height,
                                const int32_t* d_pix, int32_t pix_shared, float mean, float* d_patches, uint32_t* d_status,
                                void* stream_v) {

@@ -145,6 +145,8 @@ struct SelectParams {
     const double* sf;            // [n][H]
     const int32_t* img_idx;      // [n][H][4]
     const double* hyp_pose;      // [n][H][6]
+    int seeded;                  // a seeded backward: select only hypotheses whose seed is not all zero (none: null seed)
+    const double* seed;          // [n][H][6]
     // selection (k_dsac_select): selected hypotheses in (frame, h) order
     int32_t* sel;                // [n H] global hypothesis index
     int32_t* sel_frame;          // [n H] frame, -1 behind the last selected (unused k_refine job slots)
@@ -169,7 +171,8 @@ struct SelectParams {
     int32_t* pair_scale;         // [pairs]
 };
 
-// The hypotheses with sf > 1e-4 and a minimal set (train_ransac.cpp:320), stably compacted; one CTA walks the frames.
+// The hypotheses with sf > 1e-4 and a minimal set (train_ransac.cpp:320), and in a seeded backward a nonzero seed (a zero
+// seed contributes nothing to path I), stably compacted; one CTA walks the frames.
 constexpr int SELECT_THREADS = 1024;   // = DSAC_MAX_HYPS: one pass per frame
 __global__ void __launch_bounds__(SELECT_THREADS) k_dsac_select(SelectParams p) {
     __shared__ int s_warp[33];
@@ -177,7 +180,13 @@ __global__ void __launch_bounds__(SELECT_THREADS) k_dsac_select(SelectParams p) 
     int base = 0;
     for (int f = 0; f < p.n; f++) {
         const size_t g = (size_t)f * p.H + tid;
-        const bool take = tid < p.H && p.sf[g] > SELECT_MIN_SF && p.img_idx[g * 4] >= 0;
+        bool take = tid < p.H && p.sf[g] > SELECT_MIN_SF && p.img_idx[g * 4] >= 0;
+        if (take && p.seeded) {
+            bool nz = false;
+            if (p.seed)
+                for (int k = 0; k < 6; k++) nz |= p.seed[g * 6 + k] != 0.0;
+            take = nz;
+        }
         int count;
         const int r = block_exclusive_sum(take ? 1 : 0, s_warp, &count);
         if (take) {

@@ -21,7 +21,8 @@ EXPORTS = [
     "dsac_default_config", "dsac_engine_create", "dsac_engine_destroy", "dsac_last_error", "dsac_engine_config",
     "dsac_forward", "dsac_forward_submit", "dsac_forward_wait", "dsac_forward_device", "dsac_fetch", "dsac_device_view_get", "dsac_set_stages",
     "dsac_set_tail_split", "dsac_launch_count", "dsac_sampler_profile", "dsac_sampler_profile_read", "dsac_debug_spec_result", "dsac_set_score_hook", "dsac_set_score_backward_hook", "dsac_backward", "dsac_backward_device", "dsac_forward_dsac", "dsac_forward_dsac_device",
-    "dsac_backward_dsac", "dsac_backward_dsac_device", "dsac_gather_patches_device", "dsac_coords_from_prediction_device", "dsac_kabsch",
+    "dsac_backward_dsac", "dsac_backward_dsac_device", "dsac_refined_jp6_device", "dsac_backward_pose_device",
+    "dsac_backward_dsac_pose_device", "dsac_gather_patches_device", "dsac_coords_from_prediction_device", "dsac_kabsch",
     "dsac_stochastic_subsample",
     "dsac_synth_frames", "dsac_version",
 ]
@@ -123,6 +124,10 @@ def load(build_if_missing=True):
                                              C.c_int32, C.POINTER(DsacOut), C.c_void_p]
     lib.dsac_backward_dsac_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(BackwardDsacOut), C.c_void_p, C.c_float,
                                               C.c_void_p]
+    lib.dsac_refined_jp6_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.dsac_backward_pose_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]
+    lib.dsac_backward_dsac_pose_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(BackwardDsacOut),
+                                                   C.c_void_p, C.c_float, C.c_void_p]
     lib.dsac_gather_patches_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
                                                C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.dsac_coords_from_prediction_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -444,6 +449,31 @@ class Engine:
         self._check(self.lib.dsac_backward_dsac_device(self.h, n, C.c_void_p(d_loss_grad) if d_loss_grad else None, C.byref(raw),
                                                        C.c_void_p(d_dloss_dpred) if d_dloss_dpred else None, C.c_float(clamp),
                                                        C.c_void_p(stream) if stream else None))
+
+    def refined_jp6_device(self, n, d_jp6, stream=None):
+        """dsac_refined_jp6_device (raw device pointers as ints): jp 6-vectors of the preceding pass's refined poses,
+        [n][6] after a soft-argmax forward, [n][H][6] after a DSAC-variant forward."""
+        self._check(self.lib.dsac_refined_jp6_device(self.h, n, C.c_void_p(d_jp6), C.c_void_p(stream) if stream else None))
+
+    def backward_pose_device(self, n, d_grad_ref, d_dloss_dobj=None, d_dloss_dpred=None, clamp=0.0, stream=None):
+        """dsac_backward_pose_device (raw device pointers as ints): soft-argmax backward seeded by dOuter/d(refined jp6)."""
+        self._check(self.lib.dsac_backward_pose_device(self.h, n, C.c_void_p(d_grad_ref),
+                                                       C.c_void_p(d_dloss_dobj) if d_dloss_dobj else None,
+                                                       C.c_void_p(d_dloss_dpred) if d_dloss_dpred else None, C.c_float(clamp),
+                                                       C.c_void_p(stream) if stream else None))
+
+    def backward_dsac_pose_device(self, n, d_grad_ref=None, d_grad_sf=None, d_dloss_dpred=None, clamp=0.0, stream=None, **ptrs):
+        """dsac_backward_dsac_pose_device (raw device pointers as ints): DSAC-variant backward seeded by dOuter/d(refined
+        jp6) [n][H][6] and dOuter/dsf [n][H], either None; ptrs: device destinations of dsac_backward_dsac_out fields."""
+        raw = BackwardDsacOut()
+        for k, v in ptrs.items():
+            if k not in _BWD_FIELDS:
+                raise KeyError(k)
+            setattr(raw, k, v)
+        self._check(self.lib.dsac_backward_dsac_pose_device(self.h, n, C.c_void_p(d_grad_ref) if d_grad_ref else None,
+                                                            C.c_void_p(d_grad_sf) if d_grad_sf else None, C.byref(raw),
+                                                            C.c_void_p(d_dloss_dpred) if d_dloss_dpred else None,
+                                                            C.c_float(clamp), C.c_void_p(stream) if stream else None))
 
     def gather_patches_device(self, n, d_frames, width, height, d_pix, pix_shared, d_patches, mean=127.0, d_status=None, stream=None):
         """dsac_gather_patches_device (raw device pointers as ints): BGR frames -> normalised 3x42x42 CNN patches."""

@@ -274,6 +274,26 @@ int dsac_backward_dsac(dsac_engine* e, int32_t n_frames, dsac_backward_dsac_out*
 int dsac_backward_dsac_device(dsac_engine* e, int32_t n_frames, const double* d_loss_grad, const dsac_backward_dsac_out* d_out,
                               float* d_dloss_dpred, float clamp, void* stream);
 
+/* Pose-valued outputs (INTEGRATION.md, "Pose-valued outputs").  All pointers are DEVICE pointers, the calls run on the
+ * caller's `stream`, ordered after the preceding forward by an event, and need no ground truth.  A pose is the jp 6-vector
+ * [rodrigues(R_jp); t_jp in mm] of Hypothesis(cv2our(pose)).getRodVecAndTrans() (Hypothesis.cpp:274-290): the vector
+ * refine() and dLossMax work on.  A seeded backward is the reference's chain with the seed in place of dLossMax (with its
+ * quirks, DESIGN.md), not a finite-difference-exact derivative of the pose.
+ *
+ * jp 6-vectors of the refined poses of the preceding pass: [n][6] after dsac_forward(_device/_submit),
+ * [n][H][6] after dsac_forward_dsac(_device). */
+int dsac_refined_jp6_device(dsac_engine* e, int32_t n_frames, double* d_jp6, void* stream);
+
+/* Soft-argmax backward seeded by d_grad_ref [n][6] = dOuter/d(refined jp6) instead of dLossMax.
+ * No ground truth needed. dloss_dobj / dloss_dpred / clamp as in dsac_backward_device; clamp applies to the total. */
+int dsac_backward_pose_device(dsac_engine* e, int32_t n_frames, const double* d_grad_ref,
+                              double* d_dloss_dobj, float* d_dloss_dpred, float clamp, void* stream);
+
+/* DSAC-variant backward seeded by d_grad_ref [n][H][6] (path I, over hypotheses with sf > 1e-4 and a nonzero seed)
+ * and d_grad_sf [n][H] (path II through the softmax Jacobian); either may be NULL. d_out as in dsac_backward_dsac_device. */
+int dsac_backward_dsac_pose_device(dsac_engine* e, int32_t n_frames, const double* d_grad_ref, const double* d_grad_sf,
+                                   const dsac_backward_dsac_out* d_out, float* d_dloss_dpred, float clamp, void* stream);
+
 /* Upstream step on the device (SURVEY.md section 8f row N3), so that frames never leave HBM between the image and the
  * hypothesis engine.  All pointers are DEVICE pointers; `stream` is a cudaStream_t (NULL: default stream).
  * dsac_gather_patches_device replaces the patch assembly of getCoordImg (cnn_softam.h:221-256) fused with forward()'s

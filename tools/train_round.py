@@ -4,7 +4,9 @@
     python tools/train_round.py [--reps 3]
 
 Workloads: the soft-argmax round (forward + backward) on 64 frames per call and the DSAC / RANSAC variant's round
-(forward_dsac + backward_dsac) on 16 frames per call, 256 hypotheses, bench.py's seeded synthetic frames.  Each record is
+(forward_dsac + backward_dsac) on 16 frames per call, 256 hypotheses, bench.py's seeded synthetic frames.  The same
+rounds through the pose-valued outputs: softam_pose with a random seed per frame, and dsac_hypotheses with the
+expected-loss form (every hypothesis seeded, as in the loss round) and with only the drawn hypothesis seeded.  Each record is
 the wall time of `reps` calls between device synchronisations, per frame.  The card's name and power limit are read in
 the same run.
 """
@@ -26,7 +28,7 @@ def main():
     args = ap.parse_args()
     import torch
     import dsac_b200.engine as E
-    from dsac_b200.autograd import dsac_expected_loss, softam_loss
+    from dsac_b200.autograd import dsac_expected_loss, dsac_hypotheses, softam_loss, softam_pose
     if not torch.cuda.is_available():
         raise SystemExit("train_round.py needs a CUDA device")
     nb3, nb5 = 64, 16
@@ -58,9 +60,14 @@ def main():
 
     def softam_autograd():
         softam_loss(eng3, pred3, d_pix, d_gt).sum().backward()
+    w3 = torch.randn((nb3, 6), dtype=torch.float64, device="cuda", generator=torch.Generator("cuda").manual_seed(0))
+
+    def softam_pose_autograd():   # a random seed on every frame's refined pose
+        (softam_pose(eng3, pred3, d_pix) * w3).sum().backward()
     out["softam_64_frames"] = {"host_entries_ms_per_frame": per_frame_ms(softam_host, nb3),
                                "device_entries_ms_per_frame": per_frame_ms(softam_device, nb3),
-                               "autograd_ms_per_frame": per_frame_ms(softam_autograd, nb3)}
+                               "autograd_ms_per_frame": per_frame_ms(softam_autograd, nb3),
+                               "softam_pose_random_seed_ms_per_frame": per_frame_ms(softam_pose_autograd, nb3)}
     eng3.close()
 
     eng5 = E.Engine(max_frames=nb5)
@@ -79,9 +86,21 @@ def main():
 
     def dsac_autograd():
         dsac_expected_loss(eng5, pred5, p5, g5).sum().backward()
+    w5 = torch.randn((nb5, eng5.cfg.n_hyps, 6), dtype=torch.float64, device="cuda", generator=torch.Generator("cuda").manual_seed(1))
+
+    def hyps_expected():   # expected-loss form: seeds sf_h w_h on every hypothesis, dL/dsf = ref_h . w_h
+        sf, ref = dsac_hypotheses(eng5, pred5, p5)
+        (sf * (ref * w5).sum(-1)).sum().backward()
+
+    def hyps_drawn():      # the drawn (arg-max) hypothesis only: one seeded hypothesis per frame, no path II
+        sf, ref = dsac_hypotheses(eng5, pred5, p5, random_draw=False)
+        pick = sf.detach().argmax(1)
+        (ref[torch.arange(nb5, device="cuda"), pick] * w5[:, 0]).sum().backward()
     out["dsac_16_frames"] = {"host_entries_ms_per_frame": per_frame_ms(dsac_host, nb5),
                              "device_entries_ms_per_frame": per_frame_ms(dsac_device, nb5),
-                             "autograd_ms_per_frame": per_frame_ms(dsac_autograd, nb5)}
+                             "autograd_ms_per_frame": per_frame_ms(dsac_autograd, nb5),
+                             "hypotheses_expected_loss_form_ms_per_frame": per_frame_ms(hyps_expected, nb5),
+                             "hypotheses_drawn_only_ms_per_frame": per_frame_ms(hyps_drawn, nb5)}
     eng5.close()
     try:
         card = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=name,power.limit",
