@@ -222,6 +222,21 @@ DSAC_HD float score_sigmoid_sum5(const float e[5], float kbeta, float tau_k) {
 }
 
 // ----------------------------------------------------------------------------- P3P
+// Products of the exact P3P solve's closed forms (cubic_first_root, quartic_roots) that are never contracted into a
+// fused multiply-add.  Those closed forms take exact sign decisions (D <= 0, R2 >= 0, D2 >= 0, E2 >= 0) that sit on a
+// near-double root for some minimal sets; nvcc's default contraction rounds such a discriminant differently from the
+// reference's (uncontracted) arithmetic and can flip it, and the sampler then drops a minimal set the reference accepts
+// (seen at f = 1500: tests/test_gpu_params.py).  __dmul_rn is never fused; on the host the product goes through a volatile,
+// which no -ffp-contract setting can fuse into the following sum (tests/test_host_params.py builds it with -mfma to check).
+DSAC_HD double p3p_mul(double a, double b) {
+#if defined(__CUDA_ARCH__)
+    return __dmul_rn(a, b);
+#else
+    volatile double r = a * b;
+    return r;
+#endif
+}
+
 // Largest real root of y^3 + a2 y^2 + a1 y + a0 (the resolvent cubic of Ferrari's method).
 #if defined(__CUDA_ARCH__)
 #define DSAC_RSQRTF_EARLY(x) rsqrtf(x)
@@ -230,13 +245,14 @@ DSAC_HD float score_sigmoid_sum5(const float e[5], float kbeta, float tau_k) {
 #endif
 
 DSAC_HD double cubic_first_root(double a2, double a1, double a0) {
-    double Q = (3 * a1 - a2 * a2) / 9;
-    double R = (9 * a2 * a1 - 27 * a0 - 2 * a2 * a2 * a2) / 54;
-    double Q3 = Q * Q * Q, D = Q3 + R * R, sh = a2 / 3;
+    const double a22 = p3p_mul(a2, a2);
+    double Q = (p3p_mul(3, a1) - a22) / 9;
+    double R = (p3p_mul(p3p_mul(9, a2), a1) - p3p_mul(27, a0) - p3p_mul(p3p_mul(2, a22), a2)) / 54;
+    double Q3 = p3p_mul(p3p_mul(Q, Q), Q), D = Q3 + p3p_mul(R, R), sh = a2 / 3;
     if (Q == 0) return (R == 0) ? -sh : cbrt(2 * R) - sh;
     if (D <= 0) {
         double theta = acos(R / sqrt(-Q3));
-        return 2 * sqrt(-Q) * cos(theta / 3.0) - sh;
+        return p3p_mul(2 * sqrt(-Q), cos(theta / 3.0)) - sh;
     }
     double AD = cbrt(fabs(R) + sqrt(D)) * (R > 0 ? 1 : (R < 0 ? -1 : 0));
     double BD = (AD == 0) ? 0 : -Q / AD;
@@ -244,40 +260,41 @@ DSAC_HD double cubic_first_root(double a2, double a1, double a0) {
 }
 
 // Real roots of the quartic (closed form; accuracy is restored afterwards by Newton steps
-// on the two-quadric system, see p3p_best).
+// on the two-quadric system, see p3p_best).  Every product that feeds a sum is p3p_mul (see above).
 DSAC_HD int quartic_roots(double a, double b, double c, double d, double e, double x[4]) {
     if (a == 0) return 0;
     double ia = 1.0 / a;
     b *= ia; c *= ia; d *= ia; e *= ia;
-    double y1 = cubic_first_root(-c, d * b - 4 * e, 4 * c * e - d * d - b * b * e);
-    double R2 = 0.25 * b * b - c + y1;
+    const double bb = p3p_mul(b, b);
+    double y1 = cubic_first_root(-c, p3p_mul(d, b) - p3p_mul(4, e), p3p_mul(p3p_mul(4, c), e) - p3p_mul(d, d) - p3p_mul(bb, e));
+    double R2 = p3p_mul(0.25, bb) - c + y1;
     if (!(R2 >= 0)) return 0;
     double R = sqrt(R2), D2, E2;
     if (R < 10e-12) {
-        double t = y1 * y1 - 4 * e;
+        double t = p3p_mul(y1, y1) - p3p_mul(4, e);
         if (t < 0) {
             D2 = E2 = -1;
         } else {
             double st = sqrt(t);
-            D2 = 0.75 * b * b - 2 * c + 2 * st;
-            E2 = D2 - 4 * st;
+            D2 = p3p_mul(p3p_mul(0.75, b), b) - p3p_mul(2, c) + p3p_mul(2, st);
+            E2 = D2 - p3p_mul(4, st);
         }
     } else {
-        double u = 0.75 * b * b - 2 * c - R2;
-        double v = 0.25 * (4 * b * c - 8 * d - b * b * b) / R;
+        double u = p3p_mul(p3p_mul(0.75, b), b) - p3p_mul(2, c) - R2;
+        double v = p3p_mul(0.25, p3p_mul(p3p_mul(4, b), c) - p3p_mul(8, d) - p3p_mul(bb, b)) / R;
         D2 = u + v;
         E2 = u - v;
     }
     int n = 0;
     if (D2 >= 0) {
         double Dq = sqrt(D2);
-        x[0] = 0.5 * R + 0.5 * Dq - 0.25 * b;
+        x[0] = p3p_mul(0.5, R) + p3p_mul(0.5, Dq) - p3p_mul(0.25, b);
         x[1] = x[0] - Dq;
         n = 2;
     }
     if (E2 >= 0) {
         double Eq = sqrt(E2);
-        x[n] = -0.5 * R + 0.5 * Eq - 0.25 * b;
+        x[n] = p3p_mul(-0.5, R) + p3p_mul(0.5, Eq) - p3p_mul(0.25, b);
         x[n + 1] = x[n] - Eq;
         n += 2;
     }

@@ -60,6 +60,14 @@ def _p(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else None
 
 
+def set_camera(focal=525.0, cx=320.0, cy=240.0):
+    """The reference's camera (GlobalProperties' focal length and principal-point shift from the 640 x 480 image centre)
+    for the soft-argmax and DSAC pipelines; the values must be exact floats.  The default is the reference's own."""
+    for name in ("libref_softam.so", "libref_dsac.so"):
+        rc = _lib(name).ref_set_camera(C.c_float(focal), C.c_float(cx - 320.0), C.c_float(cy - 240.0))
+        assert rc == 0
+
+
 class Forward:
     def __init__(self, cfg):
         H = cfg.n_hyps

@@ -50,6 +50,16 @@ void vec3(const cv::Mat& m, double* out) {
 
 extern "C" {
 
+// The camera GlobalProperties::getCamMat() builds the calibration matrix from (properties.cpp:55-57 defaults, the drivers'
+// -fl / -xs / -ys flags): principal point = image centre (320, 240) + shift.  Persists across calls; the default is 525, 0, 0.
+int ref_set_camera(float focal, float x_shift, float y_shift) {
+    GlobalProperties* gp = GlobalProperties::getInstance();
+    gp->dP.focalLength = focal;
+    gp->dP.xShift = x_shift;
+    gp->dP.yShift = y_shift;
+    return 0;
+}
+
 struct ref_config {
     double alpha, beta, grad_clamp;
     int32_t n_hyps, thr2d, inlier_count, ref_steps;
