@@ -314,7 +314,7 @@ __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS) k_sample(SamplePara
                 mu3 = mu; mv3 = mv;
             }
         }
-        return p3p_quick_core(bear, X, mu3, mv3, p.f, p.cx, p.cy, (double)p.thr);
+        return p3p_lambda_core(bear, X, mu3, mv3, p.f, p.cx, p.cy, (double)p.thr);
     };
 
     long long tA1 = 0, tA2 = 0, tB = 0, tC = 0, tD = 0, tE = 0, tmark = clock64();

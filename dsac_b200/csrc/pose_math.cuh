@@ -309,7 +309,7 @@ DSAC_HD double rsqrt_or(double x) {
 #endif
 }
 
-// Reciprocal / reciprocal square root / square root for the CONSERVATIVE FILTER only (quartic_roots_banded, p3p_quick_core):
+// Reciprocal / reciprocal square root / square root for the CONSERVATIVE FILTER only (p3p_lambda_core):
 // the hardware's 20-bit approximation refined by two Newton steps -- a few ulp, five to nine instructions instead of the
 // IEEE division / square root sequences (which were ~30 % of the filter's instructions).  The filter's decisions are
 // protected by bands >= 1e-9 relative (and 0.05 px), nine orders of magnitude above that error; zero, subnormal, infinite
@@ -348,13 +348,12 @@ DSAC_HD double filt_sqrt(double x) {   // x > 0
 #endif
 }
 
-// quartic_roots with an "uncertain" verdict: set when any sign decision of Ferrari's method lies
-// within a relative band of 1e-9 (>= 10^6 x double rounding), i.e. when another instance of the same
-// computation with different rounding could decide differently.  Used by the conservative filter.
-// The same root of the resolvent cubic as cubic_first_root (the largest one when there are three), for the
-// conservative filter only: an fp32 closed-form seed (a handful of MUFU operations instead of fp64
-// acos/cos/cbrt/sqrt, ~300 instructions) restored to fp64 accuracy by Newton steps on the cubic.  *ok is false
-// when the last step has not collapsed below 1e-9 of the problem's scale (near-double root, overflow, NaN) and
+// A real root of y^3 + a2 y^2 + a1 y + a0 (the largest one when there are three), for the conservative filter only
+// (p3p_lambda_core's cubic): an fp32 closed-form seed (a handful of MUFU operations instead of fp64 acos/cos/cbrt/sqrt,
+// ~300 instructions) restored to fp64 accuracy by three Newton steps (quadratic convergence from the seed's ~1e-6 relative
+// error).  *ok is false
+// when the last step has not collapsed below 1e-13 of the problem's scale (near-multiple root: there Newton converges only
+// linearly and the root is no better than a few steps' size; overflow, NaN) and
 // the caller must then treat the candidate as uncertain.
 DSAC_HD double cubic_first_root_seeded(double a2, double a1, double a0, bool* ok) {
     // Branch-free: the lanes of a warp hold different candidates, and a divergent branch here costs every lane the
@@ -383,38 +382,8 @@ DSAC_HD double cubic_first_root_seeded(double a2, double a1, double a0, bool* ok
         dy = g * filt_rcp(gp);
         y -= dy;
     }
-    *ok = fabs(dy) <= 1e-9 * (fabs(y) + fabs(sh));
+    *ok = fabs(dy) <= 1e-13 * (fabs(y) + fabs(sh));
     return y;
-}
-
-// Real roots of the quartic by Ferrari's method, branch-free (see above): x[0..n) are the roots, n in {0, 2, 4}.
-// *uncertain: some sign decision lies within the 1e-9 band (then n = 0 and the caller flags the candidate).
-DSAC_HD int quartic_roots_banded(double a, double b, double c, double d, double e, double x[4], bool* uncertain) {
-    const double TOL = 1e-9;
-    const double ia = filt_rcp(a);
-    b *= ia; c *= ia; d *= ia; e *= ia;
-    bool cubic_ok;
-    const double y1 = cubic_first_root_seeded(-c, d * b - 4 * e, 4 * c * e - d * d - b * b * e, &cubic_ok);
-    const double R2 = 0.25 * b * b - c + y1, mR = 0.25 * b * b + fabs(c) + fabs(y1);
-    bool unc = !cubic_ok;
-    unc |= !(fabs(R2) > TOL * mR);                    // also catches NaN and the R ~ 0 branch of the closed form
-    const bool none = (R2 < 0);                       // no real root, by a margin no rounding can bridge
-    const double R2p = fabs(R2);
-    const double R = filt_sqrt(R2p);
-    const double u = 0.75 * b * b - 2 * c - R2p;
-    const double v = 0.25 * (4 * b * c - 8 * d - b * b * b) * filt_rcp(R);
-    const double D2 = u + v, E2 = u - v, mD = fabs(0.75 * b * b) + fabs(2 * c) + R2p + fabs(v);
-    unc |= (!(fabs(D2) > TOL * mD)) | (!(fabs(E2) > TOL * mD));
-    const bool hasD = D2 > 0, hasE = E2 > 0;
-    const double Dq = filt_sqrt(fabs(D2)), Eq = filt_sqrt(fabs(E2));
-    const double xd0 = 0.5 * R + 0.5 * Dq - 0.25 * b, xd1 = xd0 - Dq;
-    const double xe0 = -0.5 * R + 0.5 * Eq - 0.25 * b, xe1 = xe0 - Eq;
-    x[0] = hasD ? xd0 : xe0;
-    x[1] = hasD ? xd1 : xe1;
-    x[2] = xe0;
-    x[3] = xe1;
-    *uncertain = unc;
-    return (unc | none) ? 0 : ((hasD ? 2 : 0) + (hasE ? 2 : 0));
 }
 
 struct P3PProblem {
@@ -775,104 +744,155 @@ static double g_filter_fp32_maxdev = 0;
 #ifndef DSAC_FILTER_FP32_BAND
 #define DSAC_FILTER_FP32_BAND 0.25     /* px: candidates whose 4th point lands within thr + 0.25 px go to the full solve (fp32 deviates <= 0.007 px) */
 #endif
-#ifndef DSAC_FILTER_UNROLL
-#define DSAC_FILTER_UNROLL 1   /* root slots evaluated per trip of the filter's root loop (register pressure vs ILP) */
-#endif
 // Core of the filter on prepared inputs: unit bearings of points 0..2, the four scene coordinates and the pixel
 // (mu3, mv3) of the 4th point as P3P sees it (k_sample keeps 1/|(u, v, 1)| per cell in shared memory).
-DSAC_HD bool p3p_quick_core(const double bear[3][3], const double X[4][3], double mu3, double mv3, double f, double cx,
-                            double cy, double thr) {
-    // BRANCH-FREE on purpose.  One thread filters one candidate, and the candidates of a warp differ in everything that a
-    // branch could test (number of real roots, sign of the roots, degeneracy): with early exits the warp ran at 16 of 32
-    // lanes (profiled with Nsight Compute).  Every test below therefore only sets a flag; all four root slots are evaluated by
-    // all lanes (slots >= nroots are masked) and the verdict is the OR of the flags.  A NaN or infinity anywhere makes
-    // the comparison it reaches fail, and every comparison is written so that failing means "needs the full solve".
-    // Flag k <-> the early exit DSAC_FLAG(k) of the sequential formulation (kept for the host statistics build).
+//
+// Lambda Twist (Persson & Nordberg, ECCV 2018), written from the published algorithm.  With a_ij = |X_i - X_j|^2 and
+// b_ij = bear_i . bear_j the depths lambda of points 0..2 solve E_ij: l_i^2 + l_j^2 - 2 b_ij l_i l_j = a_ij.
+//   a12 E01 - a01 E12 and a12 E02 - a02 E12 cancel the right-hand sides: two homogeneous conics l^T D1 l = l^T D2 l = 0
+//   (below divided by a12: A01 = a01 / a12, A02 = a02 / a12).
+//   A real root g of the cubic det(D1 + g D2) makes D0 = D1 + g D2 singular, and every solution lies on D0.  Its
+//   2 x 2 minors decide what D0 is: two real planes through its null vector (P = d01^2 - d00 d11 >= 0, Q = d02^2 - d00 d22
+//   >= 0, P Q = m^2), or a single real direction, the null vector (P, Q <= 0).
+//   Two planes: d00 l0 = (-d01 +- alpha) l1 + (-d02 +- beta) l2 with (alpha l1 + beta l2)^2 = P l1^2 + 2 m l1 l2 + Q l2^2.
+//   Each plane substituted into a second conic of the pencil (D2, or D1 where |g| > 1 makes D0 close to g D2) gives a
+//   quadratic in tau = l1 / l2; then l2 = sqrt(a12 / (tau^2 - 2 b12 tau + 1)), l1 = tau l2, l0 from the plane.
+// So one cubic, one 2 x 2 split and one quadratic per plane: no quartic and no y-from-x division.  The exact solve (Gao's
+// quartic, p3p_front / p3p_full) finds the same real solutions x = l0 / l2, y = l1 / l2 with x, y > 0.
+//
+// BRANCH-FREE on purpose.  One thread filters one candidate, and the candidates of a warp differ in everything that a
+// branch could test (number of real solutions, their signs, degeneracy): with early exits the warp ran at 16 of 32 lanes
+// (profiled with Nsight Compute).  Every test below therefore only sets a flag; root slots 0 and 1 are evaluated by all
+// lanes (slots >= nroots are masked) and the verdict is the OR of the flags.  A NaN or infinity anywhere makes the
+// comparison it reaches fail, and every comparison is written so that failing means "needs the full solve".
+// Flag k: the guard DSAC_FLAG(k) of the statistics build (tools/filter_stats.py).
+DSAC_HD bool p3p_lambda_core(const double bear[3][3], const double X[4][3], double mu3, double mv3, double f, double cx,
+                             double cy, double thr) {
     const double ax = X[1][0] - X[0][0], ay = X[1][1] - X[0][1], az = X[1][2] - X[0][2];
     const double bx = X[2][0] - X[0][0], by = X[2][1] - X[0][1], bz = X[2][2] - X[0][2];
     const double gx = X[2][0] - X[1][0], gy = X[2][1] - X[1][1], gz = X[2][2] - X[1][2];
     const double s01 = ax * ax + ay * ay + az * az, s02 = bx * bx + by * by + bz * bz, s12 = gx * gx + gy * gy + gz * gz;
     const double nx = ay * bz - az * by, ny = az * bx - ax * bz, nz = ax * by - ay * bx;
     const double nn = nx * nx + ny * ny + nz * nz;
-    bool flag = (!(s01 > 0)) | (!(nn > 0));                                              // (1) degenerate triangle
-    const double p = 2 * (bear[1][0] * bear[2][0] + bear[1][1] * bear[2][1] + bear[1][2] * bear[2][2]);
-    const double q = 2 * (bear[0][0] * bear[2][0] + bear[0][1] * bear[2][1] + bear[0][2] * bear[2][2]);
-    const double r = 2 * (bear[0][0] * bear[1][0] + bear[0][1] * bear[1][1] + bear[0][2] * bear[1][2]);
-    const double inv_c2 = filt_rcp(s01);
-    const double a = inv_c2 * s12, b = inv_c2 * s02;
-    flag |= !(fabs(p * p + q * q + r * r - p * q * r - 1) > 1e-12);                      // (2)
-    const double N2 = 1 - a - b, N1 = q * (a - 1), N0 = 1 - a + b;
-    const double D1 = b * r, D0 = -b * p;
-    double xr[4];
-    int nroots;
-    {
-        const double F2 = 1 - b, F1 = -q;
-        const double DD2 = D1 * D1, DD1 = 2 * D1 * D0, DD0 = D0 * D0, br = b * r;
-        const double c4 = F2 * DD2 - b * (N2 * N2) - br * (N2 * D1);
-        const double c3 = F2 * DD1 + F1 * DD2 - b * (2 * N2 * N1) - br * (N2 * D0 + N1 * D1);
-        const double c2 = F2 * DD0 + F1 * DD1 + DD2 - b * (2 * N2 * N0 + N1 * N1) - br * (N1 * D0 + N0 * D1);
-        const double c1 = F1 * DD0 + DD1 - b * (2 * N1 * N0) - br * (N0 * D0);
-        const double c0 = DD0 - b * (N0 * N0);
-        flag |= !(fabs(c4) > 1e-12 * (fabs(c3) + fabs(c2) + fabs(c1) + fabs(c0)));      // (3)
-        bool uncertain;
-        nroots = quartic_roots_banded(c4, c3, c2, c1, c0, xr, &uncertain);
-        flag |= uncertain;                                                               // (4)
-    }
-#if defined(DSAC_FILTER_STATS) && !defined(__CUDA_ARCH__)
-    g_filter_reason[20 + nroots / 2]++;   // statistics build: candidates with 0 / 2 / 4 real roots (the roofline's flop model)
-#endif
-    // world triangle frame and the 4th point's coordinates in it
-    const double inv_d = filt_rsqrt(s01), inv_n = filt_rsqrt(nn), d01 = s01 * inv_d;
+    const bool g1 = (!(s01 > 0)) | (!(s12 > 0)) | (!(nn > 0));                          // (1) degenerate triangle
+    // world triangle frame and the 4th point's coordinates in it (first, so that the scene coordinates are dead early)
+    const double inv_d = filt_rsqrt(s01), inv_n = filt_rsqrt(nn);
     const double e1x = ax * inv_d, e1y = ay * inv_d, e1z = az * inv_d;
     const double e3x = nx * inv_n, e3y = ny * inv_n, e3z = nz * inv_n;
     const double e2x = e3y * e1z - e3z * e1y, e2y = e3z * e1x - e3x * e1z, e2z = e3x * e1y - e3y * e1x;
     const double wx = X[3][0] - X[0][0], wy = X[3][1] - X[0][1], wz = X[3][2] - X[0][2];
-    const double al = wx * e1x + wy * e1y + wz * e1z, be = wx * e2x + wy * e2y + wz * e2z, ga = wx * e3x + wy * e3y + wz * e3z;
+    const double alw = wx * e1x + wy * e1y + wz * e1z, bew = wx * e2x + wy * e2y + wz * e2z, gaw = wx * e3x + wy * e3y + wz * e3z;
 #if !DSAC_FILTER_FP32_TAIL
     const double lim2 = (thr + DSAC_FILTER_BAND_PX) * (thr + DSAC_FILTER_BAND_PX);
 #else
     const float b0x = (float)bear[0][0], b0y = (float)bear[0][1], b0z = (float)bear[0][2];
     const float b1x = (float)bear[1][0], b1y = (float)bear[1][1], b1z = (float)bear[1][2];
     const float b2x = (float)bear[2][0], b2y = (float)bear[2][1], b2z = (float)bear[2][2];
-    const float d01f = (float)d01, inv_df = (float)inv_d, inv_nf = (float)inv_n;
-    const float alf = (float)al, bef = (float)be, gaf = (float)ga, ff = (float)f, du3f = (float)(mu3 - cx), dv3f = (float)(mv3 - cy);
+    const float inv_df = (float)inv_d, inv_nf = (float)inv_n, sa12f = (float)filt_sqrt(s12);
+    const float alf = (float)alw, bef = (float)bew, gaf = (float)gaw, ff = (float)f, du3f = (float)(mu3 - cx), dv3f = (float)(mv3 - cy);
     const float lim2f = (float)((thr + DSAC_FILTER_FP32_BAND) * (thr + DSAC_FILTER_FP32_BAND));
     const bool illcond = !(nn > 1e-3 * s01 * s02);   // sin^2 of the world triangle's angle at point 0: cross products lose 1 / sin of their digits
 #endif
-    // 96.9 % of the candidates have exactly two real roots, 0.7 % four (tools/filter_stats.py): slots 0 and 1 are evaluated
-    // by every lane, slots 2 and 3 only by the lanes that have them (a divergent branch one warp in five takes).
+    const double b01 = bear[0][0] * bear[1][0] + bear[0][1] * bear[1][1] + bear[0][2] * bear[1][2];
+    const double b02 = bear[0][0] * bear[2][0] + bear[0][1] * bear[2][1] + bear[0][2] * bear[2][2];
+    const double b12 = bear[1][0] * bear[2][0] + bear[1][1] * bear[2][1] + bear[1][2] * bear[2][2];
+    const double i12 = filt_rcp(s12), A01 = s01 * i12, A02 = s02 * i12;
+    // det(D1 + g D2) = c3 g^3 + c2 g^2 + c1 g + c0
+    const double sn = 1 - b12 * b12, u01 = 1 - b01 * b01, u02 = 1 - b02 * b02, k2 = 2 - 2 * b01 * b02 * b12;
+    const double c3 = A02 * (A02 * sn - u02), c0 = A01 * (A01 * sn - u01), cr = 2 * A01 * A02 * sn;
+    const double c2 = A02 * (A02 * sn - k2) + cr - A01 * u02 + u02;
+    const double c1 = A01 * (A01 * sn - k2) + cr - A02 * u01 + u01;
+    const double i3 = filt_rcp(c3);
+    bool cubic_ok;
+    const double g = cubic_first_root_seeded(c2 * i3, c1 * i3, c0 * i3, &cubic_ok);
+    const bool g2 = (!(fabs(c3) > 1e-12 * (fabs(c2) + fabs(c1) + fabs(c0)))) | (!cubic_ok);   // (2) cubic not settled
+    // D0 = D1 + g D2 (symmetric) and its 2 x 2 minors
+    const double d00 = 1 + g, d01 = -b01, d02 = -g * b02, d11 = 1 - A01 - g * A02, d12 = b12 * (A01 + g * A02),
+                 d22 = g * (1 - A02) - A01;
+    const double P = d01 * d01 - d00 * d11, Q = d02 * d02 - d00 * d22, m = d01 * d02 - d00 * d12;
+    // P, Q and the planes move by ~eps |D0|^2 / |S| under a relative error eps of D0's entries (|D0| = Frobenius norm): the
+    // sign of S and every quadratic discriminant below are decided only outside bands scaled by kappa = |D0|^2 / |S|
+    const double S = P + Q, F2 = d00 * d00 + d11 * d11 + d22 * d22 + 2 * (d01 * d01 + d02 * d02 + d12 * d12);
+    const bool g3 = !(fabs(S) > 1e-9 * F2);                                              // (3) planes or none
+    const bool planes = S > 0;
+    const bool pP = fabs(P) >= fabs(Q);
+    const double pv = fabs(pP ? P : Q), ir = filt_rsqrt(pv), sq = pv * ir, mr = m * ir;
+    const double al = pP ? sq : mr, be = pP ? mr : sq;
+    const bool g4 = planes & !(fabs(d00) > 1e-4 * (fabs(d01) + fabs(d02) + sq + fabs(mr)));   // (4) small pivot d00
+    const double id0 = filt_rcp(d00);
+    const double wA0 = (al - d01) * id0, wA1 = (be - d02) * id0, wB0 = (-al - d01) * id0, wB1 = (-be - d02) * id0;
+    // the second conic, e00 = 1
+    const bool big = fabs(g) > 1;
+    const double e01 = big ? -b01 : 0., e02 = big ? 0. : -b02, e11 = big ? 1 - A01 : -A02, e12 = b12 * (big ? A01 : A02),
+                 e22 = big ? -A01 : 1 - A02;
+    // per plane: qa tau^2 + 2 hb tau + qc = 0
+    auto plane_quadratic = [&](double w0, double w1, double q[3], bool* real, bool* unc) {
+        q[0] = w0 * (w0 + 2 * e01) + e11;
+        q[1] = w0 * (w1 + e02) + e01 * w1 + e12;
+        q[2] = w1 * (w1 + 2 * e02) + e22;
+        const double disc = q[1] * q[1] - q[0] * q[2];
+        *unc = !(fabs(disc) * fabs(S) > 1e-9 * F2 * (q[1] * q[1] + fabs(q[0] * q[2])));   // |disc| > 1e-9 kappa (scale)
+        *real = disc > 0;
+    };
+    // its roots as t / qa and qc / t with t = -hb - sign(hb) sqrt(disc)
+    auto plane_roots = [&](const double q[3], double* t1, double* t2) {
+        const double ad = fabs(q[1] * q[1] - q[0] * q[2]), sd = ad * filt_rsqrt(ad);
+        const double t = -q[1] - copysign(sd, q[1]), r = filt_rcp(q[0] * t);
+        *t1 = t * t * r;
+        *t2 = q[2] * q[0] * r;
+    };
+    double qA[3], qB[3];
+    bool realA, realB, uncA, uncB;
+    plane_quadratic(wA0, wA1, qA, &realA, &uncA);
+    plane_quadratic(wB0, wB1, qB, &realB, &uncB);
+    const bool g5 = planes & (uncA | uncB);                                               // (5) tau discriminant ~ 0
+    const bool hasA = planes & realA, hasB = planes & realB;
+    const int nroots = (hasA ? 2 : 0) + (hasB ? 2 : 0);
+    // no planes: the null vector of D0 is the only real direction left; it is a solution only if it lies on the second
+    // conic as well (a tangency, i.e. a double root: flagged)
+    const double v0 = pP ? d01 * d12 - d02 * d11 : d01 * d22 - d02 * d12, v1 = pP ? m : Q, v2 = pP ? -P : -m;
+    const double vev = v0 * v0 + e11 * v1 * v1 + e22 * v2 * v2 + 2 * (e01 * v0 * v1 + e02 * v0 * v2 + e12 * v1 * v2);
+    const double vsc = (v0 * v0 + v1 * v1 + v2 * v2) * (1 + fabs(e11) + fabs(e22) + fabs(e01) + fabs(e02) + fabs(e12));
+    const bool g9 = (!planes) & !(fabs(vev) > 1e-7 * vsc);                                // (9) null vector on the conic
+    bool flag = g1 | g2 | g3 | g4 | g5 | g9;
+#if defined(DSAC_FILTER_STATS) && !defined(__CUDA_ARCH__)
+    g_filter_reason[20 + nroots / 2]++;   // statistics build: candidates with 0 / 2 / 4 real solutions (the roofline's flop model)
+    if (flag) g_filter_reason[g1 ? 1 : g2 ? 2 : g3 ? 3 : g4 ? 4 : g5 ? 5 : 9]++;
+#endif
+    // Two real solutions are the common case (one plane holds both, the other a complex pair), four are rare: slots 0 and 1
+    // (plane A if it is real, else plane B) are evaluated by every lane, slots 2 and 3 (plane B) only by the lanes that
+    // have them (a divergent branch few warps take).
+    // slots 0, 1: plane A if it is real, else plane B; slots 2, 3: plane B
+    const double wS0 = hasA ? wA0 : wB0, wS1 = hasA ? wA1 : wB1;
+    const double qS[3] = {hasA ? qA[0] : qB[0], hasA ? qA[1] : qB[1], hasA ? qA[2] : qB[2]};
+    double tau_s[4];
+    plane_roots(qS, &tau_s[0], &tau_s[1]);
     auto root_slot = [&](int i) {
-        double x = (i == 0) ? xr[0] : (i == 1) ? xr[1] : (i == 2) ? xr[2] : xr[3];
-        const double Dn = D1 * x + D0;
-        const bool f5 = !(fabs(Dn) > 1.1e-3 * (fabs(D1 * x) + fabs(D0)));   // (the full solve switches formula at 1e-3)
-        double y = -((N2 * x + N1) * x + N0) * filt_rcp(Dn);
-        const double f1 = (1 - a) * y * y - a * x * x - p * y + a * r * x * y + 1;
-        const double f2 = (1 - b) * x * x - b * y * y - q * x + b * r * x * y + 1;
-        const double j11 = -2 * a * x + a * r * y, j12 = 2 * (1 - a) * y - p + a * r * x;
-        const double j21 = 2 * (1 - b) * x - q + b * r * y, j22 = -2 * b * y + b * r * x;
-        const double det = j11 * j22 - j12 * j21;
-        const double jn = j11 * j11 + j12 * j12 + j21 * j21 + j22 * j22;
-        const bool f6 = !(fabs(det) > 1e-4 * jn);
-        const double idet = filt_rcp(det);
-        const double dx = (f1 * j22 - f2 * j12) * idet, dy = (j11 * f2 - j21 * f1) * idet;
-        x -= dx;
-        y -= dy;
-        const bool f7 = !(fabs(dx) + fabs(dy) <= 1e-6 * (fabs(x) + fabs(y)));
-        const bool neg = (x < -1e-6) | (y < -1e-6);        // certainly a non-physical solution: the root decides nothing
-        const bool f8 = (x < 1e-6) | (y < 1e-6);           // borderline positivity
-        const double v = x * x + y * y - x * y * r;
-        const bool f9 = !(v > 1e-12);
+        const double tau = (i == 0) ? tau_s[0] : (i == 1) ? tau_s[1] : (i == 2) ? tau_s[2] : tau_s[3];
+        const double w0 = (i < 2) ? wS0 : wB0, w1 = (i < 2) ? wS1 : wB1;
+        // depths in units of sqrt(a12) (the E_ij divided by a12)
+        const double L2 = filt_rsqrt(tau * (tau - 2 * b12) + 1), L1 = tau * L2, L0 = w0 * L1 + w1 * L2;
+        // Accuracy of lambda without taking the Gauss-Newton step on the E_ij: with J / 2 = [[A, B, 0], [C, 0, D], [0, E, F]]
+        // and residuals r, the step J^-1 r is at most 1.5 (n1 n2 + n1 n3 + n2 n3) |r|_1 / |det| in each coordinate (every
+        // cofactor is a product of entries of two different rows, n_k = row sums of |entries|).
+        const double A = L0 - b01 * L1, B = L1 - b01 * L0, C = L0 - b02 * L2, D = L2 - b02 * L0, E = L1 - b12 * L2,
+                     F = L2 - b12 * L1;
+        const double r01 = L0 * A + L1 * B - A01, r02 = L0 * C + L2 * D - A02, r12 = L1 * E + L2 * F - 1;
+        const double n1 = fabs(A) + fabs(B), n2 = fabs(C) + fabs(D), n3 = fabs(E) + fabs(F);
+        const double det = A * D * E + B * C * F;                      // -det(J / 2)
+        const double Ls = fabs(L0) + fabs(L1) + fabs(L2);
+        const bool f6 = !(fabs(det) > 1e-4 * n1 * n2 * n3);            // ill-conditioned Jacobian (NaN)
+        const bool f7 = !(1.5 * (n1 * (n2 + n3) + n2 * n3) * (fabs(r01) + fabs(r02) + fabs(r12)) <= 1e-7 * fabs(det) * Ls);
+        const bool neg = (L0 < -1e-6 * Ls) | (L1 < -1e-6 * Ls);       // certainly a non-physical solution: it decides nothing
+        const bool f8 = (L0 < 1e-6 * Ls) | (L1 < 1e-6 * Ls);          // borderline positivity
 #if DSAC_FILTER_FP32_TAIL
-        // The 4th point's camera position and pixel error in fp32 (FMA pipe, idle in this kernel) instead of fp64: (x, y) are
-        // polished in fp64 above; from here on the quantities are lengths of ~10^2..10^4 mm combined without dangerous
-        // cancellation unless the triangle is nearly degenerate (guarded: cond below).  Measured on 2 * 10^6 benchmark
-        // candidates (tools/filter_stats.py, statistics build): |pixel error fp32 - fp64| <= DSAC_FILTER_FP32_MAXDEV px; the
-        // threshold band is widened from 0.05 px to DSAC_FILTER_FP32_BAND px to cover it many times over.
-        const float xf = (float)x, yf = (float)y;
-        const float Zf = d01f * DSAC_RSQRTF_EARLY((float)v);
-        const float L0 = xf * Zf, L1 = yf * Zf;
-        const float M0x = L0 * b0x, M0y = L0 * b0y, M0z = L0 * b0z;
-        const float ux = L1 * b1x - M0x, uy = L1 * b1y - M0y, uz = L1 * b1z - M0z;
+        // The 4th point's camera position and pixel error in fp32 (FMA pipe, idle in this kernel) instead of fp64: the depths
+        // are accurate to 1e-7 in fp64 (f7); from here on the quantities are lengths of ~10^2..10^4 mm combined without dangerous
+        // cancellation unless the triangle is nearly degenerate (guarded: illcond).  Measured on the benchmark candidates
+        // (tools/filter_stats.py, statistics build): |pixel error fp32 - fp64| stays far below DSAC_FILTER_FP32_BAND.
+        const float Zf = (float)L2 * sa12f, L0f = (float)L0 * sa12f, L1f = (float)L1 * sa12f;
+        const float M0x = L0f * b0x, M0y = L0f * b0y, M0z = L0f * b0z;
+        const float ux = L1f * b1x - M0x, uy = L1f * b1y - M0y, uz = L1f * b1z - M0z;
         const float vx = Zf * b2x - M0x, vy = Zf * b2y - M0y, vz = Zf * b2z - M0z;
         const float cxn = uy * vz - uz * vy, cyn = uz * vx - ux * vz, czn = ux * vy - uy * vx;
         const float c1x = ux * inv_df, c1y = uy * inv_df, c1z = uz * inv_df;
@@ -888,48 +908,49 @@ DSAC_HD bool p3p_quick_core(const double bear[3][3], const double X[4][3], doubl
         const bool f10 = (!(gu * gu + gv * gv > lim2f * zz)) | (!(zz > 0.f)) | shallow | illcond;
 #if defined(DSAC_FILTER_STATS) && !defined(__CUDA_ARCH__)
         {   // statistics build: the same quantity in fp64, to record the largest deviation of the fp32 pixel error
-            const double Zd = d01 * filt_rsqrt(v), l0 = x * Zd, l1 = y * Zd;
+            const double sa12 = sqrt(s12), l0 = L0 * sa12, l1 = L1 * sa12, l2 = L2 * sa12;
             const double m0x = l0 * bear[0][0], m0y = l0 * bear[0][1], m0z = l0 * bear[0][2];
             const double Ux = l1 * bear[1][0] - m0x, Uy = l1 * bear[1][1] - m0y, Uz = l1 * bear[1][2] - m0z;
-            const double Vx = Zd * bear[2][0] - m0x, Vy = Zd * bear[2][1] - m0y, Vz = Zd * bear[2][2] - m0z;
+            const double Vx = l2 * bear[2][0] - m0x, Vy = l2 * bear[2][1] - m0y, Vz = l2 * bear[2][2] - m0z;
             const double Cx = Uy * Vz - Uz * Vy, Cy = Uz * Vx - Ux * Vz, Cz = Ux * Vy - Uy * Vx;
             const double k1x = Ux * inv_d, k1y = Uy * inv_d, k1z = Uz * inv_d, k3x = Cx * inv_n, k3y = Cy * inv_n, k3z = Cz * inv_n;
             const double k2x = k3y * k1z - k3z * k1y, k2y = k3z * k1x - k3x * k1z, k2z = k3x * k1y - k3y * k1x;
-            const double X3d = m0x + al * k1x + be * k2x + ga * k3x, Y3d = m0y + al * k1y + be * k2y + ga * k3y, Z3d = m0z + al * k1z + be * k2z + ga * k3z;
+            const double X3d = m0x + alw * k1x + bew * k2x + gaw * k3x, Y3d = m0y + alw * k1y + bew * k2y + gaw * k3y,
+                         Z3d = m0z + alw * k1z + bew * k2z + gaw * k3z;
             const double e64 = sqrt((f * X3d / Z3d - (mu3 - cx)) * (f * X3d / Z3d - (mu3 - cx)) + (f * Y3d / Z3d - (mv3 - cy)) * (f * Y3d / Z3d - (mv3 - cy)));
             const double e32 = sqrt((double)(gu * gu + gv * gv)) / fabs((double)Z3);
-            if (i < nroots && !neg && !(f5 | f6 | f7 | f8 | f9) && !shallow && !illcond && e64 < 200.0) {
+            if (i < nroots && !neg && !(f6 | f7 | f8) && !shallow && !illcond && e64 < 200.0) {
                 const double dev = fabs(e32 - e64);
                 if (dev > g_filter_fp32_maxdev) g_filter_fp32_maxdev = dev;
             }
         }
 #endif
 #else
-        const double Z = d01 * filt_rsqrt(v);
-        const double L0 = x * Z, L1 = y * Z;
-        const double M0x = L0 * bear[0][0], M0y = L0 * bear[0][1], M0z = L0 * bear[0][2];
-        const double ux = L1 * bear[1][0] - M0x, uy = L1 * bear[1][1] - M0y, uz = L1 * bear[1][2] - M0z;
-        const double vx = Z * bear[2][0] - M0x, vy = Z * bear[2][1] - M0y, vz = Z * bear[2][2] - M0z;
+        const double sa12 = filt_sqrt(s12), l0 = L0 * sa12, l1 = L1 * sa12, l2 = L2 * sa12;
+        const double M0x = l0 * bear[0][0], M0y = l0 * bear[0][1], M0z = l0 * bear[0][2];
+        const double ux = l1 * bear[1][0] - M0x, uy = l1 * bear[1][1] - M0y, uz = l1 * bear[1][2] - M0z;
+        const double vx = l2 * bear[2][0] - M0x, vy = l2 * bear[2][1] - M0y, vz = l2 * bear[2][2] - M0z;
         const double cxn = uy * vz - uz * vy, cyn = uz * vx - ux * vz, czn = ux * vy - uy * vx;
         const double c1x = ux * inv_d, c1y = uy * inv_d, c1z = uz * inv_d;
         const double c3x = cxn * inv_n, c3y = cyn * inv_n, c3z = czn * inv_n;
         const double c2x = c3y * c1z - c3z * c1y, c2y = c3z * c1x - c3x * c1z, c2z = c3x * c1y - c3y * c1x;
-        const double X3 = M0x + al * c1x + be * c2x + ga * c3x;
-        const double Y3 = M0y + al * c1y + be * c2y + ga * c3y;
-        const double Z3 = M0z + al * c1z + be * c2z + ga * c3z;
+        const double X3 = M0x + alw * c1x + bew * c2x + gaw * c3x;
+        const double Y3 = M0y + alw * c1y + bew * c2y + gaw * c3y;
+        const double Z3 = M0z + alw * c1z + bew * c2z + gaw * c3z;
         // |(cx + f X3 / Z3 - mu3, cy + f Y3 / Z3 - mv3)|^2 > lim2, multiplied through by Z3^2 (no division)
         const double gu = f * X3 - (mu3 - cx) * Z3, gv = f * Y3 - (mv3 - cy) * Z3, zz = Z3 * Z3;
         const bool f10 = (!(gu * gu + gv * gv > lim2 * zz)) | (!(zz > 0));
 #endif
-        const bool root_flag = f5 | f6 | f7 | ((!neg) & (f8 | f9 | f10));
+        const bool root_flag = f6 | f7 | ((!neg) & (f8 | f10));
 #if defined(DSAC_FILTER_STATS) && !defined(__CUDA_ARCH__)
-        if (!flag && i < nroots && root_flag) g_filter_reason[f5 ? 5 : f6 ? 6 : f7 ? 7 : f8 ? 8 : f9 ? 9 : 10]++;
+        if (!flag && i < nroots && root_flag) g_filter_reason[f6 ? 6 : f7 ? 7 : f8 ? 8 : 10]++;
 #endif
         flag |= (i < nroots) & root_flag;
     };
     root_slot(0);
     root_slot(1);
     if (nroots > 2) {
+        plane_roots(qB, &tau_s[2], &tau_s[3]);
         root_slot(2);
         root_slot(3);
     }
@@ -949,7 +970,7 @@ DSAC_HD bool p3p_quick_inline(const P3PProblem& pr, double f, double cx, double 
 #endif
         bear[i][0] = u * k; bear[i][1] = v * k; bear[i][2] = k;
     }
-    return p3p_quick_core(bear, pr.X, pr.mu[3], pr.mv[3], f, cx, cy, thr);
+    return p3p_lambda_core(bear, pr.X, pr.mu[3], pr.mv[3], f, cx, cy, thr);
 }
 
 // ---------------------------------------------------------------------------------------

@@ -1210,7 +1210,7 @@ __device__ __forceinline__ bool k1_filter_candidate(const CellRec* cell, const i
             mu3 = mu; mv3 = mv;
         }
     }
-    return p3p_quick_core(bear, X, mu3, mv3, f, cx, cy, thr);
+    return p3p_lambda_core(bear, X, mu3, mv3, f, cx, cy, thr);
 }
 
 #ifndef K1F_MAXREG
