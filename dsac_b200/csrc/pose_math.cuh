@@ -742,8 +742,11 @@ static double g_filter_fp32_maxdev = 0;
 #define DSAC_FILTER_FP32_TAIL 1        /* 4th-point stage of the conservative filter in fp32 with a widened band (else fp64) */
 #endif
 #ifndef DSAC_FILTER_FP32_BAND
-#define DSAC_FILTER_FP32_BAND 0.25     /* px: candidates whose 4th point lands within thr + 0.25 px go to the full solve (fp32 deviates <= 0.007 px) */
+#define DSAC_FILTER_FP32_BAND 0.25     /* px: candidates whose 4th point lands within thr + 0.25 px go to the full solve */
 #endif
+#define DSAC_U32 5.9604645e-8f         /* 2^-24: unit roundoff of fp32 */
+#define DSAC_TAIL_EPS 4.6e-7f          /* 1e-7 (depth accuracy, f7) + 6 u: relative error of a camera point the tail forms */
+#define DSAC_TAIL_MARGIN 0.05          /* px: headroom beyond thr + the fp32 tail's error bound (not derived: see the tail) */
 // Core of the filter on prepared inputs: unit bearings of points 0..2, the four scene coordinates and the pixel
 // (mu3, mv3) of the 4th point as P3P sees it (k_sample keeps 1/|(u, v, 1)| per cell in shared memory).
 //
@@ -792,6 +795,15 @@ DSAC_HD bool p3p_lambda_core(const double bear[3][3], const double X[4][3], doub
     const float alf = (float)alw, bef = (float)bew, gaf = (float)gaw, ff = (float)f, du3f = (float)(mu3 - cx), dv3f = (float)(mv3 - cy);
     const float lim2f = (float)((thr + DSAC_FILTER_FP32_BAND) * (thr + DSAC_FILTER_FP32_BAND));
     const bool illcond = !(nn > 1e-3 * s01 * s02);   // sin^2 of the world triangle's angle at point 0: cross products lose 1 / sin of their digits
+    // Per-candidate factors of the bound dP3 = errA * Lam + errB on the fp32 tail's camera coordinates of the 4th point
+    // (derived at the tail below): errA = eps (1 + 2 W (1 / d01 + (d01 + d02) / |n|)) + 5 u,
+    // errB = u W (7.2 d01 d02 / |n| + 15.2), with W = |alpha| + |beta| + |gamma|.
+    const float d01f = (float)s01 * inv_df, s02f = (float)s02, d02f = s02f * DSAC_RSQRTF_EARLY(s02f), Wf = fabsf(alf) + fabsf(bef) + fabsf(gaf);
+    const float errA = DSAC_TAIL_EPS * (1.f + 2.f * Wf * (inv_df + (d01f + d02f) * inv_nf)) + 5.f * DSAC_U32;
+    const float errB = DSAC_U32 * Wf * (7.2f * d01f * d02f * inv_nf + 15.2f), errL = errA * sa12f;
+    // 1.25 de_zz = kf dP3 (2 |Z3| + |X3| + |Y3|) + |Z3| (kuf (|X3| + |Y3|) + kud |Z3|)
+    const float kf = 1.25f * ff, kuf = 10.f * DSAC_U32 * ff, kud = 10.f * DSAC_U32 * (fabsf(du3f) + fabsf(dv3f));
+    const float thrm = (float)(thr + DSAC_TAIL_MARGIN);
 #endif
     const double b01 = bear[0][0] * bear[1][0] + bear[0][1] * bear[1][1] + bear[0][2] * bear[1][2];
     const double b02 = bear[0][0] * bear[2][0] + bear[0][1] * bear[2][1] + bear[0][2] * bear[2][2];
@@ -886,10 +898,37 @@ DSAC_HD bool p3p_lambda_core(const double bear[3][3], const double X[4][3], doub
         const bool neg = (L0 < -1e-6 * Ls) | (L1 < -1e-6 * Ls);       // certainly a non-physical solution: it decides nothing
         const bool f8 = (L0 < 1e-6 * Ls) | (L1 < 1e-6 * Ls);          // borderline positivity
 #if DSAC_FILTER_FP32_TAIL
-        // The 4th point's camera position and pixel error in fp32 (FMA pipe, idle in this kernel) instead of fp64: the depths
-        // are accurate to 1e-7 in fp64 (f7); from here on the quantities are lengths of ~10^2..10^4 mm combined without dangerous
-        // cancellation unless the triangle is nearly degenerate (guarded: illcond).  Measured on the benchmark candidates
-        // (tools/filter_stats.py, statistics build): |pixel error fp32 - fp64| stays far below DSAC_FILTER_FP32_BAND.
+        // The 4th point's camera position and pixel error in fp32 (FMA pipe, idle in this kernel) instead of fp64.  The result
+        // decides only where the pixel error exceeds thr by more than its error bound, derived here.  u = 2^-24, |.| are
+        // 2-norms, lengths in mm, and "true" means the exact solve's pose for the same root.
+        //  (a) Camera points P_i = l_i b_i.  The depths are within 1e-7 Lam of the root (Lam = l0 + l1 + l2): f7 bounds the
+        //      Gauss-Newton step on the distance equations, a first-order estimate of the depth error, not an enclosure of
+        //      the root (its remainder is quadratic in a step below 1e-7).  The fp32 roundings of L_i, sqrt(a12), the bearing
+        //      and two products add 5 u l_i: |dP_i| <= eps Lam, eps = 1e-7 + 6 u.
+        //  (b) u = P1 - P0, v = P2 - P0 (|u| = d01, |v| = d02): |du| <= 2 eps Lam + u d01, |dv| <= 2 eps Lam + u d02.
+        //  (c) c1 = u / d01: |dc1| <= 2 eps Lam / d01 + 3 u (the roundings of inv_d and of the product add 2 u).
+        //  (d) n = u x v, |n| = d01 d02 sin(theta): |dn| <= |du| d02 + d01 |dv| + 3 sqrt(3) u d01 d02
+        //      <= 2 eps Lam (d01 + d02) + 7.2 u d01 d02, so c3 = n / |n|: |dc3| <= (2 eps Lam (d01 + d02) + 7.2 u d01 d02) / |n| + 2 u.
+        //  (e) c2 = c3 x c1 (unit vectors): |dc2| <= |dc3| + |dc1| + 3 sqrt(3) u.
+        //  (f) X3 = M0x + alpha c1x + beta c2x + gamma c3x, the same for Y3 and Z3, W = |alpha| + |beta| + |gamma|:
+        //      |dX3| <= |dM0| + W max|dc_k| + u W (alpha .. gamma rounded to fp32) + 4 u (Lam + W) (three products, three sums)
+        //      <= Lam (eps (1 + 2 W (1 / d01 + (d01 + d02) / |n|)) + 5 u) + u W (7.2 d01 d02 / |n| + 15.2) = errA Lam + errB = dP3.
+        //      This is the term the triangle's size enters: a 5 mm triangle metres away from the camera and from its 4th point
+        //      gives W / d01 ~ 10^3, and |dc_k| ~ 10^3 eps.
+        //  (g) Pixel error e = |(f X3 / Z3 - du3, f Y3 / Z3 - dv3)|: |d(f X3 / Z3)| <= f (|dX3| + |X3 / Z3| |dZ3|) / |Z3|.
+        //      gu = f X3 - du3 Z3 rounds ff, du3f, two products and a difference: 3 u (f |X3| + |du3| |Z3|); the norm
+        //      sqrt(gu^2 + gv^2) adds 4 u of itself, which is <= 4 u (f (|X3| + |Y3|) + (|du3| + |dv3|) |Z3|).  Together
+        //      |de| Z3^2 <= de_zz = f dP3 (2 |Z3| + |X3| + |Y3|) + 8 u |Z3| (f (|X3| + |Y3|) + (|du3| + |dv3|) |Z3|).
+        //      Beyond first order in dP3: X'/Z' - X/Z = (Z dX - X dZ) / (Z Z'), so, given (a), the bound holds without a
+        //      remainder once multiplied by |Z3| / (|Z3| - dP3) (dP3 < |Z3| / 2 required).
+        // A 4th point counts as certainly off only if e - 1.25 |de| |Z3| / (|Z3| - dP3) > thr + DSAC_TAIL_MARGIN (multiplied
+        // through by |Z3| (|Z3| - dP3) and squared: no division, no square root), on top of the band test
+        // e > thr + DSAC_FILTER_FP32_BAND.  The factor 1.25 covers the rounding of the bound itself (sums and products of
+        // positive terms: a few u relative).  DSAC_TAIL_MARGIN (0.05 px, the fp64 tail's DSAC_FILTER_BAND_PX) is not derived:
+        // it is headroom for what the bound leaves out, the quadratic remainder of f7's estimate in (a) and the exact
+        // solve's own fp64 error on its 4th-point error (~1e-12 px).  Otherwise the candidate is flagged.
+        // The bound grows with f, with the 4th pixel's distance from the principal point (|X3|, |Y3| against |Z3|), and
+        // with Lam and W against |Z3|: a 4th point close to the camera of a distant triangle is the dangerous case.
         const float Zf = (float)L2 * sa12f, L0f = (float)L0 * sa12f, L1f = (float)L1 * sa12f;
         const float M0x = L0f * b0x, M0y = L0f * b0y, M0z = L0f * b0z;
         const float ux = L1f * b1x - M0x, uy = L1f * b1y - M0y, uz = L1f * b1z - M0z;
@@ -902,9 +941,11 @@ DSAC_HD bool p3p_lambda_core(const double bear[3][3], const double X[4][3], doub
         const float Y3 = M0y + alf * c1y + bef * c2y + gaf * c3y;
         const float Z3 = M0z + alf * c1z + bef * c2z + gaf * c3z;
         const float gu = ff * X3 - du3f * Z3, gv = ff * Y3 - dv3f * Z3, zz = Z3 * Z3;
-        // depth of the 4th point not tiny against the lengths it was summed from: the fp32 error of Z3 is ~10 eps (sum), so above
-        // this guard Z3 is good to 0.6 %, i.e. 0.06 px on an error at the 10 px threshold (a larger error need not be accurate)
-        const bool shallow = !(fabsf(Z3) > 2e-4f * (fabsf(M0z) + fabsf(alf) + fabsf(bef) + fabsf(gaf)));
+        const float aX = fabsf(X3) + fabsf(Y3), aZ = fabsf(Z3), dP3 = errL * (float)Ls + errB;
+        const float de125 = kf * dP3 * (2.f * aZ + aX) + aZ * (kuf * aX + kud * aZ), tz = aZ - dP3;
+        const float rin = thrm * aZ * tz + de125;
+        // (g): |(gu, gv)| tz > (thr + margin) |Z3| tz + 1.25 de_zz, squared (both sides positive), and dP3 < |Z3| / 2
+        const bool shallow = !(dP3 < tz) | !((gu * gu + gv * gv) * (tz * tz) > rin * rin);
         const bool f10 = (!(gu * gu + gv * gv > lim2f * zz)) | (!(zz > 0.f)) | shallow | illcond;
 #if defined(DSAC_FILTER_STATS) && !defined(__CUDA_ARCH__)
         {   // statistics build: the same quantity in fp64, to record the largest deviation of the fp32 pixel error

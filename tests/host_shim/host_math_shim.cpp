@@ -59,6 +59,16 @@ void shim_stream_chunk(int H, int T, int s, int* h0, int* cnt) { dsac::stream_ch
 extern "C" int shim_needs_full(const float* obj, const float* img, double f, double cx, double cy, int thr) {
     return dsac::minimal_set_needs_full(obj, img, f, cx, cy, thr) ? 1 : 0;
 }
+// n minimal sets (obj [n][12], img [n][8]): the exact solve's verdict and the conservative filter's, one byte each
+extern "C" void shim_filter_batch(int n, const float* obj, const float* img, double f, double cx, double cy, int thr,
+                                  uint8_t* accepted, uint8_t* needs_full) {
+    for (int k = 0; k < n; k++) {
+        double rv[3], tv[3];
+        bool fr;
+        accepted[k] = dsac::minimal_set_hypothesis(obj + 12 * k, img + 8 * k, f, cx, cy, thr, rv, tv, &fr) ? 1 : 0;
+        needs_full[k] = dsac::minimal_set_needs_full(obj + 12 * k, img + 8 * k, f, cx, cy, thr) ? 1 : 0;
+    }
+}
 
 #include <random>
 static long long* g_reasons = nullptr; static int g_miss[64]; static int g_nmiss = 0;
