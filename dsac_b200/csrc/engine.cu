@@ -23,6 +23,7 @@
 #include "sampler_split.cuh"
 #include "train.cuh"
 #include "upstream.cuh"
+#include "objtrain.cuh"
 
 using namespace dsac;
 
@@ -42,6 +43,8 @@ struct dsac_engine {
     cudaEvent_t ev_fwd = nullptr;   // recorded after the last forward launch: the backward waits on it
     double* d_kabsch = nullptr;     // dsac_kabsch: inputs and outputs in one grow-only block
     size_t kabsch_bytes = 0;
+    uint64_t* d_reg_keys = nullptr; // dsac_register_depth_device: per-pixel scatter keys, grow-only
+    size_t reg_keys_bytes = 0;
     int sm_count = 132;
     // inputs (device copies for the host-buffer entry point)
     int16_t* d_coords = nullptr;
@@ -223,6 +226,7 @@ void dsac_engine_destroy(dsac_engine* e) {
     if (e->ev_fwd) cudaEventDestroy(e->ev_fwd);
     if (e->d_ext_g) cudaFree(e->d_ext_g);
     if (e->d_kabsch) cudaFree(e->d_kabsch);
+    if (e->d_reg_keys) cudaFree(e->d_reg_keys);
     if (e->d_phase) {
         unsigned long long h[16];
         if (cudaMemcpy(h, e->d_phase, sizeof(h), cudaMemcpyDeviceToHost) == cudaSuccess)
@@ -1385,6 +1389,137 @@ int dsac_coords_from_prediction_device(dsac_engine* e, int32_t n, const float* d
 int dsac_kabsch(dsac_engine* e, int32_t n, int32_t m, const double* a, const double* b, double* R, double* t) {
     if (!e) return DSAC_ERR_ARG;
     return kabsch_run(e, n, m, a, b, R, t);
+}
+
+// ----------------------------------------------------------------------------- coordinate-CNN pre-training data path
+
+int dsac_default_rgbd_camera(dsac_rgbd_camera* c) {
+    if (!c) return DSAC_ERR_ARG;
+    memset(c, 0, sizeof(*c));
+    c->focal = 525.f;              // properties.cpp defaults, as the shipped 7-Scenes default.config also sets them
+    c->secondary_focal = 585.f;
+    c->raw_data = 1;
+    c->width = 640;
+    c->height = 480;
+    for (int k = 0; k < 4; k++) c->sensor_trans[5 * k] = 1.0;   // no sensorTrans.dat: identity
+    return DSAC_OK;
+}
+
+static bool obj_cam(dsac_engine* e, const dsac_rgbd_camera* c, ObjCam* o) {
+    if (!c || c->width < 1 || c->height < 1) { fail(e, DSAC_ERR_ARG, "bad camera"); return false; }
+    o->focal = c->focal; o->x_shift = c->x_shift; o->y_shift = c->y_shift;
+    o->secondary_focal = c->secondary_focal; o->raw_x_shift = c->raw_x_shift; o->raw_y_shift = c->raw_y_shift;
+    memcpy(o->sensor_trans, c->sensor_trans, sizeof(o->sensor_trans));
+    o->raw_data = c->raw_data ? 1 : 0; o->width = c->width; o->height = c->height;
+    return true;
+}
+
+static inline unsigned grid_of(size_t n, int threads) { return (unsigned)((n + threads - 1) / threads); }
+
+__global__ void k_dropped_status(int n, const int32_t* dropped, uint32_t* status) {
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f < n) status[f] = dropped[f] ? DSAC_ST_DEPTH_DROPPED : 0u;
+}
+
+int dsac_register_depth_device(dsac_engine* e, const dsac_rgbd_camera* cam, int32_t n, const uint16_t* d_raw,
+                               uint16_t* d_depth, int32_t* d_dropped, uint32_t* d_status, void* stream_v) {
+    if (!e) return DSAC_ERR_ARG;
+    ObjCam c;
+    if (!obj_cam(e, cam, &c)) return DSAC_ERR_ARG;
+    if (n < 1 || !d_raw || !d_depth || d_raw == d_depth || (d_status && !d_dropped))
+        return fail(e, DSAC_ERR_ARG, "dsac_register_depth_device: bad arguments");
+    CU(cudaSetDevice(e->cfg.device));
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    const size_t count = (size_t)n * c.width * c.height;
+    if (d_dropped) CU(cudaMemsetAsync(d_dropped, 0, (size_t)n * sizeof(int32_t), stream));
+    if (c.raw_data) {
+        if (e->reg_keys_bytes < count * sizeof(uint64_t)) {
+            if (e->d_reg_keys) CU(cudaFree(e->d_reg_keys));
+            e->d_reg_keys = nullptr; e->reg_keys_bytes = 0;
+            CU(cudaMalloc(&e->d_reg_keys, count * sizeof(uint64_t)));
+            e->reg_keys_bytes = count * sizeof(uint64_t);
+        }
+        CU(cudaMemsetAsync(e->d_reg_keys, 0, count * sizeof(uint64_t), stream));
+    }
+    k_register_depth<<<grid_of(count, 256), 256, 0, stream>>>(c, n, d_raw, e->d_reg_keys, d_depth, d_dropped);
+    e->launches++;
+    if (c.raw_data) {
+        k_register_finish<<<grid_of(count, 256), 256, 0, stream>>>(count, e->d_reg_keys, d_depth);
+        e->launches++;
+    }
+    if (d_status) {
+        k_dropped_status<<<grid_of(n, 128), 128, 0, stream>>>(n, d_dropped, d_status);
+        e->launches++;
+    }
+    CU(cudaGetLastError());
+    return DSAC_OK;
+}
+
+int dsac_obj_coords_device(dsac_engine* e, const dsac_rgbd_camera* cam, int32_t n_frames, int32_t n, const int32_t* d_idx,
+                           const uint16_t* d_depth, const double* d_poses, int16_t* d_coords, void* stream_v) {
+    if (!e) return DSAC_ERR_ARG;
+    ObjCam c;
+    if (!obj_cam(e, cam, &c)) return DSAC_ERR_ARG;
+    if (n < 1 || n_frames < 1 || (!d_idx && n > n_frames) || !d_depth || !d_poses || !d_coords)
+        return fail(e, DSAC_ERR_ARG, "dsac_obj_coords_device: bad arguments");
+    CU(cudaSetDevice(e->cfg.device));
+    const size_t count = (size_t)n * c.width * c.height;
+    k_obj_coords<<<grid_of(count, 256), 256, 0, (cudaStream_t)stream_v>>>(c, n_frames, n, d_idx, d_depth, d_poses, d_coords);
+    e->launches++;
+    CU(cudaGetLastError());
+    return DSAC_OK;
+}
+
+int dsac_obj_rng_init_device(dsac_engine* e, uint32_t seed, int32_t n_streams, uint32_t* d_state, void* stream_v) {
+    if (!e) return DSAC_ERR_ARG;
+    if (n_streams < 1 || !d_state) return fail(e, DSAC_ERR_ARG, "dsac_obj_rng_init_device: bad arguments");
+    CU(cudaSetDevice(e->cfg.device));
+    k_obj_rng_init<<<grid_of(n_streams, 32), 32, 0, (cudaStream_t)stream_v>>>(seed, n_streams, d_state);
+    e->launches++;
+    CU(cudaGetLastError());
+    return DSAC_OK;
+}
+
+int dsac_obj_draw_device(dsac_engine* e, const dsac_rgbd_camera* cam, int32_t n_frames, const uint16_t* d_depth,
+                         const double* d_poses, int32_t n_images, int32_t n_patches, int32_t n_streams,
+                         int32_t max_attempts, uint32_t* d_state, int32_t* d_img, int32_t* d_centre, float* d_label,
+                         uint32_t* d_status, void* stream_v) {
+    if (!e) return DSAC_ERR_ARG;
+    ObjDrawParams p;
+    if (!obj_cam(e, cam, &p.cam)) return DSAC_ERR_ARG;
+    if (p.cam.width <= UP_PATCH || p.cam.height <= UP_PATCH)
+        return fail(e, DSAC_ERR_ARG, "a %dx%d frame holds no %d-pixel patch centre", p.cam.width, p.cam.height, UP_PATCH);
+    if (n_frames < 1 || n_images < 1 || n_patches < 1 || n_streams < 1 || max_attempts < 32 || !d_depth || !d_poses ||
+        !d_state || !d_img || !d_centre || !d_label || !d_status)
+        return fail(e, DSAC_ERR_ARG, "dsac_obj_draw_device: bad arguments");
+    CU(cudaSetDevice(e->cfg.device));
+    p.depth = d_depth; p.poses = d_poses;
+    p.n_frames = n_frames; p.n_images = n_images; p.n_patches = n_patches; p.n_streams = n_streams;
+    p.max_attempts = max_attempts; p.state = d_state;
+    p.img = d_img; p.centre = d_centre; p.label = d_label; p.status = d_status;
+    k_obj_draw<<<grid_of(n_streams, OBJ_DRAW_WARPS), 32 * OBJ_DRAW_WARPS, 0, (cudaStream_t)stream_v>>>(p);
+    e->launches++;
+    CU(cudaGetLastError());
+    return DSAC_OK;
+}
+
+int dsac_gather_patches_at_device(dsac_engine* e, int32_t n, const uint8_t* d_frames, int32_t n_frames, int32_t width,
+                                  int32_t height, const int32_t* d_frame, const int32_t* d_centre, float mean,
+                                  float* d_patches, uint32_t* d_status, void* stream_v) {
+    if (!e) return DSAC_ERR_ARG;
+    if (n < 1 || n_frames < 1 || !d_frames || !d_frame || !d_centre || !d_patches)
+        return fail(e, DSAC_ERR_ARG, "dsac_gather_patches_at_device: bad arguments");
+    if (width < UP_PATCH || height < UP_PATCH) return fail(e, DSAC_ERR_ARG, "frame %dx%d smaller than a %d-pixel patch", width, height, UP_PATCH);
+    CU(cudaSetDevice(e->cfg.device));
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    GatherAtParams p;
+    p.frames = d_frames; p.width = width; p.height = height; p.n_frames = n_frames;
+    p.frame = d_frame; p.centre = d_centre; p.mean = mean; p.patches = d_patches; p.status = d_status;
+    if (d_status) CU(cudaMemsetAsync(d_status, 0, sizeof(uint32_t), stream));
+    k_gather_patches_at<<<n, UP_THREADS, 0, stream>>>(p);
+    e->launches++;
+    CU(cudaGetLastError());
+    return DSAC_OK;
 }
 
 }  // extern "C"

@@ -1,9 +1,11 @@
 // host_util.cpp -- host-side helpers of the C ABI that carry the reference's RNG contract
 // and the synthetic-input generator of SURVEY.md section 8(d).  No device code.
+#include <algorithm>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
 #include <random>
+#include <vector>
 
 #include "../../include/dsac_b200.h"
 #define DSAC_HOST_ONLY 1
@@ -51,6 +53,18 @@ inline int16_t sat16(double v) {
 }  // namespace
 
 extern "C" {
+
+// train_obj.cpp:266-270: iota(n), then std::shuffle with std::mt19937(seed) (the reference's is default-seeded: 5489).
+// Compiled by the host compiler so that the permutation is libstdc++'s own.
+int dsac_shuffle_permutation(int32_t n, uint32_t seed, int32_t* out) {
+    if (n < 1 || !out) return DSAC_ERR_ARG;
+    std::vector<int> v((size_t)n);
+    for (int i = 0; i < n; i++) v[(size_t)i] = i;
+    std::mt19937 gen(seed);
+    std::shuffle(v.begin(), v.end(), gen);
+    for (int i = 0; i < n; i++) out[i] = v[(size_t)i];
+    return DSAC_OK;
+}
 
 // stochasticSubSample (cnn_softam.h:283-309; targetSize 40, patchSize 42) drawing from the
 // thread-0 generator of ThreadRand (mt19937 seeded `seed`, thread_rand.cpp:52) through

@@ -25,7 +25,13 @@ EXPORTS = [
     "dsac_backward_dsac_pose_device", "dsac_gather_patches_device", "dsac_coords_from_prediction_device", "dsac_kabsch",
     "dsac_stochastic_subsample",
     "dsac_synth_frames", "dsac_version",
+    "dsac_default_rgbd_camera", "dsac_register_depth_device", "dsac_obj_coords_device", "dsac_obj_rng_init_device",
+    "dsac_obj_draw_device", "dsac_gather_patches_at_device", "dsac_shuffle_permutation",
 ]
+
+ST_OBJ_DRAW_EXHAUSTED = 8    # DSAC_ST_OBJ_DRAW_EXHAUSTED
+ST_DEPTH_DROPPED = 16        # DSAC_ST_DEPTH_DROPPED
+OBJ_STATE_WORDS = 625        # one ThreadRand stream: std::mt19937's 624 words and its position
 
 
 class Config(C.Structure):
@@ -37,6 +43,39 @@ class Config(C.Structure):
         ("fix_q4", C.c_int32), ("grad_clamp", C.c_double),
         ("write_diffmaps", C.c_int32), ("device", C.c_int32), ("max_frames", C.c_int32), ("hyps_per_cta", C.c_int32),
     ]
+
+
+class RGBDCamera(C.Structure):
+    """dsac_rgbd_camera: the RGB camera, the depth camera, sensorTrans (row-major 4x4), rawData and the frame size."""
+    _fields_ = [
+        ("focal", C.c_float), ("x_shift", C.c_float), ("y_shift", C.c_float),
+        ("secondary_focal", C.c_float), ("raw_x_shift", C.c_float), ("raw_y_shift", C.c_float),
+        ("sensor_trans", C.c_double * 16), ("raw_data", C.c_int32), ("width", C.c_int32), ("height", C.c_int32),
+    ]
+
+
+def default_rgbd_camera(**kw):
+    """dsac_default_rgbd_camera with fields overridden by keyword (sensor_trans: any 4x4 / 16-element array)."""
+    cam = RGBDCamera()
+    rc = load().dsac_default_rgbd_camera(C.byref(cam))
+    assert rc == 0
+    for k, v in kw.items():
+        if k == "sensor_trans":
+            v = np.asarray(v, np.float64).reshape(16)
+            for i in range(16):
+                cam.sensor_trans[i] = float(v[i])
+        else:
+            setattr(cam, k, v)
+    return cam
+
+
+def shuffle_permutation(n, seed=5489):
+    """dsac_shuffle_permutation: std::shuffle(iota(n), std::mt19937(seed)), libstdc++'s permutation."""
+    out = np.empty(n, np.int32)
+    rc = load().dsac_shuffle_permutation(n, seed, _p(out))
+    if rc != 0:
+        raise ValueError("dsac_shuffle_permutation: bad arguments")
+    return out
 
 
 _OUT_FIELDS = ["hyp_pose", "img_idx", "cand_idx", "scores", "sf", "diffmaps", "entropy", "avg_pose", "ref_pose",
@@ -136,6 +175,18 @@ def load(build_if_missing=True):
     lib.dsac_synth_frames.argtypes = [C.c_uint32, C.c_uint32, C.c_int32, C.c_int64, C.c_int32, C.c_double, C.c_double,
                                       C.c_int32, C.c_double, C.c_double, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p]
+    lib.dsac_default_rgbd_camera.argtypes = [C.POINTER(RGBDCamera)]
+    lib.dsac_register_depth_device.argtypes = [C.c_void_p, C.POINTER(RGBDCamera), C.c_int32, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.dsac_obj_coords_device.argtypes = [C.c_void_p, C.POINTER(RGBDCamera), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.dsac_obj_rng_init_device.argtypes = [C.c_void_p, C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.dsac_obj_draw_device.argtypes = [C.c_void_p, C.POINTER(RGBDCamera), C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
+                                         C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p]
+    lib.dsac_gather_patches_at_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                                  C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.dsac_shuffle_permutation.argtypes = [C.c_int32, C.c_uint32, C.c_void_p]
     _lib = lib
     return lib
 
@@ -494,3 +545,41 @@ class Engine:
         t = np.zeros((n, 3))
         self._check(self.lib.dsac_kabsch(self.h, n, m, _p(a), _p(b), _p(R), _p(t)))
         return R.reshape(n, 3, 3), t
+
+    # ------------------------------------------------------------------ coordinate-CNN pre-training data path
+    # Raw device pointers as ints; `cam` is an RGBDCamera; stream: a cudaStream_t as int or None.
+
+    def register_depth_device(self, cam, n, d_raw, d_depth, d_dropped=None, d_status=None, stream=None):
+        """dsac_register_depth_device: raw depth [n][H][W] uint16 -> depth registered to the RGB camera."""
+        self._check(self.lib.dsac_register_depth_device(self.h, C.byref(cam), n, C.c_void_p(d_raw), C.c_void_p(d_depth),
+                                                        C.c_void_p(d_dropped) if d_dropped else None,
+                                                        C.c_void_p(d_status) if d_status else None,
+                                                        C.c_void_p(stream) if stream else None))
+
+    def obj_coords_device(self, cam, n_frames, n, d_depth, d_poses, d_coords, d_idx=None, stream=None):
+        """dsac_obj_coords_device: getObj images [n][H][W][3] int16 (mm) of frames d_idx[0..n) (None: 0..n) of a
+        dataset of n_frames frames."""
+        self._check(self.lib.dsac_obj_coords_device(self.h, C.byref(cam), n_frames, n, C.c_void_p(d_idx) if d_idx else None,
+                                                    C.c_void_p(d_depth), C.c_void_p(d_poses), C.c_void_p(d_coords),
+                                                    C.c_void_p(stream) if stream else None))
+
+    def obj_rng_init_device(self, seed, n_streams, d_state, stream=None):
+        """dsac_obj_rng_init_device: ThreadRand::init(seed) for n_streams threads into d_state [n_streams][625] uint32."""
+        self._check(self.lib.dsac_obj_rng_init_device(self.h, C.c_uint32(seed), n_streams, C.c_void_p(d_state),
+                                                      C.c_void_p(stream) if stream else None))
+
+    def obj_draw_device(self, cam, n_frames, d_depth, d_poses, n_images, n_patches, n_streams, max_attempts, d_state,
+                        d_img, d_centre, d_label, d_status, stream=None):
+        """dsac_obj_draw_device: one round of assembleData's draw."""
+        self._check(self.lib.dsac_obj_draw_device(self.h, C.byref(cam), n_frames, C.c_void_p(d_depth), C.c_void_p(d_poses),
+                                                  n_images, n_patches, n_streams, max_attempts, C.c_void_p(d_state),
+                                                  C.c_void_p(d_img), C.c_void_p(d_centre), C.c_void_p(d_label),
+                                                  C.c_void_p(d_status), C.c_void_p(stream) if stream else None))
+
+    def gather_patches_at_device(self, n, d_frames, n_frames, width, height, d_frame, d_centre, d_patches, mean=127.0,
+                                 d_status=None, stream=None):
+        """dsac_gather_patches_at_device: patches [n][3][42][42] around listed (frame, x, y) of device-resident frames."""
+        self._check(self.lib.dsac_gather_patches_at_device(self.h, n, C.c_void_p(d_frames), n_frames, width, height,
+                                                           C.c_void_p(d_frame), C.c_void_p(d_centre), C.c_float(mean),
+                                                           C.c_void_p(d_patches), C.c_void_p(d_status) if d_status else None,
+                                                           C.c_void_p(stream) if stream else None))

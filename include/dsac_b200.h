@@ -45,6 +45,8 @@ extern "C" {
 #define DSAC_ST_SAMPLER_EXHAUSTED 1u      /* max_candidates reached before n_hyps accepts */
 #define DSAC_ST_BORDER_PATCH 4u           /* dsac_gather_patches_device met a border cell (the reference would skip it, cnn_softam.h:236-240) */
 #define DSAC_ST_REFINE_ABORTED 2u         /* refinement stopped early (<50 inliers / NaN), cnn_softam.h:1136,1147 */
+#define DSAC_ST_OBJ_DRAW_EXHAUSTED 8u     /* dsac_obj_draw_device: a patch found no valid centre within max_attempts */
+#define DSAC_ST_DEPTH_DROPPED 16u         /* dsac_register_depth_device: registration targets outside the image were dropped */
 
 typedef struct dsac_engine dsac_engine;
 
@@ -324,6 +326,56 @@ int dsac_stochastic_subsample(uint32_t seed, int32_t width, int32_t height, int3
 int dsac_synth_frames(uint32_t data_seed, uint32_t sampler_seed, int32_t n_streams, int64_t frame0, int32_t n_frames,
                       double rho, double sigma, int32_t traj, double focal, double cx, double cy, int16_t* coords,
                       int32_t* pix, double* gt_cv /* [n][6] */, double* gt_jp /* [n][12] */);
+
+/* Pre-training of the coordinate CNN (train_obj.cpp): the data path on the device.  All pointers are DEVICE pointers
+ * except the camera; `stream` is a cudaStream_t (NULL: default stream).
+ *
+ * The RGB-D camera of jp::Dataset (properties.h dP): the RGB camera (focal, x_shift, y_shift; the principal point is
+ * width / 2.f + x_shift in float, so the shifts are kept apart from a cx), the depth camera (secondary_focal,
+ * raw_x_shift, raw_y_shift), sensor_trans (row-major 4x4, depth -> RGB, the file sensorTrans.dat), raw_data (1:
+ * depth is registered to the RGB camera, dataset.h:180-202) and the frame size. */
+typedef struct dsac_rgbd_camera {
+    float focal, x_shift, y_shift;
+    float secondary_focal, raw_x_shift, raw_y_shift;
+    double sensor_trans[16];
+    int32_t raw_data, width, height;
+} dsac_rgbd_camera;
+/* The reference's defaults, which the shipped 7-Scenes default.config repeats: focal 525, secondary focal 585, no shifts,
+ * raw_data 1, 640 x 480; sensor_trans identity (the reference's value when sensorTrans.dat is absent). */
+int dsac_default_rgbd_camera(dsac_rgbd_camera* cam);
+/* getDepth for n frames: raw [n][H][W] uint16 -> depth [n][H][W] uint16 (raw_data 0: a copy).  Where several depth
+ * pixels land on one RGB pixel the last in the reference's order (x outer, y inner) wins.  Targets outside the image are
+ * dropped; dropped [n] (nullable) counts them and status [n] (nullable; needs dropped) gets DSAC_ST_DEPTH_DROPPED.
+ * With raw_data the scatter uses a per-pixel buffer the engine owns and grows on demand (growing frees the old one,
+ * which waits for the device): registrations on one engine must be issued on one stream at a time, as its forward
+ * passes are; use one engine per concurrent stream. */
+int dsac_register_depth_device(dsac_engine* e, const dsac_rgbd_camera* cam, int32_t n_frames, const uint16_t* d_raw,
+                               uint16_t* d_depth, int32_t* d_dropped, uint32_t* d_status, void* stream);
+/* getObj: registered depth [n_frames][H][W] and jp poses [n_frames][12] (dsac_forward's gt_jp: row-major rotation,
+ * translation in mm; taken through float as jp::info_t holds it) -> int16 scene coordinates [n][H][W][3] in mm of
+ * frames idx[0..n) (idx NULL: frames 0..n, n <= n_frames).  A listed index outside [0, n_frames) gives a zero image. */
+int dsac_obj_coords_device(dsac_engine* e, const dsac_rgbd_camera* cam, int32_t n_frames, int32_t n, const int32_t* d_idx,
+                           const uint16_t* d_depth, const double* d_poses, int16_t* d_coords, void* stream);
+/* ThreadRand::init(seed) for n_streams threads: state [n_streams][625] = std::mt19937(seed + t) words and position. */
+int dsac_obj_rng_init_device(dsac_engine* e, uint32_t seed, int32_t n_streams, uint32_t* d_state, void* stream);
+/* assembleData's draw (train_obj.cpp:47-102) over n_streams OpenMP threads: image i (of n_images, static schedule) draws
+ * its frame from [0, n_frames), then n_patches centres (x, y) whose getObj label is nonzero.  Writes img [n_images *
+ * n_patches], centre [..][2], label [..][3] (metres, Vec3f /= 1000) and status [n_images].  state is read and advanced,
+ * so consecutive calls continue like the reference's rounds.  A patch not found within max_attempts (>= 32) pairs ends
+ * its image: the remaining centres are (-1, -1) and status gets DSAC_ST_OBJ_DRAW_EXHAUSTED.  The frame must exceed 42 px
+ * in both dimensions. */
+int dsac_obj_draw_device(dsac_engine* e, const dsac_rgbd_camera* cam, int32_t n_frames, const uint16_t* d_depth,
+                         const double* d_poses, int32_t n_images, int32_t n_patches, int32_t n_streams,
+                         int32_t max_attempts, uint32_t* d_state, int32_t* d_img, int32_t* d_centre, float* d_label,
+                         uint32_t* d_status, void* stream);
+/* dsac_gather_patches_device at listed centres: patch k = frames[frame[k]] around centre[k] = (x, y), minus mean,
+ * [n][3][42][42].  A centre whose patch leaves the frame, or a frame index outside [0, n_frames), yields a zero patch and
+ * DSAC_ST_BORDER_PATCH in status[0] (nullable). */
+int dsac_gather_patches_at_device(dsac_engine* e, int32_t n, const uint8_t* d_frames, int32_t n_frames, int32_t width,
+                                  int32_t height, const int32_t* d_frame, const int32_t* d_centre, float mean,
+                                  float* d_patches, uint32_t* d_status, void* stream);
+/* train_obj.cpp:266-270: out = std::shuffle(iota(n), std::mt19937(seed)); the reference uses seed 5489 (default). */
+int dsac_shuffle_permutation(int32_t n, uint32_t seed, int32_t* out);
 
 const char* dsac_version(void);
 
