@@ -79,7 +79,7 @@ __device__ void dloss_max_dev(const double est[6], const double gt[6], double ja
     for (int i = 0; i < 3; i++)
         for (int k = 0; k < 3; k++) diag += rot1[i * 3 + k] * rot2[i * 3 + k];
     double trace = fmin(3.0, fmax(-1.0, diag));
-    double rotErr = 180 * acos((trace - 1.0) / 2.0) / kPi;
+    double rotErr = rot_err_deg(trace);
     double a1[3] = {-est[3] / 10, -est[4] / 10, -est[5] / 10}, a2[3] = {-gt[3] / 10, -gt[4] / 10, -gt[5] / 10};
     double invT1[3], invT2[3];
     for (int r = 0; r < 3; r++) {  // invRot = rot^T

@@ -24,6 +24,7 @@
 #include "train.cuh"
 #include "upstream.cuh"
 #include "objtrain.cuh"
+#include "scoretrain.cuh"
 
 using namespace dsac;
 
@@ -1517,6 +1518,52 @@ int dsac_gather_patches_at_device(dsac_engine* e, int32_t n, const uint8_t* d_fr
     p.frame = d_frame; p.centre = d_centre; p.mean = mean; p.patches = d_patches; p.status = d_status;
     if (d_status) CU(cudaMemsetAsync(d_status, 0, sizeof(uint32_t), stream));
     k_gather_patches_at<<<n, UP_THREADS, 0, stream>>>(p);
+    e->launches++;
+    CU(cudaGetLastError());
+    return DSAC_OK;
+}
+
+// ----------------------------------------------------------------------------- score-CNN pre-training data path
+
+int dsac_score_draw_device(dsac_engine* e, int32_t n_frames, int32_t width, int32_t height, int32_t n_images,
+                           int32_t hyps_per_image, int32_t n_streams, uint32_t* d_state, int32_t* d_img, int32_t* d_pix,
+                           int32_t* d_drift, double* d_noise, void* stream_v) {
+    if (!e) return DSAC_ERR_ARG;
+    if (n_frames < 1 || n_images < 1 || hyps_per_image < 1 || n_streams < 1 || !d_state || !d_img || !d_pix || !d_drift ||
+        !d_noise)
+        return fail(e, DSAC_ERR_ARG, "dsac_score_draw_device: bad arguments");
+    ScoreDrawParams p;
+    if (width <= UP_PATCH || height <= UP_PATCH)
+        return fail(e, DSAC_ERR_ARG, "a %dx%d frame holds no %d-pixel patch centre", width, height, UP_PATCH);
+    p.nx = score_grid_bounds(width, p.xb, SCORE_GRID_MAX);
+    p.ny = score_grid_bounds(height, p.yb, SCORE_GRID_MAX);
+    // below 83 px the loop runs more than 40 times and the reference writes past its 40x40 sampling grid
+    if (p.nx != DSAC_GRID || p.ny != DSAC_GRID)
+        return fail(e, DSAC_ERR_ARG, "a %dx%d frame gives a %dx%d sampling loop (40x40 needed: 83 px or more)", width,
+                    height, p.nx, p.ny);
+    CU(cudaSetDevice(e->cfg.device));
+    p.n_frames = n_frames; p.n_images = n_images; p.hyps = hyps_per_image; p.n_streams = n_streams;
+    p.state = d_state; p.img = d_img; p.pix = d_pix; p.drift = d_drift; p.noise = d_noise;
+    k_score_draw<<<grid_of(n_streams, OBJ_DRAW_WARPS), 32 * OBJ_DRAW_WARPS, 0, (cudaStream_t)stream_v>>>(p);
+    e->launches++;
+    CU(cudaGetLastError());
+    return DSAC_OK;
+}
+
+int dsac_score_maps_device(dsac_engine* e, int32_t n_images, int32_t hyps_per_image, const int32_t* d_img,
+                           const double* d_gt_jp, const int16_t* d_coords, const int32_t* d_pix, const double* d_noise,
+                           float temperature, float* d_maps, double* d_labels, int32_t* d_correct, void* stream_v) {
+    if (!e) return DSAC_ERR_ARG;
+    if (n_images < 1 || hyps_per_image < 1 || (int64_t)n_images * hyps_per_image > INT32_MAX || !d_img || !d_gt_jp ||
+        !d_coords || !d_pix || !d_noise || !d_maps || !d_labels)
+        return fail(e, DSAC_ERR_ARG, "dsac_score_maps_device: bad arguments");
+    CU(cudaSetDevice(e->cfg.device));
+    ScoreMapsParams p;
+    p.img = d_img; p.gt_jp = d_gt_jp; p.coords = d_coords; p.pix = d_pix; p.noise = d_noise;
+    p.hyps = hyps_per_image;
+    p.f = e->cfg.focal; p.cxf = (float)e->cfg.cx; p.cyf = (float)e->cfg.cy; p.temperature = temperature;
+    p.maps = d_maps; p.labels = d_labels; p.correct = d_correct;
+    k_score_maps<<<(unsigned)(n_images * hyps_per_image), SM_THREADS, 0, (cudaStream_t)stream_v>>>(p);
     e->launches++;
     CU(cudaGetLastError());
     return DSAC_OK;

@@ -66,6 +66,22 @@ int dsac_shuffle_permutation(int32_t n, uint32_t seed, int32_t* out) {
     return DSAC_OK;
 }
 
+// train_score.cpp:286,381-384: one std::mt19937(seed) that continues across the training rounds, each round a
+// std::shuffle of a fresh iota(n).  Writes the permutations of rounds first_round .. first_round + n_rounds - 1,
+// replaying the earlier rounds from the seed.
+int dsac_shuffle_permutations(int32_t n, uint32_t seed, int32_t first_round, int32_t n_rounds, int32_t* out) {
+    if (n < 1 || first_round < 0 || n_rounds < 1 || !out) return DSAC_ERR_ARG;
+    std::mt19937 gen(seed);
+    std::vector<int> v((size_t)n);
+    for (int32_t r = 0; r < first_round + n_rounds; r++) {
+        for (int i = 0; i < n; i++) v[(size_t)i] = i;
+        std::shuffle(v.begin(), v.end(), gen);
+        if (r >= first_round)
+            for (int i = 0; i < n; i++) out[(size_t)(r - first_round) * n + i] = v[(size_t)i];
+    }
+    return DSAC_OK;
+}
+
 // stochasticSubSample (cnn_softam.h:283-309; targetSize 40, patchSize 42) drawing from the
 // thread-0 generator of ThreadRand (mt19937 seeded `seed`, thread_rand.cpp:52) through
 // fresh uniform_real_distribution<double> objects (drand, thread_rand.cpp:71-81).

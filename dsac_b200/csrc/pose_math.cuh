@@ -84,6 +84,13 @@ DSAC_HD void rodrigues_m2v(const double R[9], double r[3]) {
     }
 }
 
+// The angle (degrees) of a relative rotation from its trace, as maxloss.h and Hypothesis::calcAngularDistance compute
+// it: the trace clamped to [-1, 3], then 180 acos((trace - 1) / 2) / pi.
+DSAC_HD double rot_err_deg(double trace) {
+    trace = fmin(3.0, fmax(-1.0, trace));
+    return 180 * acos((trace - 1.0) / 2.0) / kPi;
+}
+
 // cv::projectPoints for one point, zero distortion (double arithmetic, z==0 -> 1).
 DSAC_HD void project_point(const double R[9], const double t[3], double X, double Y, double Z, double f, double cx,
                            double cy, double* u, double* v) {

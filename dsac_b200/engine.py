@@ -27,6 +27,7 @@ EXPORTS = [
     "dsac_synth_frames", "dsac_version",
     "dsac_default_rgbd_camera", "dsac_register_depth_device", "dsac_obj_coords_device", "dsac_obj_rng_init_device",
     "dsac_obj_draw_device", "dsac_gather_patches_at_device", "dsac_shuffle_permutation",
+    "dsac_score_draw_device", "dsac_score_maps_device", "dsac_shuffle_permutations",
 ]
 
 ST_OBJ_DRAW_EXHAUSTED = 8    # DSAC_ST_OBJ_DRAW_EXHAUSTED
@@ -75,6 +76,16 @@ def shuffle_permutation(n, seed=5489):
     rc = load().dsac_shuffle_permutation(n, seed, _p(out))
     if rc != 0:
         raise ValueError("dsac_shuffle_permutation: bad arguments")
+    return out
+
+
+def shuffle_permutations(n, seed=5489, first_round=0, n_rounds=1):
+    """dsac_shuffle_permutations: [n_rounds][n], the permutations of rounds first_round .. of one continuing
+    std::mt19937(seed), each a std::shuffle of a fresh iota(n) (train_score.cpp's batch order)."""
+    out = np.empty((n_rounds, n), np.int32)
+    rc = load().dsac_shuffle_permutations(n, seed, first_round, n_rounds, _p(out))
+    if rc != 0:
+        raise ValueError("dsac_shuffle_permutations: bad arguments")
     return out
 
 
@@ -187,6 +198,11 @@ def load(build_if_missing=True):
     lib.dsac_gather_patches_at_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                                   C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.dsac_shuffle_permutation.argtypes = [C.c_int32, C.c_uint32, C.c_void_p]
+    lib.dsac_score_draw_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.dsac_score_maps_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.dsac_shuffle_permutations.argtypes = [C.c_int32, C.c_uint32, C.c_int32, C.c_int32, C.c_void_p]
     _lib = lib
     return lib
 
@@ -583,3 +599,24 @@ class Engine:
                                                            C.c_void_p(d_frame), C.c_void_p(d_centre), C.c_float(mean),
                                                            C.c_void_p(d_patches), C.c_void_p(d_status) if d_status else None,
                                                            C.c_void_p(stream) if stream else None))
+
+    # ------------------------------------------------------------------ score-CNN pre-training data path
+
+    def score_draw_device(self, n_frames, width, height, n_images, hyps_per_image, n_streams, d_state, d_img, d_pix,
+                          d_drift, d_noise, stream=None):
+        """dsac_score_draw_device: one round of train_score.cpp's assembleData draw (frames, grids, drift levels and
+        getRandHyp vectors) on ThreadRand state d_state [n_streams][625]."""
+        self._check(self.lib.dsac_score_draw_device(self.h, n_frames, width, height, n_images, hyps_per_image, n_streams,
+                                                    C.c_void_p(d_state), C.c_void_p(d_img), C.c_void_p(d_pix),
+                                                    C.c_void_p(d_drift), C.c_void_p(d_noise),
+                                                    C.c_void_p(stream) if stream else None))
+
+    def score_maps_device(self, n_images, hyps_per_image, d_img, d_gt_jp, d_coords, d_pix, d_noise, temperature, d_maps,
+                          d_labels, d_correct=None, stream=None):
+        """dsac_score_maps_device: reprojection-error images [n][1600], labels [n] and the 5 deg / 50 mm flags of a
+        draw's perturbed ground-truth poses against the coordinate CNN's grids."""
+        self._check(self.lib.dsac_score_maps_device(self.h, n_images, hyps_per_image, C.c_void_p(d_img), C.c_void_p(d_gt_jp),
+                                                    C.c_void_p(d_coords), C.c_void_p(d_pix), C.c_void_p(d_noise),
+                                                    C.c_float(temperature), C.c_void_p(d_maps), C.c_void_p(d_labels),
+                                                    C.c_void_p(d_correct) if d_correct else None,
+                                                    C.c_void_p(stream) if stream else None))

@@ -377,6 +377,31 @@ int dsac_gather_patches_at_device(dsac_engine* e, int32_t n, const uint8_t* d_fr
 /* train_obj.cpp:266-270: out = std::shuffle(iota(n), std::mt19937(seed)); the reference uses seed 5489 (default). */
 int dsac_shuffle_permutation(int32_t n, uint32_t seed, int32_t* out);
 
+/* Pre-training of the score CNN (train_score.cpp): the data path on the device.  Pointers are DEVICE pointers;
+ * `stream` is a cudaStream_t (NULL: default stream).
+ *
+ * assembleData's draw over n_streams OpenMP threads on ThreadRand state [n_streams][625] (dsac_obj_rng_init_device),
+ * read and advanced so that consecutive calls continue like the reference's rounds.  Per image i: stream 0 draws the
+ * frame img[i] from [0, n_frames) and the sampling grid pix [i][1600][2] of a width x height frame (stochasticSubSample,
+ * cell y * 40 + x); then hypothesis h (static schedule over the streams) draws drift [i * hyps + h] (0: small, 1: large
+ * pose error) and getRandHyp's 6-vector noise [i * hyps + h][6] (rotation vector in radians, translation in mm).  The
+ * frame must be at least 83 px in both dimensions, where stochasticSubSample's loop runs exactly 40 times per axis
+ * (below that the reference writes past its sampling grid). */
+int dsac_score_draw_device(dsac_engine* e, int32_t n_frames, int32_t width, int32_t height, int32_t n_images,
+                           int32_t hyps_per_image, int32_t n_streams, uint32_t* d_state, int32_t* d_img, int32_t* d_pix,
+                           int32_t* d_drift, double* d_noise, void* stream);
+/* The training samples of a draw: pose k = i * hyps + h is poseGT(gt_jp[img[i]]) * Hypothesis(noise[k]); maps [k][1600]
+ * is its reprojection-error image against coords [i][1600][3] (mm, the coordinate CNN's grid at pix [i]) with the
+ * engine's camera (config focal / cx / cy), clamped at 100 and computed like the forward's diffmaps; labels [k] =
+ * -temperature * max(angular error in degrees, translation error in mm / 10); correct [k] (nullable) = 1 where the
+ * errors are below 5 degrees and 50 mm.  img must index gt_jp (as dsac_score_draw_device writes it). */
+int dsac_score_maps_device(dsac_engine* e, int32_t n_images, int32_t hyps_per_image, const int32_t* d_img,
+                           const double* d_gt_jp, const int16_t* d_coords, const int32_t* d_pix, const double* d_noise,
+                           float temperature, float* d_maps, double* d_labels, int32_t* d_correct, void* stream);
+/* train_score.cpp:286,381-384: out [n_rounds][n] = the permutations of rounds first_round .. of one continuing
+ * std::mt19937(seed), each round std::shuffle of a fresh iota(n); the reference uses seed 5489 (default). */
+int dsac_shuffle_permutations(int32_t n, uint32_t seed, int32_t first_round, int32_t n_rounds, int32_t* out);
+
 const char* dsac_version(void);
 
 #ifdef __cplusplus
