@@ -24,11 +24,9 @@ namespace dsac {
 constexpr int BW_MAX_OBJ_PIX = 16;                       // ceil(1600 / skip) with skip = 1/rSS = 100
 constexpr int BW_JOBS = 12 + BW_MAX_OBJ_PIX * 6;         // refine jobs per frame (dRefineHyp + dRefineObj)
 
+// Views into the engine's backward scratch block (dsac_engine::bw_buf); passed to the kernels by value, so it owns nothing.
 struct BackwardScratch {
-    void* buf = nullptr;
-    size_t bytes = 0;
     int n_cap = 0;
-    // carved from buf
     int32_t* job_frame = nullptr;    // [n][BW_JOBS]
     double* job_init = nullptr;      // [n][BW_JOBS][6]
     int32_t* job_pert = nullptr;     // [n][BW_JOBS][2]
@@ -46,10 +44,6 @@ struct BackwardScratch {
     double* part = nullptr;          // [n][groups][N*3] partial rows of k_dscore
     int groups = 1;
 };
-inline void backward_scratch_free(BackwardScratch* s) {
-    if (s->buf) cudaFree(s->buf);
-    *s = BackwardScratch();
-}
 
 // Hypothesis(cv2our(pose)).getRodVecAndTrans()  (Hypothesis.cpp:274-290)
 __device__ __forceinline__ void jp6_from_cv_dev(const double pose[6], double out[6]) {

@@ -30,6 +30,69 @@ using namespace dsac;
 
 static std::string g_create_error;
 
+// Owners of the engine's CUDA resources, the only code here that frees any.  Each releases what it holds in its
+// destructor, is move-only, and converts to the raw pointer or handle for use at call sites.
+template <typename T, cudaError_t (*Alloc)(void**, size_t), cudaError_t (*Free)(void*)>
+class Mem {
+  public:
+    Mem() = default;
+    Mem(Mem&& o) noexcept : p_(o.p_), bytes_(o.bytes_) { o.p_ = nullptr; o.bytes_ = 0; }
+    Mem& operator=(Mem&& o) noexcept { std::swap(p_, o.p_); std::swap(bytes_, o.bytes_); return *this; }
+    ~Mem() { release(); }
+    // Grow-only: a request beyond the capacity frees the old block before it allocates the new one (the contents are not
+    // kept, and a block of gigabytes is never held twice), with a quarter more with `headroom`.  On failure the buffer is
+    // empty and the CUDA error is returned.
+    cudaError_t reserve(size_t bytes, bool headroom = false) {
+        if (bytes <= bytes_) return cudaSuccess;
+        release();
+        const size_t cap = headroom ? bytes + bytes / 4 : bytes;
+        void* p = nullptr;
+        const cudaError_t st = Alloc(&p, cap);
+        if (st != cudaSuccess) return st;
+        p_ = static_cast<T*>(p);
+        bytes_ = cap;
+        return cudaSuccess;
+    }
+    operator T*() const { return p_; }
+    T* get() const { return p_; }
+    size_t bytes() const { return bytes_; }
+
+  private:
+    void release() {
+        if (p_) Free(p_);
+        p_ = nullptr;
+        bytes_ = 0;
+    }
+    T* p_ = nullptr;
+    size_t bytes_ = 0;
+};
+template <typename T> using DevMem = Mem<T, cudaMalloc, cudaFree>;
+template <typename T> using PinnedMem = Mem<T, cudaMallocHost, cudaFreeHost>;
+
+template <typename H, cudaError_t (*Destroy)(H)>
+class Handle {
+  public:
+    Handle() = default;
+    Handle(Handle&& o) noexcept : h_(o.h_) { o.h_ = nullptr; }
+    Handle& operator=(Handle&& o) noexcept { std::swap(h_, o.h_); return *this; }
+    ~Handle() { release(); }
+    // where a cudaStreamCreate* / cudaEventCreate* call writes the new handle (what the owner held is released first)
+    H* put() {
+        release();
+        return &h_;
+    }
+    operator H() const { return h_; }
+
+  private:
+    void release() {
+        if (h_) Destroy(h_);
+        h_ = nullptr;
+    }
+    H h_ = nullptr;
+};
+using Stream = Handle<cudaStream_t, cudaStreamDestroy>;
+using Event = Handle<cudaEvent_t, cudaEventDestroy>;
+
 struct dsac_engine {
     dsac_config cfg;
     std::string err;
@@ -39,18 +102,15 @@ struct dsac_engine {
     void* hook_user = nullptr;
     dsac_score_backward_hook bw_hook = nullptr;
     void* bw_hook_user = nullptr;
-    double* d_ext_g = nullptr;      // [n][H][N] dScore/dDiffMap from the backward hook (grow-only)
-    size_t ext_g_count = 0;
-    cudaEvent_t ev_fwd = nullptr;   // recorded after the last forward launch: the backward waits on it
-    double* d_kabsch = nullptr;     // dsac_kabsch: inputs and outputs in one grow-only block
-    size_t kabsch_bytes = 0;
-    uint64_t* d_reg_keys = nullptr; // dsac_register_depth_device: per-pixel scatter keys, grow-only
-    size_t reg_keys_bytes = 0;
+    DevMem<double> d_ext_g;         // [n][H][N] dScore/dDiffMap from the backward hook, then its clamped input [n][H] (grow-only)
+    Event ev_fwd;                   // recorded after the last forward launch: the backward waits on it
+    DevMem<double> d_kabsch;        // dsac_kabsch: inputs and outputs in one grow-only block
+    DevMem<uint64_t> d_reg_keys;    // dsac_register_depth_device: per-pixel scatter keys, grow-only
     int sm_count = 132;
     // inputs (device copies for the host-buffer entry point)
-    int16_t* d_coords = nullptr;
-    int32_t* d_pix = nullptr;
-    double* d_gt = nullptr;
+    DevMem<int16_t> d_coords;
+    DevMem<int32_t> d_pix;
+    DevMem<double> d_gt;
     // last-call input views (device), used by fetch / backward
     const int16_t* cur_coords = nullptr;
     const int32_t* cur_pix = nullptr;
@@ -61,49 +121,50 @@ struct dsac_engine {
     int dsac_n = 0;                 // frames of the last dsac_forward_dsac (0: none), for dsac_backward_dsac
     long long cur_frame0 = 0;
     // state
-    uint16_t* d_perm = nullptr;
-    double* d_hyp_pose = nullptr;
-    float* d_hyp_P = nullptr;
-    int32_t* d_img_idx = nullptr;
-    int32_t* d_cand_idx = nullptr;
-    long long* d_stream_ncand = nullptr;
-    unsigned long long* d_stream_endpos = nullptr;
-    // refine-all (DSAC variant) buffers, allocated on first use
-    int32_t* d_ra_frame = nullptr; double* d_ra_pose = nullptr; double* d_ra_loss = nullptr; double* d_ra_rot = nullptr;
-    double* d_ra_t = nullptr; int32_t* d_ra_correct = nullptr; int32_t* d_ra_steps = nullptr; int32_t* d_ra_imap = nullptr;
-    size_t ra_jobs = 0, ra_imap_jobs = 0;
+    DevMem<uint16_t> d_perm;
+    DevMem<double> d_hyp_pose;
+    DevMem<float> d_hyp_P;
+    DevMem<int32_t> d_img_idx;
+    DevMem<int32_t> d_cand_idx;
+    DevMem<long long> d_stream_ncand;
+    DevMem<unsigned long long> d_stream_endpos;
+    // refine-all (DSAC variant) buffers, grown on use; d_ra_frame holds the job -> frame table for ra_jobs jobs
+    DevMem<int32_t> d_ra_frame; DevMem<double> d_ra_pose, d_ra_loss, d_ra_rot, d_ra_t;
+    DevMem<int32_t> d_ra_correct, d_ra_steps, d_ra_imap;
+    size_t ra_jobs = 0;
     // per-frame results of k_dsac_draw: drawn hypothesis, expected loss, its errors
-    int32_t* d_dsac_pick = nullptr; double* d_dsac_exp = nullptr; double* d_dsac_rot = nullptr; double* d_dsac_terr = nullptr;
-    int32_t* d_dsac_correct = nullptr;
-    int32_t* h_totals = nullptr;    // pinned [2]: selected hypotheses and refinement jobs of dsac_backward_dsac_device
-    uint32_t* d_status = nullptr;
-    unsigned long long* d_fragile = nullptr;
-    unsigned long long* d_phase = nullptr;   // K1 per-phase cycle counters (DSAC_K1_TIMERS=1), else null
-    float* d_diffmaps = nullptr;
-    double* d_scores = nullptr;
-    double* d_sf = nullptr;
-    double* d_entropy = nullptr;
-    double* d_avg = nullptr;
-    double* d_ref = nullptr;
-    int32_t* d_inlier_map = nullptr;
-    int32_t* d_steps_done = nullptr;
-    int32_t* d_n_perm = nullptr;
-    double* d_loss = nullptr;
-    double* d_rot_err = nullptr;
-    double* d_t_err = nullptr;
-    int32_t* d_correct = nullptr;
-    unsigned int* d_frame_counter = nullptr;
-    long long* h_stream_ncand = nullptr;   // [max_frames][n_streams], pinned (so that a submitted pass stays asynchronous)
+    DevMem<int32_t> d_dsac_pick; DevMem<double> d_dsac_exp, d_dsac_rot, d_dsac_terr;
+    DevMem<int32_t> d_dsac_correct;
+    PinnedMem<int32_t> h_totals;    // [2]: selected hypotheses and refinement jobs of dsac_backward_dsac_device
+    DevMem<uint32_t> d_status;
+    DevMem<unsigned long long> d_fragile;
+    DevMem<unsigned long long> d_phase;   // K1 per-phase cycle counters (DSAC_K1_TIMERS=1), else null
+    DevMem<float> d_diffmaps;
+    DevMem<double> d_scores;
+    DevMem<double> d_sf;
+    DevMem<double> d_entropy;
+    DevMem<double> d_avg;
+    DevMem<double> d_ref;
+    DevMem<int32_t> d_inlier_map;
+    DevMem<int32_t> d_steps_done;
+    DevMem<int32_t> d_n_perm;
+    DevMem<double> d_loss;
+    DevMem<double> d_rot_err;
+    DevMem<double> d_t_err;
+    DevMem<int32_t> d_correct;
+    DevMem<unsigned int> d_frame_counter;
+    PinnedMem<long long> h_stream_ncand;   // [max_frames][n_streams] (pinned, so that a submitted pass stays asynchronous)
     dsac_forward_out* pending_out = nullptr;   // results of a submitted, not yet awaited pass
     int pending_n = 0, pending_chunks = 0;
-    BackwardScratch bw;
-    std::vector<std::pair<void*, size_t>> bw_pool;   // device buffers of dsac_backward_dsac, kept across calls
-    cudaStream_t pipe[4] = {nullptr, nullptr, nullptr, nullptr};   // chunked H2D / compute / D2H pipeline of dsac_forward
+    BackwardScratch bw;             // views into bw_buf
+    DevMem<char> bw_buf;            // the soft-argmax backward's scratch block, grow-only
+    std::vector<DevMem<char>> bw_pool;   // device buffers of dsac_backward_dsac, kept across calls
+    Stream pipe[4];                 // chunked H2D / compute / D2H pipeline of dsac_forward
     // tail split (dsac_set_tail_split): the whole sampler waves of a batch run on a high-priority side stream, the
     // frames of the last, partial wave on the caller's stream, so that scoring / refinement of the first part fill
     // the SMs the partial wave leaves idle
-    cudaStream_t hi = nullptr;
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+    Stream hi;
+    Event ev_fork, ev_join;
     int tail_split = 1;
     // split sampler (sampler_split.cuh): per-stream state and round buffers, sized at creation
     int k1_mode = 1;                // 1: round-based pipeline of flat kernels; 0: monolithic k_sample (DSAC_K1_MODE=mono)
@@ -111,47 +172,47 @@ struct dsac_engine {
     bool k1_rounds_fixed = false;   // DSAC_K1_ROUNDS given
     int k1_filter_grid = 0, k1_solve_grid = 0;
     unsigned long long k1_calls = 0;
-    K1SlotState* d_k1_state = nullptr;
-    CellRec* d_k1_celltab = nullptr;
-    uint2* d_k1_cells = nullptr;
-    uint32_t* d_k1_endw = nullptr;
-    uint32_t* d_k1_accbits = nullptr;
-    double* d_k1_pose = nullptr;
-    uint2* d_k1_wq = nullptr;
-    uint32_t* d_k1_fq = nullptr;
-    int* d_k1_counters = nullptr;                 // wq_n[K1S_MAX_ROUNDS], fq_n[K1S_MAX_ROUNDS]
-    unsigned long long* d_k1_stats = nullptr;     // [2][2]: candidates / hypotheses of finished streams, by call parity
-    unsigned long long* d_k1_dbg = nullptr;       // [K1S_MAX_ROUNDS][4] (DSAC_K1_DEBUG=1 or dsac_sampler_profile), else null
+    DevMem<K1SlotState> d_k1_state;
+    DevMem<CellRec> d_k1_celltab;
+    DevMem<uint2> d_k1_cells;
+    DevMem<uint32_t> d_k1_endw;
+    DevMem<uint32_t> d_k1_accbits;
+    DevMem<double> d_k1_pose;
+    DevMem<uint2> d_k1_wq;
+    DevMem<uint32_t> d_k1_fq;
+    DevMem<int> d_k1_counters;                    // wq_n[K1S_MAX_ROUNDS], fq_n[K1S_MAX_ROUNDS]
+    DevMem<unsigned long long> d_k1_stats;        // [2][2]: candidates / hypotheses of finished streams, by call parity
+    DevMem<unsigned long long> d_k1_dbg;          // [K1S_MAX_ROUNDS][4] (DSAC_K1_DEBUG=1 or dsac_sampler_profile), else null
     // dsac_sampler_profile: CUDA events between the sampler's launches of the last forward pass
     int k1_profile = 0;
-    std::vector<cudaEvent_t> k1_ev;               // event i is recorded after launch i (event 0 before the first)
+    std::vector<Event> k1_ev;                     // event i is recorded after launch i (event 0 before the first)
     std::vector<int> k1_ev_kind;                  // 0 cells/slot (integer generation + selection), 1 filter, 2 solve, 3 resume tail
     int k1_ev_n = 0;
     // generator / filter overlap: k1_slot runs on the caller's stream, k1_filter + k1_solve on this side stream
-    cudaStream_t k1_side = nullptr;
-    cudaStream_t k1_side2 = nullptr;              // k1_solve, when it runs next to the following set's filter (overlap mode 2)
-    cudaEvent_t k1_ev_filt[K1S_MAX_SETS] = {};    // filter of launch set i done
-    cudaEvent_t k1_ev_solve[K1S_MAX_SETS] = {};   // solve of launch set i done
-    cudaEvent_t k1_ev_gen[K1S_MAX_SETS] = {};     // generation of launch set i done
-    cudaEvent_t k1_ev_round = nullptr;            // last solve of a round done
+    Stream k1_side;
+    Stream k1_side2;                              // k1_solve, when it runs next to the following set's filter (overlap mode 2)
+    Event k1_ev_filt[K1S_MAX_SETS];               // filter of launch set i done
+    Event k1_ev_solve[K1S_MAX_SETS];              // solve of launch set i done
+    Event k1_ev_gen[K1S_MAX_SETS];                // generation of launch set i done
+    Event k1_ev_round;                            // last solve of a round done
     // a second, independent set of the per-pass sampler resources: a large batch runs as two concurrent half-batches (forward_split)
     struct K1Lane {
-        cudaStream_t main = nullptr, side = nullptr, side2 = nullptr;
-        cudaEvent_t ev_filt[K1S_MAX_SETS] = {}, ev_solve[K1S_MAX_SETS] = {}, ev_gen[K1S_MAX_SETS] = {}, ev_round = nullptr;
-        int* counters = nullptr;
-        unsigned long long* stats = nullptr;
+        Stream main, side, side2;
+        Event ev_filt[K1S_MAX_SETS], ev_solve[K1S_MAX_SETS], ev_gen[K1S_MAX_SETS], ev_round;
+        DevMem<int> counters;
+        DevMem<unsigned long long> stats;
         unsigned long long calls = 0;
     } lane1;
     int k1_lanes = 1;                             // DSAC_K1_LANES: 0 = never split a batch into two lanes
     int k1_overlap = 1;
     bool k1_overlap_fixed = false;                // DSAC_K1_OVERLAP given
     int k1_solve_batch = 0;                       // 1: one k1_solve per round over the flagged candidates of all its launch sets (a per-set solve runs beside the next set's generator, a per-round one runs alone; on an H100 SXM at 700 W 3.05 vs 3.09 ms per 1024-frame step)
-    K1SlotState* d_k1_vstate = nullptr;           // k1_spec: virtual slots of the speculative first round (few streams)
-    uint2* d_k1_vcells = nullptr;
-    uint32_t* d_k1_vendw = nullptr;
-    int* d_k1_spec_result = nullptr;
-    int* d_k1_spec_table = nullptr;
-    uint32_t* d_k1_chain = nullptr;               // k1_pipe: hand-over records of the window chain, [slots][K1Q_MAX_WIN + 1][4]
+    DevMem<K1SlotState> d_k1_vstate;              // k1_spec: virtual slots of the speculative first round (few streams)
+    DevMem<uint2> d_k1_vcells;
+    DevMem<uint32_t> d_k1_vendw;
+    DevMem<int> d_k1_spec_result;
+    DevMem<int> d_k1_spec_table;
+    DevMem<uint32_t> d_k1_chain;                  // k1_pipe: hand-over records of the window chain, [slots][K1Q_MAX_WIN + 1][4]
     unsigned long long k1_epoch = 0;              // k1_pipe: one value per launch, engine-wide (a stale hand-over record never matches)
     int k1_pipe = 0;                              // DSAC_K1_PIPE=1: chained generator for 9 .. ~190 streams (experimental, off by default)
     int k1_slot_capacity = 0;                     // CTAs of k1_pipe / k1_slot (256 threads) the GPU holds at once
@@ -219,22 +280,17 @@ int dsac_engine_config(const dsac_engine* e, dsac_config* out) {
 void dsac_engine_destroy(dsac_engine* e) {
     if (!e) return;
     cudaSetDevice(e->cfg.device);
-    for (cudaStream_t st : e->pipe)
-        if (st) { cudaStreamSynchronize(st); cudaStreamDestroy(st); }
-    if (e->hi) { cudaStreamSynchronize(e->hi); cudaStreamDestroy(e->hi); }
-    if (e->ev_fork) cudaEventDestroy(e->ev_fork);
-    if (e->ev_join) cudaEventDestroy(e->ev_join);
-    if (e->ev_fwd) cudaEventDestroy(e->ev_fwd);
-    if (e->d_ext_g) cudaFree(e->d_ext_g);
-    if (e->d_kabsch) cudaFree(e->d_kabsch);
-    if (e->d_reg_keys) cudaFree(e->d_reg_keys);
+    // nothing is freed while work on the engine's streams may still use it
+    const cudaStream_t streams[] = {e->pipe[0], e->pipe[1], e->pipe[2], e->pipe[3], e->hi, e->k1_side, e->k1_side2,
+                                    e->lane1.main, e->lane1.side, e->lane1.side2};
+    for (cudaStream_t st : streams)
+        if (st) cudaStreamSynchronize(st);
     if (e->d_phase) {
         unsigned long long h[16];
         if (cudaMemcpy(h, e->d_phase, sizeof(h), cudaMemcpyDeviceToHost) == cudaSuccess)
             fprintf(stderr, "[dsac K1 thread-0 cycles] A1 gen %llu  A2 bounds %llu  B filter %llu  C queue %llu  D full %llu  E advance %llu\n"
                             "[dsac k1_slot thread-0 cycles] regenerate+decode %llu  scan %llu  walk %llu  starts %llu  write %llu  leftover %llu\n",
                     h[0], h[1], h[2], h[3], h[4], h[5], h[8], h[9], h[10], h[11], h[12], h[13]);
-        cudaFree(e->d_phase);
     }
     if (e->d_k1_dbg && e->d_k1_spec_result && e->k1_spec_slots > 0) {
         int h[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -249,42 +305,6 @@ void dsac_engine_destroy(dsac_engine* e) {
                 fprintf(stderr, "[dsac K1 split, last call] round %d: %llu active streams, %llu candidates, %llu flagged, %llu accepted\n", r,
                         h[r * 4], h[r * 4 + 1], h[r * 4 + 2], h[r * 4 + 3]);
     }
-    for (cudaEvent_t ev : e->k1_ev) cudaEventDestroy(ev);
-    if (e->k1_side) { cudaStreamSynchronize(e->k1_side); cudaStreamDestroy(e->k1_side); }
-    if (e->k1_side2) { cudaStreamSynchronize(e->k1_side2); cudaStreamDestroy(e->k1_side2); }
-    for (cudaEvent_t ev : e->k1_ev_filt) if (ev) cudaEventDestroy(ev);
-    for (cudaEvent_t ev : e->k1_ev_solve) if (ev) cudaEventDestroy(ev);
-    for (cudaEvent_t ev : e->k1_ev_gen) if (ev) cudaEventDestroy(ev);
-    if (e->k1_ev_round) cudaEventDestroy(e->k1_ev_round);
-    {
-        dsac_engine::K1Lane& L = e->lane1;
-        for (cudaStream_t st : {L.main, L.side, L.side2}) if (st) { cudaStreamSynchronize(st); cudaStreamDestroy(st); }
-        for (int i = 0; i < K1S_MAX_SETS; i++) {
-            if (L.ev_filt[i]) cudaEventDestroy(L.ev_filt[i]);
-            if (L.ev_solve[i]) cudaEventDestroy(L.ev_solve[i]);
-            if (L.ev_gen[i]) cudaEventDestroy(L.ev_gen[i]);
-        }
-        if (L.ev_round) cudaEventDestroy(L.ev_round);
-        if (L.counters) cudaFree(L.counters);
-        if (L.stats) cudaFree(L.stats);
-    }
-    void* k1ptrs[] = {e->d_k1_chain, e->d_k1_spec_table, e->d_k1_vstate, e->d_k1_vcells, e->d_k1_vendw, e->d_k1_spec_result, e->d_k1_state, e->d_k1_celltab, e->d_k1_cells, e->d_k1_endw, e->d_k1_accbits, e->d_k1_pose, e->d_k1_wq,
-                      e->d_k1_fq, e->d_k1_counters, e->d_k1_stats, e->d_k1_dbg};
-    for (void* p : k1ptrs)
-        if (p) cudaFree(p);
-    void* ptrs[] = {e->d_coords, e->d_pix, e->d_gt, e->d_perm, e->d_hyp_pose, e->d_hyp_P, e->d_img_idx, e->d_cand_idx,
-                    e->d_stream_ncand, e->d_stream_endpos, e->d_ra_frame, e->d_ra_pose, e->d_ra_loss, e->d_ra_rot, e->d_ra_t,
-                    e->d_ra_correct, e->d_ra_steps, e->d_ra_imap, e->d_status, e->d_fragile, e->d_diffmaps, e->d_scores, e->d_sf, e->d_entropy,
-                    e->d_avg, e->d_ref, e->d_inlier_map, e->d_steps_done, e->d_n_perm, e->d_loss, e->d_rot_err,
-                    e->d_t_err, e->d_correct, e->d_frame_counter, e->d_dsac_pick, e->d_dsac_exp, e->d_dsac_rot, e->d_dsac_terr,
-                    e->d_dsac_correct};
-    for (void* p : ptrs)
-        if (p) cudaFree(p);
-    if (e->h_stream_ncand) cudaFreeHost(e->h_stream_ncand);
-    if (e->h_totals) cudaFreeHost(e->h_totals);
-    backward_scratch_free(&e->bw);
-    for (auto& slot : e->bw_pool)
-        if (slot.first) cudaFree(slot.first);
     delete e;
 }
 
@@ -308,7 +328,7 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
     if (e->cfg.max_candidates <= 0) e->cfg.max_candidates = 1 << 20;
     auto bail = [&](int code) {
         g_create_error = e->err;
-        dsac_engine_destroy(e);
+        delete e;
         return code;
     };
 #define CUC(call)                                                                                   \
@@ -324,42 +344,42 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
     CUC(cudaGetDeviceProperties(&prop, cfg->device));
     e->sm_count = prop.multiProcessorCount;
     const size_t n = (size_t)cfg->max_frames, H = (size_t)cfg->n_hyps, N = DSAC_N;
-    CUC(cudaMalloc(&e->d_coords, n * N * 3 * sizeof(int16_t)));
-    CUC(cudaMalloc(&e->d_pix, n * N * 2 * sizeof(int32_t)));
-    CUC(cudaMalloc(&e->d_gt, n * 12 * sizeof(double)));
-    CUC(cudaMalloc(&e->d_perm, (size_t)std::max(1, cfg->ref_steps) * N * sizeof(uint16_t)));
-    CUC(cudaMalloc(&e->d_hyp_pose, n * H * 6 * sizeof(double)));
-    CUC(cudaMalloc(&e->d_hyp_P, n * H * 12 * sizeof(float)));
-    CUC(cudaMalloc(&e->d_img_idx, n * H * 4 * sizeof(int32_t)));
-    CUC(cudaMalloc(&e->d_cand_idx, n * H * sizeof(int32_t)));
-    CUC(cudaMalloc(&e->d_stream_ncand, n * cfg->n_streams * sizeof(long long)));
-    CUC(cudaMalloc(&e->d_stream_endpos, n * cfg->n_streams * sizeof(unsigned long long)));
-    CUC(cudaMalloc(&e->d_status, n * sizeof(uint32_t)));
-    CUC(cudaMalloc(&e->d_fragile, sizeof(unsigned long long)));
-    if (cfg->write_diffmaps) CUC(cudaMalloc(&e->d_diffmaps, n * H * N * sizeof(float)));
-    CUC(cudaMalloc(&e->d_scores, n * H * sizeof(double)));
-    CUC(cudaMalloc(&e->d_sf, n * H * sizeof(double)));
-    CUC(cudaMalloc(&e->d_entropy, n * sizeof(double)));
-    CUC(cudaMalloc(&e->d_avg, n * 6 * sizeof(double)));
-    CUC(cudaMalloc(&e->d_ref, n * 6 * sizeof(double)));
-    CUC(cudaMalloc(&e->d_inlier_map, n * N * sizeof(int32_t)));
-    CUC(cudaMalloc(&e->d_steps_done, n * sizeof(int32_t)));
-    CUC(cudaMalloc(&e->d_n_perm, n * sizeof(int32_t)));
-    CUC(cudaMalloc(&e->d_loss, n * sizeof(double)));
-    CUC(cudaMalloc(&e->d_rot_err, n * sizeof(double)));
-    CUC(cudaMalloc(&e->d_t_err, n * sizeof(double)));
-    CUC(cudaMalloc(&e->d_correct, n * sizeof(int32_t)));
-    CUC(cudaMalloc(&e->d_frame_counter, n * sizeof(unsigned int)));
-    CUC(cudaMalloc(&e->d_dsac_pick, n * sizeof(int32_t)));
-    CUC(cudaMalloc(&e->d_dsac_exp, n * sizeof(double)));
-    CUC(cudaMalloc(&e->d_dsac_rot, n * sizeof(double)));
-    CUC(cudaMalloc(&e->d_dsac_terr, n * sizeof(double)));
-    CUC(cudaMalloc(&e->d_dsac_correct, n * sizeof(int32_t)));
-    CUC(cudaMallocHost(&e->h_totals, 2 * sizeof(int32_t)));
+    CUC(e->d_coords.reserve(n * N * 3 * sizeof(int16_t)));
+    CUC(e->d_pix.reserve(n * N * 2 * sizeof(int32_t)));
+    CUC(e->d_gt.reserve(n * 12 * sizeof(double)));
+    CUC(e->d_perm.reserve((size_t)std::max(1, cfg->ref_steps) * N * sizeof(uint16_t)));
+    CUC(e->d_hyp_pose.reserve(n * H * 6 * sizeof(double)));
+    CUC(e->d_hyp_P.reserve(n * H * 12 * sizeof(float)));
+    CUC(e->d_img_idx.reserve(n * H * 4 * sizeof(int32_t)));
+    CUC(e->d_cand_idx.reserve(n * H * sizeof(int32_t)));
+    CUC(e->d_stream_ncand.reserve(n * cfg->n_streams * sizeof(long long)));
+    CUC(e->d_stream_endpos.reserve(n * cfg->n_streams * sizeof(unsigned long long)));
+    CUC(e->d_status.reserve(n * sizeof(uint32_t)));
+    CUC(e->d_fragile.reserve(sizeof(unsigned long long)));
+    if (cfg->write_diffmaps) CUC(e->d_diffmaps.reserve(n * H * N * sizeof(float)));
+    CUC(e->d_scores.reserve(n * H * sizeof(double)));
+    CUC(e->d_sf.reserve(n * H * sizeof(double)));
+    CUC(e->d_entropy.reserve(n * sizeof(double)));
+    CUC(e->d_avg.reserve(n * 6 * sizeof(double)));
+    CUC(e->d_ref.reserve(n * 6 * sizeof(double)));
+    CUC(e->d_inlier_map.reserve(n * N * sizeof(int32_t)));
+    CUC(e->d_steps_done.reserve(n * sizeof(int32_t)));
+    CUC(e->d_n_perm.reserve(n * sizeof(int32_t)));
+    CUC(e->d_loss.reserve(n * sizeof(double)));
+    CUC(e->d_rot_err.reserve(n * sizeof(double)));
+    CUC(e->d_t_err.reserve(n * sizeof(double)));
+    CUC(e->d_correct.reserve(n * sizeof(int32_t)));
+    CUC(e->d_frame_counter.reserve(n * sizeof(unsigned int)));
+    CUC(e->d_dsac_pick.reserve(n * sizeof(int32_t)));
+    CUC(e->d_dsac_exp.reserve(n * sizeof(double)));
+    CUC(e->d_dsac_rot.reserve(n * sizeof(double)));
+    CUC(e->d_dsac_terr.reserve(n * sizeof(double)));
+    CUC(e->d_dsac_correct.reserve(n * sizeof(int32_t)));
+    CUC(e->h_totals.reserve(2 * sizeof(int32_t)));
     CUC(cudaMemset(e->d_frame_counter, 0, n * sizeof(unsigned int)));
     CUC(cudaMemset(e->d_fragile, 0, sizeof(unsigned long long)));
     if (getenv("DSAC_K1_TIMERS")) {
-        CUC(cudaMalloc(&e->d_phase, 16 * sizeof(unsigned long long)));
+        CUC(e->d_phase.reserve(16 * sizeof(unsigned long long)));
         CUC(cudaMemset(e->d_phase, 0, 16 * sizeof(unsigned long long)));
     }
     CUC(cudaMemset(e->d_status, 0, n * sizeof(uint32_t)));
@@ -397,7 +417,7 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cfg->device);
         if (per_sm > 0 && sms > 0) e->k1_slots = per_sm * sms;
     }
-    CUC(cudaMallocHost(&e->h_stream_ncand, n * cfg->n_streams * sizeof(long long)));
+    CUC(e->h_stream_ncand.reserve(n * cfg->n_streams * sizeof(long long)));
     if (const char* m = getenv("DSAC_K1_MODE")) e->k1_mode = (strcmp(m, "mono") == 0) ? 0 : 1;
     if (const char* r = getenv("DSAC_K1_ROUNDS")) { e->k1_rounds = std::max(1, std::min(K1S_MAX_ROUNDS - 1, atoi(r))); e->k1_rounds_fixed = true; }
     if (e->k1_mode) {
@@ -409,16 +429,16 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
         cap = (cap + 1023) & ~1023;     // a round is generated in portions of cap / 4, themselves multiples of 256
         e->k1_cap = cap;
         e->k1_wq_stride = (int)(slots * 128);
-        CUC(cudaMalloc(&e->d_k1_state, slots * sizeof(K1SlotState)));
-        CUC(cudaMalloc(&e->d_k1_celltab, n * N * sizeof(CellRec)));
-        CUC(cudaMalloc(&e->d_k1_cells, slots * cap * sizeof(uint2)));
-        CUC(cudaMalloc(&e->d_k1_endw, slots * cap * sizeof(uint32_t)));
-        CUC(cudaMalloc(&e->d_k1_accbits, slots * (cap / 32) * sizeof(uint32_t)));
-        CUC(cudaMalloc(&e->d_k1_pose, slots * cap * 6 * sizeof(double)));
-        CUC(cudaMalloc(&e->d_k1_wq, (size_t)K1S_MAX_SETS * slots * 128 * sizeof(uint2)));
-        CUC(cudaMalloc(&e->d_k1_fq, 2 * slots * cap * sizeof(uint32_t)));   // two regions: the filter of set k+1 writes one while the solve of set k reads the other
-        CUC(cudaMalloc(&e->d_k1_counters, 2 * K1S_MAX_SETS * sizeof(int)));
-        CUC(cudaMalloc(&e->d_k1_chain, slots * (K1Q_MAX_WIN + 1) * 4 * sizeof(uint32_t)));
+        CUC(e->d_k1_state.reserve(slots * sizeof(K1SlotState)));
+        CUC(e->d_k1_celltab.reserve(n * N * sizeof(CellRec)));
+        CUC(e->d_k1_cells.reserve(slots * cap * sizeof(uint2)));
+        CUC(e->d_k1_endw.reserve(slots * cap * sizeof(uint32_t)));
+        CUC(e->d_k1_accbits.reserve(slots * (cap / 32) * sizeof(uint32_t)));
+        CUC(e->d_k1_pose.reserve(slots * cap * 6 * sizeof(double)));
+        CUC(e->d_k1_wq.reserve((size_t)K1S_MAX_SETS * slots * 128 * sizeof(uint2)));
+        CUC(e->d_k1_fq.reserve(2 * slots * cap * sizeof(uint32_t)));   // two regions: the filter of set k+1 writes one while the solve of set k reads the other
+        CUC(e->d_k1_counters.reserve(2 * K1S_MAX_SETS * sizeof(int)));
+        CUC(e->d_k1_chain.reserve(slots * (K1Q_MAX_WIN + 1) * 4 * sizeof(uint32_t)));
         CUC(cudaMemset(e->d_k1_chain, 0, slots * (K1Q_MAX_WIN + 1) * 4 * sizeof(uint32_t)));
         {
             int per_sm = 0;
@@ -431,12 +451,12 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
             if (const char* sv = getenv("DSAC_K1_SPEC")) want = atoi(sv);
             if (want) {
                 const size_t ss = std::min<size_t>(slots, 8);    // 8 frames x 1 stream: 0.513 -> 0.466 ms per step (H100 SXM, 700 W); at 16 frames the 1360 window CTAs are no longer one wave
-                CUC(cudaMalloc(&e->d_k1_vstate, ss * K1P_VPER * sizeof(K1SlotState)));
-                CUC(cudaMalloc(&e->d_k1_vcells, ss * K1P_VPER * K1P_CAPW * sizeof(uint2)));
-                CUC(cudaMalloc(&e->d_k1_vendw, ss * K1P_VPER * K1P_CAPW * sizeof(uint32_t)));
-                CUC(cudaMalloc(&e->d_k1_spec_result, ss * sizeof(int)));
+                CUC(e->d_k1_vstate.reserve(ss * K1P_VPER * sizeof(K1SlotState)));
+                CUC(e->d_k1_vcells.reserve(ss * K1P_VPER * K1P_CAPW * sizeof(uint2)));
+                CUC(e->d_k1_vendw.reserve(ss * K1P_VPER * K1P_CAPW * sizeof(uint32_t)));
+                CUC(e->d_k1_spec_result.reserve(ss * sizeof(int)));
                 CUC(cudaMemset(e->d_k1_spec_result, 0, ss * sizeof(int)));
-                CUC(cudaMalloc(&e->d_k1_spec_table, ss * K1P_TABLE * sizeof(int)));
+                CUC(e->d_k1_spec_table.reserve(ss * K1P_TABLE * sizeof(int)));
                 e->k1_spec_slots = (int)ss;
             }
         }
@@ -446,30 +466,30 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
             CUC(cudaDeviceGetStreamPriorityRange(&least, &greatest));
             int prio = greatest;
             if (const char* pr = getenv("DSAC_K1_SIDE_PRIO")) prio = atoi(pr) ? greatest : least;
-            CUC(cudaStreamCreateWithPriority(&e->k1_side, cudaStreamNonBlocking, prio));
-            CUC(cudaStreamCreateWithPriority(&e->k1_side2, cudaStreamNonBlocking, prio));
+            CUC(cudaStreamCreateWithPriority(e->k1_side.put(), cudaStreamNonBlocking, prio));
+            CUC(cudaStreamCreateWithPriority(e->k1_side2.put(), cudaStreamNonBlocking, prio));
             for (int i = 0; i < K1S_MAX_SETS; i++) {
-                CUC(cudaEventCreateWithFlags(&e->k1_ev_filt[i], cudaEventDisableTiming));
-                CUC(cudaEventCreateWithFlags(&e->k1_ev_solve[i], cudaEventDisableTiming));
+                CUC(cudaEventCreateWithFlags(e->k1_ev_filt[i].put(), cudaEventDisableTiming));
+                CUC(cudaEventCreateWithFlags(e->k1_ev_solve[i].put(), cudaEventDisableTiming));
             }
         }
-        for (int i = 0; i < K1S_MAX_SETS; i++) CUC(cudaEventCreateWithFlags(&e->k1_ev_gen[i], cudaEventDisableTiming));
-        CUC(cudaEventCreateWithFlags(&e->k1_ev_round, cudaEventDisableTiming));
+        for (int i = 0; i < K1S_MAX_SETS; i++) CUC(cudaEventCreateWithFlags(e->k1_ev_gen[i].put(), cudaEventDisableTiming));
+        CUC(cudaEventCreateWithFlags(e->k1_ev_round.put(), cudaEventDisableTiming));
         {   // the second lane (forward_split: two concurrent half-batches)
             int least = 0, greatest = 0;
             CUC(cudaDeviceGetStreamPriorityRange(&least, &greatest));
             dsac_engine::K1Lane& L = e->lane1;
-            CUC(cudaStreamCreateWithFlags(&L.main, cudaStreamNonBlocking));
-            CUC(cudaStreamCreateWithPriority(&L.side, cudaStreamNonBlocking, greatest));
-            CUC(cudaStreamCreateWithPriority(&L.side2, cudaStreamNonBlocking, greatest));
+            CUC(cudaStreamCreateWithFlags(L.main.put(), cudaStreamNonBlocking));
+            CUC(cudaStreamCreateWithPriority(L.side.put(), cudaStreamNonBlocking, greatest));
+            CUC(cudaStreamCreateWithPriority(L.side2.put(), cudaStreamNonBlocking, greatest));
             for (int i = 0; i < K1S_MAX_SETS; i++) {
-                CUC(cudaEventCreateWithFlags(&L.ev_filt[i], cudaEventDisableTiming));
-                CUC(cudaEventCreateWithFlags(&L.ev_solve[i], cudaEventDisableTiming));
-                CUC(cudaEventCreateWithFlags(&L.ev_gen[i], cudaEventDisableTiming));
+                CUC(cudaEventCreateWithFlags(L.ev_filt[i].put(), cudaEventDisableTiming));
+                CUC(cudaEventCreateWithFlags(L.ev_solve[i].put(), cudaEventDisableTiming));
+                CUC(cudaEventCreateWithFlags(L.ev_gen[i].put(), cudaEventDisableTiming));
             }
-            CUC(cudaEventCreateWithFlags(&L.ev_round, cudaEventDisableTiming));
-            CUC(cudaMalloc(&L.counters, 2 * K1S_MAX_SETS * sizeof(int)));
-            CUC(cudaMalloc(&L.stats, 4 * sizeof(unsigned long long)));
+            CUC(cudaEventCreateWithFlags(L.ev_round.put(), cudaEventDisableTiming));
+            CUC(L.counters.reserve(2 * K1S_MAX_SETS * sizeof(int)));
+            CUC(L.stats.reserve(4 * sizeof(unsigned long long)));
             CUC(cudaMemset(L.stats, 0, 4 * sizeof(unsigned long long)));
             if (const char* ln = getenv("DSAC_K1_LANES")) e->k1_lanes = atoi(ln);
         }
@@ -479,9 +499,9 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
         if (const char* s4 = getenv("DSAC_K1_SOLVE4")) e->k1_solve_group4 = atoi(s4);
         if (const char* sb = getenv("DSAC_K1_SOLVE_BATCH")) e->k1_solve_batch = atoi(sb);
         CUC(cudaFuncSetAttribute(k1_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1XSmem)));
-        CUC(cudaMalloc(&e->d_k1_stats, 4 * sizeof(unsigned long long)));
+        CUC(e->d_k1_stats.reserve(4 * sizeof(unsigned long long)));
         CUC(cudaMemset(e->d_k1_stats, 0, 4 * sizeof(unsigned long long)));
-        if (getenv("DSAC_K1_DEBUG")) CUC(cudaMalloc(&e->d_k1_dbg, K1S_MAX_ROUNDS * 4 * sizeof(unsigned long long)));
+        if (getenv("DSAC_K1_DEBUG")) CUC(e->d_k1_dbg.reserve(K1S_MAX_ROUNDS * 4 * sizeof(unsigned long long)));
         CUC(cudaFuncSetAttribute(k1_filter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1FSmem)));
         int per_sm = 0;
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k1_filter, K1F_THREADS, sizeof(K1FSmem));
@@ -492,14 +512,14 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
         if (const char* g = getenv("DSAC_K1_FILTER_GRID")) e->k1_filter_grid = std::max(1, atoi(g));
         if (const char* g = getenv("DSAC_K1_SOLVE_GRID")) e->k1_solve_grid = std::max(1, atoi(g));
     }
-    for (int i = 0; i < 4; i++) CUC(cudaStreamCreateWithFlags(&e->pipe[i], cudaStreamNonBlocking));
+    for (int i = 0; i < 4; i++) CUC(cudaStreamCreateWithFlags(e->pipe[i].put(), cudaStreamNonBlocking));
     {
         int least = 0, greatest = 0;
         CUC(cudaDeviceGetStreamPriorityRange(&least, &greatest));
-        CUC(cudaStreamCreateWithPriority(&e->hi, cudaStreamNonBlocking, greatest));
-        CUC(cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
-        CUC(cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming));
-        CUC(cudaEventCreateWithFlags(&e->ev_fwd, cudaEventDisableTiming));
+        CUC(cudaStreamCreateWithPriority(e->hi.put(), cudaStreamNonBlocking, greatest));
+        CUC(cudaEventCreateWithFlags(e->ev_fork.put(), cudaEventDisableTiming));
+        CUC(cudaEventCreateWithFlags(e->ev_join.put(), cudaEventDisableTiming));
+        CUC(cudaEventCreateWithFlags(e->ev_fwd.put(), cudaEventDisableTiming));
         if (const char* ts = getenv("DSAC_TAIL_SPLIT")) e->tail_split = atoi(ts);
     }
 #undef CUC
@@ -526,7 +546,7 @@ int dsac_sampler_profile(dsac_engine* e, int32_t enable) {
     if (!e) return DSAC_ERR_ARG;
     if (!e->k1_mode) return fail(e, DSAC_ERR_ARG, "dsac_sampler_profile needs the split sampler (DSAC_K1_MODE unset)");
     CU(cudaSetDevice(e->cfg.device));
-    if (enable && !e->d_k1_dbg) CU(cudaMalloc(&e->d_k1_dbg, K1S_MAX_ROUNDS * 4 * sizeof(unsigned long long)));
+    if (enable) CU(e->d_k1_dbg.reserve(K1S_MAX_ROUNDS * 4 * sizeof(unsigned long long)));
     e->k1_profile = enable ? 1 : 0;
     return DSAC_OK;
 }
@@ -587,14 +607,8 @@ static int seam_backward(dsac_engine* e, int n, const double* d_sog, cudaStream_
                     e->hook ? "the forward hook" : "the backward hook", e->hook ? "the backward hook" : "the forward hook");
     if (!e->d_diffmaps) return fail(e, DSAC_ERR_ARG, "the score seam needs write_diffmaps=1");
     const size_t H = e->cfg.n_hyps, count = (size_t)n * H * DSAC_N;
-    if (count > e->ext_g_count) {
-        if (e->d_ext_g) cudaFree(e->d_ext_g);
-    if (e->d_kabsch) cudaFree(e->d_kabsch);
-        e->d_ext_g = nullptr; e->ext_g_count = 0;
-        CU(cudaMalloc(&e->d_ext_g, (count + (size_t)n * H) * sizeof(double)));
-        e->ext_g_count = count;
-    }
-    double* clamped = e->d_ext_g + e->ext_g_count;   // [n][H] behind the gradient block
+    CU(e->d_ext_g.reserve((count + (size_t)n * H) * sizeof(double)));
+    double* clamped = e->d_ext_g + count;   // [n][H] behind the gradient block
     k_clamp_copy<<<(unsigned)(((size_t)n * H + 255) / 256), 256, 0, stream>>>(d_sog, clamped, (size_t)n * H, e->cfg.grad_clamp);
     e->launches++;
     CU(cudaGetLastError());
@@ -646,9 +660,9 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             const size_t T = (size_t)c.n_streams, cap = (size_t)e->k1_cap;
             // the lane's own streams, events, counters and statistics (lane 0: the engine's; lane 1: e->lane1)
             cudaStream_t k_side = lane ? e->lane1.side : e->k1_side, k_side2 = lane ? e->lane1.side2 : e->k1_side2;
-            cudaEvent_t* k_ev_filt = lane ? e->lane1.ev_filt : e->k1_ev_filt;
-            cudaEvent_t* k_ev_solve = lane ? e->lane1.ev_solve : e->k1_ev_solve;
-            cudaEvent_t* k_ev_gen = lane ? e->lane1.ev_gen : e->k1_ev_gen;
+            const Event* k_ev_filt = lane ? e->lane1.ev_filt : e->k1_ev_filt;
+            const Event* k_ev_solve = lane ? e->lane1.ev_solve : e->k1_ev_solve;
+            const Event* k_ev_gen = lane ? e->lane1.ev_gen : e->k1_ev_gen;
             cudaEvent_t k_ev_round = lane ? e->lane1.ev_round : e->k1_ev_round;
             int* k_counters = lane ? e->lane1.counters : e->d_k1_counters;
             unsigned long long* k_stats = lane ? e->lane1.stats : e->d_k1_stats;
@@ -693,9 +707,9 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             auto mark = [&](int kind) {   // dsac_sampler_profile: an event after every launch
                 if (!e->k1_profile) return;
                 if ((size_t)e->k1_ev_n >= e->k1_ev.size()) {
-                    cudaEvent_t ev;
-                    if (cudaEventCreate(&ev) != cudaSuccess) return;
-                    e->k1_ev.push_back(ev);
+                    Event ev;
+                    if (cudaEventCreate(ev.put()) != cudaSuccess) return;
+                    e->k1_ev.push_back(std::move(ev));
                     e->k1_ev_kind.push_back(0);
                 }
                 e->k1_ev_kind[e->k1_ev_n] = kind;
@@ -1044,7 +1058,7 @@ static int forward_submit_impl(dsac_engine* e, int32_t n, int64_t frame0, const 
     e->cur_coords = e->d_coords;
     e->cur_pix = e->d_pix;
     e->cur_pix_shared = pix_shared;
-    e->cur_gt = gt_jp ? e->d_gt : nullptr;
+    e->cur_gt = gt_jp ? e->d_gt.get() : nullptr;
     e->cur_n = n;
     e->dsac_n = 0;
     e->cur_frame0 = frame0;
@@ -1052,9 +1066,9 @@ static int forward_submit_impl(dsac_engine* e, int32_t n, int64_t frame0, const 
     // H2D(chunk) -> K1 -> K2 -> K4 -> D2H(chunk).  Copies of later chunks overlap the kernels of earlier
     // ones and the tail of one chunk's kernels is filled by the next chunk's CTAs.
     static const bool trace = getenv("DSAC_TRACE") != nullptr;
-    cudaEvent_t tev[4];
+    Event tev[4];
     const auto t_host0 = std::chrono::steady_clock::now();
-    if (trace) for (int k = 0; k < 4; k++) cudaEventCreate(&tev[k]);
+    if (trace) for (int k = 0; k < 4; k++) cudaEventCreate(tev[k].put());
     int chunks = 1;   // the sampler kernel wants the whole batch (tools/e2e_probe.py compares chunks)
     if (const char* ev = getenv("DSAC_PIPE_CHUNKS")) chunks = std::max(1, std::min(4, atoi(ev)));
     if (pix_shared) CU(cudaMemcpyAsync(e->d_pix, pix, N * 2 * sizeof(int32_t), cudaMemcpyHostToDevice, e->pipe[0]));
@@ -1084,7 +1098,7 @@ static int forward_submit_impl(dsac_engine* e, int32_t n, int64_t frame0, const 
         // one chunk: the tail split applies (mode 1: blocking calls only -- with several passes in flight the other
         // pass already fills the partial wave and a high-priority stream would only delay it; mode 2: always)
         int rc = (chunks == 1)
-                     ? forward_split(e, m, frame0, e->d_coords, e->d_pix, pix_shared, gt_jp ? e->d_gt : nullptr, st,
+                     ? forward_split(e, m, frame0, e->d_coords, e->d_pix, pix_shared, gt_jp ? e->d_gt.get() : nullptr, st,
                                      blocking ? e->tail_split >= 1 : e->tail_split >= 2)
                      : forward_range(e, lo, m, frame0 + lo, e->d_coords + f * N * 3, pix_shared ? e->d_pix : e->d_pix + f * N * 2,
                                      pix_shared, gt_jp ? e->d_gt + f * 12 : nullptr, st);
@@ -1109,7 +1123,6 @@ static int forward_submit_impl(dsac_engine* e, int32_t n, int64_t frame0, const 
         cudaEventElapsedTime(&a, tev[0], tev[1]); cudaEventElapsedTime(&b, tev[1], tev[2]); cudaEventElapsedTime(&d, tev[2], tev[3]);
         const double host_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_host0).count();
         fprintf(stderr, "[dsac trace] H2D %.3f ms  kernels %.3f ms  D2H %.3f ms  | call %.3f ms (host wall)\n", a, b, d, host_ms);
-        for (int k = 0; k < 4; k++) cudaEventDestroy(tev[k]);
     }
     return DSAC_OK;
 }
@@ -1149,33 +1162,22 @@ static int forward_dsac_run(dsac_engine* e, int32_t n, int64_t frame0, const int
     const dsac_config& c = e->cfg;
     CU(cudaSetDevice(c.device));
     const size_t N = DSAC_N, nn = (size_t)n, H = c.n_hyps, jobs = nn * H;
-    // refine-all buffers
+    // refine-all buffers: they grow together, and the job -> frame table is written whenever they do
     if (jobs > e->ra_jobs) {
-        void* old[] = {e->d_ra_frame, e->d_ra_pose, e->d_ra_loss, e->d_ra_rot, e->d_ra_t, e->d_ra_correct, e->d_ra_steps};
-        for (void* q : old)
-            if (q) cudaFree(q);
-        e->d_ra_frame = nullptr; e->d_ra_pose = nullptr; e->d_ra_loss = nullptr; e->d_ra_rot = nullptr; e->d_ra_t = nullptr;
-        e->d_ra_correct = nullptr; e->d_ra_steps = nullptr;
         e->ra_jobs = 0;
-        CU(cudaMalloc(&e->d_ra_frame, jobs * sizeof(int32_t)));
-        CU(cudaMalloc(&e->d_ra_pose, jobs * 6 * sizeof(double)));
-        CU(cudaMalloc(&e->d_ra_loss, jobs * sizeof(double)));
-        CU(cudaMalloc(&e->d_ra_rot, jobs * sizeof(double)));
-        CU(cudaMalloc(&e->d_ra_t, jobs * sizeof(double)));
-        CU(cudaMalloc(&e->d_ra_correct, jobs * sizeof(int32_t)));
-        CU(cudaMalloc(&e->d_ra_steps, jobs * sizeof(int32_t)));
+        CU(e->d_ra_frame.reserve(jobs * sizeof(int32_t)));
+        CU(e->d_ra_pose.reserve(jobs * 6 * sizeof(double)));
+        CU(e->d_ra_loss.reserve(jobs * sizeof(double)));
+        CU(e->d_ra_rot.reserve(jobs * sizeof(double)));
+        CU(e->d_ra_t.reserve(jobs * sizeof(double)));
+        CU(e->d_ra_correct.reserve(jobs * sizeof(int32_t)));
+        CU(e->d_ra_steps.reserve(jobs * sizeof(int32_t)));
         std::vector<int32_t> jf(jobs);
         for (size_t j = 0; j < jobs; j++) jf[j] = (int32_t)(j / H);
         CU(cudaMemcpy(e->d_ra_frame, jf.data(), jobs * sizeof(int32_t), cudaMemcpyHostToDevice));
         e->ra_jobs = jobs;
     }
-    if (want_imaps && jobs > e->ra_imap_jobs) {
-        if (e->d_ra_imap) cudaFree(e->d_ra_imap);
-        e->d_ra_imap = nullptr;
-        e->ra_imap_jobs = 0;
-        CU(cudaMalloc(&e->d_ra_imap, jobs * N * sizeof(int32_t)));
-        e->ra_imap_jobs = jobs;
-    }
+    if (want_imaps) CU(e->d_ra_imap.reserve(jobs * N * sizeof(int32_t)));
     e->cur_coords = d_coords; e->cur_pix = d_pix; e->cur_pix_shared = pix_shared; e->cur_gt = d_gt;
     e->cur_n = 0;   // the soft-argmax backward does not apply to this pass
     e->dsac_n = 0;
@@ -1203,7 +1205,7 @@ static int forward_dsac_run(dsac_engine* e, int32_t n, int64_t frame0, const int
         rp.job_init = e->d_hyp_pose;
         rp.out_pose = e->d_ra_pose;
         rp.steps_done = e->d_ra_steps;
-        rp.inlier_map = want_imaps ? e->d_ra_imap : nullptr;
+        rp.inlier_map = want_imaps ? e->d_ra_imap.get() : nullptr;
         if (d_gt) {
             rp.gt_jp = d_gt;
             rp.loss = e->d_ra_loss; rp.rot_err = e->d_ra_rot; rp.t_err = e->d_ra_t; rp.correct = e->d_ra_correct;
@@ -1218,7 +1220,7 @@ static int forward_dsac_run(dsac_engine* e, int32_t n, int64_t frame0, const int
         dp.seed = c.seed; dp.frame0 = frame0;
         dp.sf = e->d_sf; dp.img_idx = e->d_img_idx; dp.stream_endpos = e->d_stream_endpos;
         dp.loss = e->d_ra_loss; dp.rot_err = e->d_ra_rot; dp.t_err = e->d_ra_t; dp.correct = e->d_ra_correct;
-        dp.inlier_maps = want_imaps ? e->d_ra_imap : nullptr;
+        dp.inlier_maps = want_imaps ? e->d_ra_imap.get() : nullptr;
         dp.hyp_idx = e->d_dsac_pick; dp.expected_loss = e->d_dsac_exp;
         dp.out_rot_err = e->d_dsac_rot; dp.out_t_err = e->d_dsac_terr; dp.out_correct = e->d_dsac_correct;
         k_dsac_draw<<<n, DRAW_THREADS, 0, stream>>>(dp);
@@ -1276,7 +1278,7 @@ int dsac_forward_dsac(dsac_engine* e, int32_t n, int64_t frame0, const int16_t* 
     CU(cudaMemcpyAsync(e->d_coords, coords, nn * N * 3 * sizeof(int16_t), cudaMemcpyHostToDevice, stream));
     CU(cudaMemcpyAsync(e->d_pix, pix, (pix_shared ? 1 : nn) * N * 2 * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
     if (gt_jp) CU(cudaMemcpyAsync(e->d_gt, gt_jp, nn * 12 * sizeof(double), cudaMemcpyHostToDevice, stream));
-    int rc = forward_dsac_run(e, n, frame0, e->d_coords, e->d_pix, pix_shared, gt_jp ? e->d_gt : nullptr, random_draw,
+    int rc = forward_dsac_run(e, n, frame0, e->d_coords, e->d_pix, pix_shared, gt_jp ? e->d_gt.get() : nullptr, random_draw,
                               out->inlier_maps != nullptr, stream);
     if (rc == DSAC_OK) rc = forward_dsac_copy(e, n, out, stream);
     const cudaError_t st = cudaStreamSynchronize(stream);   // also before an error return: copies from the caller's buffers may be queued
@@ -1434,12 +1436,7 @@ int dsac_register_depth_device(dsac_engine* e, const dsac_rgbd_camera* cam, int3
     const size_t count = (size_t)n * c.width * c.height;
     if (d_dropped) CU(cudaMemsetAsync(d_dropped, 0, (size_t)n * sizeof(int32_t), stream));
     if (c.raw_data) {
-        if (e->reg_keys_bytes < count * sizeof(uint64_t)) {
-            if (e->d_reg_keys) CU(cudaFree(e->d_reg_keys));
-            e->d_reg_keys = nullptr; e->reg_keys_bytes = 0;
-            CU(cudaMalloc(&e->d_reg_keys, count * sizeof(uint64_t)));
-            e->reg_keys_bytes = count * sizeof(uint64_t);
-        }
+        CU(e->d_reg_keys.reserve(count * sizeof(uint64_t)));
         CU(cudaMemsetAsync(e->d_reg_keys, 0, count * sizeof(uint64_t), stream));
     }
     k_register_depth<<<grid_of(count, 256), 256, 0, stream>>>(c, n, d_raw, e->d_reg_keys, d_depth, d_dropped);
