@@ -18,6 +18,11 @@ Their backward is the reference's chain with the incoming gradient in place of d
 outputs"): it inherits the reference's finite differences and quirks, and the clamp applies to the total dLoss/dObj,
 since the incoming gradient is already inside it.
 
+`cameras` (float64 [n][3] = focal, cx, cy of every frame; a host array or CPU tensor) gives each frame of the batch its
+own camera: it is applied with Engine.set_cameras before the forward, on the current stream, and stays in force on the
+engine.  None leaves the engine's setting alone.  Changing the cameras between a loss and its backward() makes that
+backward() raise.
+
 Everything stays on the device, on torch.cuda.current_stream().  The engine holds one pass: a forward on the same engine
 between a loss and its backward() makes that backward() raise.
 """
@@ -43,6 +48,11 @@ def _check_inputs(engine, prediction, pix, gt_jp, need_gt=True):
     if gt_jp is not None and (gt_jp.dtype != torch.float64 or gt_jp.numel() != n * 12):
         raise ValueError("gt_jp must be float64 [n][12]")
     return n, pix.contiguous(), gt_jp.contiguous() if gt_jp is not None else None, (1 if pix.numel() == _E.N * 2 else 0)
+
+
+def _set_cameras(engine, prediction, cameras):
+    if cameras is not None:
+        engine.set_cameras(cameras, torch.cuda.current_stream(prediction.device).cuda_stream)
 
 
 def _coords(engine, prediction, stream):
@@ -152,26 +162,30 @@ class _DsacHypotheses(torch.autograd.Function):
         return grad, None, None, None, None, None
 
 
-def softam_loss(engine, prediction, pix, gt_jp, frame0=0, clamp=0.1):
+def softam_loss(engine, prediction, pix, gt_jp, frame0=0, clamp=0.1, cameras=None):
     """Per-frame loss of the soft-argmax pipeline (train_ransac_softam.cpp) on `prediction`, float64 [n]; differentiable
     with respect to `prediction`.  frame0: global index of the first frame (keys the sampler streams)."""
+    _set_cameras(engine, prediction, cameras)
     return _SoftamLoss.apply(prediction, engine, pix, gt_jp, int(frame0), float(clamp))
 
 
-def dsac_expected_loss(engine, prediction, pix, gt_jp, frame0=0, random_draw=True, clamp=0.1):
+def dsac_expected_loss(engine, prediction, pix, gt_jp, frame0=0, random_draw=True, clamp=0.1, cameras=None):
     """Per-frame expected loss of the DSAC / RANSAC variant (train_ransac.cpp) on `prediction`, float64 [n];
     differentiable with respect to `prediction`."""
+    _set_cameras(engine, prediction, cameras)
     return _DsacExpectedLoss.apply(prediction, engine, pix, gt_jp, int(frame0), bool(random_draw), float(clamp))
 
 
-def softam_pose(engine, prediction, pix, frame0=0, clamp=0.1):
+def softam_pose(engine, prediction, pix, frame0=0, clamp=0.1, cameras=None):
     """Refined pose of every frame of the soft-argmax pipeline as a jp 6-vector [rodrigues(R); t in mm], float64 [n][6];
     differentiable with respect to `prediction`.  Needs no ground truth."""
+    _set_cameras(engine, prediction, cameras)
     return _SoftamPose.apply(prediction, engine, pix, int(frame0), float(clamp))
 
 
-def dsac_hypotheses(engine, prediction, pix, frame0=0, random_draw=True, clamp=0.1):
+def dsac_hypotheses(engine, prediction, pix, frame0=0, random_draw=True, clamp=0.1, cameras=None):
     """(sf [n][H], refined jp 6-vectors [n][H][6]) of the DSAC / RANSAC variant, both float64 and differentiable with
     respect to `prediction`.  The gradient through the poses covers the hypotheses with sf > 1e-4 whose incoming
     gradient is nonzero; an output that receives no gradient costs nothing in the backward."""
+    _set_cameras(engine, prediction, cameras)
     return _DsacHypotheses.apply(prediction, engine, pix, int(frame0), bool(random_draw), float(clamp))

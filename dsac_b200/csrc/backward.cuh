@@ -122,6 +122,7 @@ struct BwParams {
     const double* gt_jp;        // [n][12]
     const double* seed;         // [n][6] dOuter/d(refined jp6) in place of dLossMax against gt_jp; null: dLossMax
     double f, cx, cy;
+    const Cam* cams;            // [n] or null: the camera of every frame is f, cx, cy
     int H, thr, skip, fix_q4;
     double alpha, beta, grad_clamp;
     // forward state
@@ -150,6 +151,7 @@ struct DsacBwParams {
     const int32_t* pix;
     int pix_stride;
     double f, cx, cy;
+    const Cam* cams;            // [n] or null: the camera of every frame is f, cx, cy
     int H;
     const int32_t* img_idx;     // [n][H][4]
     const double* ref_pose;     // [n*H][6] refined cv pose of every hypothesis (forward_dsac)
@@ -190,8 +192,9 @@ __global__ void k_dsac_job_p3p(DsacBwParams p) {
     obj[p.job_p3p[j * 3 + 1]] += (float)p.job_p3p[j * 3 + 2];   // objPts[pt] +/- eps (integers in float: exact)
     double pose[6], R[9], t[3], e2;
     P3PProblem pr;
-    make_problem(obj, img, p.f, p.cx, p.cy, pr);
-    if (p3p_best(pr, p.f, p.cx, p.cy, R, t, &e2) > 0) {
+    const Cam cam = frame_cam(p, frame);
+    make_problem(obj, img, cam.f, cam.cx, cam.cy, pr);
+    if (p3p_best(pr, cam.f, cam.cx, cam.cy, R, t, &e2) > 0) {
         rodrigues_m2v(R, pose);
         pose[3] = t[0]; pose[4] = t[1]; pose[5] = t[2];
     } else {
@@ -430,9 +433,10 @@ __global__ void __launch_bounds__(192) k_dpnp(BwParams p) {
         }
         double fS[6], bS[6], pose[6], R[9], t[3], e2;
         P3PProblem pr;
+        const Cam cam = frame_cam(p, frame);
         obj[col] += eps;
-        make_problem(obj, img, p.f, p.cx, p.cy, pr);
-        if (valid && p3p_best(pr, p.f, p.cx, p.cy, R, t, &e2) > 0) {
+        make_problem(obj, img, cam.f, cam.cx, cam.cy, pr);
+        if (valid && p3p_best(pr, cam.f, cam.cx, cam.cy, R, t, &e2) > 0) {
             rodrigues_m2v(R, pose);
             pose[3] = t[0]; pose[4] = t[1]; pose[5] = t[2];
         } else {
@@ -440,8 +444,8 @@ __global__ void __launch_bounds__(192) k_dpnp(BwParams p) {
         }
         jp6_from_cv_dev(pose, fS);
         obj[col] -= 2 * eps;
-        make_problem(obj, img, p.f, p.cx, p.cy, pr);
-        if (valid && p3p_best(pr, p.f, p.cx, p.cy, R, t, &e2) > 0) {
+        make_problem(obj, img, cam.f, cam.cx, cam.cy, pr);
+        if (valid && p3p_best(pr, cam.f, cam.cx, cam.cy, R, t, &e2) > 0) {
             rodrigues_m2v(R, pose);
             pose[3] = t[0]; pose[4] = t[1]; pose[5] = t[2];
         } else {
@@ -548,7 +552,8 @@ __global__ void __launch_bounds__(K5_THREADS) k_dscore(BwParams p) {
         pu[j] = (double)(float)pix[pt * 2]; pv[j] = (double)(float)pix[pt * 2 + 1];
         acc[j][0] = acc[j][1] = acc[j][2] = 0;
     }
-    const double f = p.f, cx = p.cx, cy = p.cy;
+    const Cam cam = frame_cam(p, frame);
+    const double f = cam.f, cx = cam.cx, cy = cam.cy;
     for (int h = h_begin; h < h_end; h++) {
         __syncthreads();
         if (tid < 39) s_h[tid] = p.s.hypjp[((size_t)frame * p.H + h) * 39 + tid];

@@ -28,6 +28,8 @@
 
 using namespace dsac;
 
+static_assert(sizeof(Cam) == sizeof(dsac_camera), "Cam mirrors dsac_camera");
+
 static std::string g_create_error;
 
 // Owners of the engine's CUDA resources, the only code here that frees any.  Each releases what it holds in its
@@ -120,6 +122,12 @@ struct dsac_engine {
     int k1_slots = 296;             // resident k_sample CTAs on this GPU (SMs x CTAs/SM), set at creation
     int dsac_n = 0;                 // frames of the last dsac_forward_dsac (0: none), for dsac_backward_dsac
     long long cur_frame0 = 0;
+    // per-frame cameras (dsac_set_cameras): sized once for max_frames; cams_n == 0: the config's camera
+    DevMem<Cam> d_cams;
+    PinnedMem<dsac_camera> h_cams;  // staging of the copy to d_cams
+    Event ev_cams;                  // recorded after that copy: the staging is rewritten, and a pass starts, only after it
+    int cams_n = 0;
+    unsigned long long cams_gen = 0, fwd_cams_gen = 0;   // generation of the setting, and the one the last forward ran with
     // state
     DevMem<uint16_t> d_perm;
     DevMem<double> d_hyp_pose;
@@ -376,6 +384,9 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
     CUC(e->d_dsac_terr.reserve(n * sizeof(double)));
     CUC(e->d_dsac_correct.reserve(n * sizeof(int32_t)));
     CUC(e->h_totals.reserve(2 * sizeof(int32_t)));
+    CUC(e->d_cams.reserve(n * sizeof(Cam)));
+    CUC(e->h_cams.reserve(n * sizeof(dsac_camera)));
+    CUC(cudaEventCreateWithFlags(e->ev_cams.put(), cudaEventDisableTiming));
     CUC(cudaMemset(e->d_frame_counter, 0, n * sizeof(unsigned int)));
     CUC(cudaMemset(e->d_fragile, 0, sizeof(unsigned long long)));
     if (getenv("DSAC_K1_TIMERS")) {
@@ -406,11 +417,16 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
         CUC(cudaMemcpy(e->d_perm, perm.data(), perm.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
     }
     CUC(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1Smem)));
+    CUC(cudaFuncSetAttribute(k_sample_cam, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1Smem)));
     // k_refine wants 8 CTAs x 26 KB of shared memory per SM: ask for the carve-out explicitly (the default heuristic
     // need not pick the split the launch bounds were written for).  k_sample is left to the default: it spills to
     // local memory, so it wants the L1 that the largest carve-out would take away (DSAC_K1_CARVEOUT overrides).
     CUC(cudaFuncSetAttribute(k_refine, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    if (const char* co = getenv("DSAC_K1_CARVEOUT")) CUC(cudaFuncSetAttribute(k_sample, cudaFuncAttributePreferredSharedMemoryCarveout, atoi(co)));
+    CUC(cudaFuncSetAttribute(k_refine_cam, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    if (const char* co = getenv("DSAC_K1_CARVEOUT")) {
+        CUC(cudaFuncSetAttribute(k_sample, cudaFuncAttributePreferredSharedMemoryCarveout, atoi(co)));
+        CUC(cudaFuncSetAttribute(k_sample_cam, cudaFuncAttributePreferredSharedMemoryCarveout, atoi(co)));
+    }
     {
         int per_sm = 0, sms = 0;
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_sample, K1_THREADS, sizeof(K1Smem));
@@ -503,6 +519,7 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
         CUC(cudaMemset(e->d_k1_stats, 0, 4 * sizeof(unsigned long long)));
         if (getenv("DSAC_K1_DEBUG")) CUC(e->d_k1_dbg.reserve(K1S_MAX_ROUNDS * 4 * sizeof(unsigned long long)));
         CUC(cudaFuncSetAttribute(k1_filter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1FSmem)));
+        CUC(cudaFuncSetAttribute(k1_filter_cam, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1FSmem)));
         int per_sm = 0;
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k1_filter, K1F_THREADS, sizeof(K1FSmem));
         e->k1_filter_grid = std::max(1, per_sm) * e->sm_count;
@@ -537,6 +554,51 @@ int dsac_set_tail_split(dsac_engine* e, int32_t mode) {
     if (!e) return DSAC_ERR_ARG;
     if (mode < 0 || mode > 2) return fail(e, DSAC_ERR_ARG, "tail split mode %d out of range [0,2]", mode);
     e->tail_split = mode;
+    return DSAC_OK;
+}
+
+int dsac_set_cameras(dsac_engine* e, int32_t n, const dsac_camera* cams, void* stream_v) {
+    if (!e) return DSAC_ERR_ARG;
+    if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_set_cameras: a submitted pass has not been awaited (dsac_forward_wait)");
+    if (!cams) {
+        if (e->cams_n) e->cams_gen++;
+        e->cams_n = 0;
+        return DSAC_OK;
+    }
+    if (n < 1 || n > e->cfg.max_frames) return fail(e, DSAC_ERR_ARG, "dsac_set_cameras: n %d out of range [1,%d]", n, e->cfg.max_frames);
+    for (int32_t i = 0; i < n; i++) {
+        const dsac_camera& c = cams[i];
+        if (!std::isfinite(c.focal) || !(c.focal > 0) || !std::isfinite(c.cx) || !std::isfinite(c.cy))
+            return fail(e, DSAC_ERR_ARG, "dsac_set_cameras: camera %d is invalid (focal %g must be finite and > 0, cx %g and cy %g finite)", i,
+                        c.focal, c.cx, c.cy);
+    }
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    CU(cudaSetDevice(e->cfg.device));
+    CU(cudaEventSynchronize(e->ev_cams));             // the previous copy has left the staging buffer
+    memcpy(e->h_cams.get(), cams, (size_t)n * sizeof(dsac_camera));
+    CU(cudaStreamWaitEvent(stream, e->ev_fwd, 0));   // the last forward pass may still read the table
+    e->cams_n = 0;                                    // (a failed copy leaves the config's camera in force)
+    e->cams_gen++;
+    CU(cudaMemcpyAsync(e->d_cams.get(), e->h_cams.get(), (size_t)n * sizeof(dsac_camera), cudaMemcpyHostToDevice, stream));
+    CU(cudaEventRecord(e->ev_cams, stream));
+    e->cams_n = n;
+    return DSAC_OK;
+}
+
+// The checks and the bookkeeping every forward entry point shares: the batch matches the camera table, the pass is
+// stamped with the table's generation and `stream` waits for the table's copy.
+static int cameras_begin_pass(dsac_engine* e, int32_t n, cudaStream_t stream) {
+    if (e->cams_n && n != e->cams_n)
+        return fail(e, DSAC_ERR_ARG, "n_frames %d differs from the %d cameras set by dsac_set_cameras", n, e->cams_n);
+    if (e->cams_n) CU(cudaStreamWaitEvent(stream, e->ev_cams, 0));
+    e->fwd_cams_gen = e->cams_gen;
+    return DSAC_OK;
+}
+
+// A backward pass differentiates the forward before it, which ran with the cameras in force then.
+static int cameras_unchanged(dsac_engine* e, const char* who) {
+    if (e->fwd_cams_gen != e->cams_gen)
+        return fail(e, DSAC_ERR_ARG, "%s: the cameras were changed (dsac_set_cameras) after the forward pass", who);
     return DSAC_OK;
 }
 
@@ -637,12 +699,13 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
     cudaStream_t stream = (cudaStream_t)stream_v;
     const dsac_config& c = e->cfg;
     const size_t o = (size_t)off, Hh = (size_t)c.n_hyps, Nn = DSAC_N;
+    const Cam* cams = e->cams_n ? e->d_cams + o : nullptr;   // per-frame cameras: those of this range's frames
 
     if (e->stages & DSAC_STAGE_SAMPLE) {
         CU(cudaMemsetAsync(e->d_status + o, 0, (size_t)n * sizeof(uint32_t), stream));
         SampleParams sp;
         sp.coords = d_coords; sp.pix = d_pix; sp.pix_stride = pix_shared ? 0 : DSAC_N * 2;
-        sp.f = c.focal; sp.cx = c.cx; sp.cy = c.cy;
+        sp.f = c.focal; sp.cx = c.cx; sp.cy = c.cy; sp.cams = cams;
         sp.H = c.n_hyps; sp.T = c.n_streams; sp.thr = c.thr2d;
         sp.seed = c.seed; sp.skip = c.stream_skip; sp.max_candidates = c.max_candidates;
         sp.frame0 = frame0;
@@ -652,7 +715,8 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
         { const char* g = getenv("DSAC_K1_A2_GENERIC"); sp.a2_generic = (g && g[0] == '1') ? 1 : 0; }
         sp.resume = nullptr;
         if (!e->k1_mode) {
-            k_sample<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
+            if (cams) k_sample_cam<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
+            else k_sample<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
             e->launches++;
             CU(cudaGetLastError());
         } else {
@@ -729,7 +793,7 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
                 else k1_slot<<<g, K1S_THREADS, 0, stream>>>(qq);
             };
             // with the profile on everything runs on one stream so that the event intervals are the kernels' own durations
-            const bool fused = e->k1_fused != 0;
+            const bool fused = e->k1_fused != 0 && !cams;   // (k1_fused has no per-frame instantiation; the schedule does not change results)
             // streams: generator on `stream`, filter (and solve) on a side stream; with a batch that does not fill the GPU several
             // times over the solve gets a stream of its own, so that the filter of set k+1 need not wait for the solve of set k
             // (DSAC_K1_OVERLAP=1 / 2 compares them; on an H100 SXM at 700 W: 128 frames 0.856 / 0.862 ms, 1024 frames 3.09 / 3.10 ms)
@@ -741,7 +805,8 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             mark(-1);
             {
                 const int cell_blocks = (int)(((size_t)n * Nn + 255) / 256), seed_blocks = (int)((n_slots + 31) / 32);
-                k1_cells<<<(unsigned)(cell_blocks + seed_blocks), 256, 0, stream>>>(q, n, seed_blocks);
+                if (cams) k1_cells_cam<<<(unsigned)(cell_blocks + seed_blocks), 256, 0, stream>>>(q, n, seed_blocks);
+                else k1_cells<<<(unsigned)(cell_blocks + seed_blocks), 256, 0, stream>>>(q, n, seed_blocks);
             }
             mark(0);
             e->launches++;
@@ -750,7 +815,7 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             // takes 115 % of the expected need and one top-up round follows (every round is three dependent launches);
             // the rare straggler goes to the monolithic kernel
             const bool few = n_slots < 128;
-            const bool fused_req = e->k1_fused != 0;
+            const bool fused_req = fused;
             if (few) q.first_frac = 1.15;
             // speculative first round (k1_spec / k1_stitch): one stream generated window by window on many SMs; pays when a
             // stream's first round is several windows long (>= 64 hypotheses per stream) and the GPU is otherwise idle
@@ -827,7 +892,8 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
                         CU(cudaStreamWaitEvent(side, k_ev_gen[set], 0));
                         if (!batch && solve_side != side && set >= 2) CU(cudaStreamWaitEvent(side, k_ev_solve[set - 2], 0));   // the flag-queue region is free again
                     }
-                    k1_filter<<<fgrid, K1F_THREADS, sizeof(K1FSmem), side>>>(q);
+                    if (cams) k1_filter_cam<<<fgrid, K1F_THREADS, sizeof(K1FSmem), side>>>(q);
+                    else k1_filter<<<fgrid, K1F_THREADS, sizeof(K1FSmem), side>>>(q);
                     if (!overlap) mark(1);
                     e->launches += 2;
                     if (!solve_now) continue;
@@ -835,7 +901,10 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
                         CU(cudaEventRecord(k_ev_filt[set], side));
                         CU(cudaStreamWaitEvent(solve_side, k_ev_filt[set], 0));
                     }
-                    if (few && e->k1_solve_group4) k1_solve4<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
+                    const bool group4 = few && e->k1_solve_group4;
+                    if (cams && group4) k1_solve4_cam<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
+                    else if (cams) k1_solve_cam<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
+                    else if (group4) k1_solve4<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
                     else k1_solve<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
                     if (solve_side != side) CU(cudaEventRecord(k_ev_solve[set], solve_side));
                     if (!overlap) mark(2);
@@ -848,9 +917,14 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             launch_slot(q);
             mark(0);
             sp.resume = q.state;   // streams the rounds left unfinished (normally none) continue in the monolithic kernel
-            k_sample<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
+            if (cams) k_sample_cam<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
+            else k_sample<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
             mark(3);
             e->launches += 2;
+            if (cams) {   // the generator's selection wrote hyp_P with the config's focal length
+                k1_focal_rows_cam<<<(unsigned)(((size_t)n * c.n_hyps + 255) / 256), 256, 0, stream>>>(sp, n);
+                e->launches++;
+            }
             CU(cudaGetLastError());
         }
     }
@@ -863,13 +937,15 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
         kp.H = c.n_hyps;
         kp.tile = pick_tile(e, n);
         kp.tiles_per_frame = (c.n_hyps + kp.tile - 1) / kp.tile;
-        kp.cxf = (float)c.cx; kp.cyf = (float)c.cy;
+        kp.cxf = (float)c.cx; kp.cyf = (float)c.cy; kp.cams = cams;
         kp.thr = (float)c.thr2d;
         kp.kbeta = (float)(c.beta * 1.4426950408889634);
         kp.alpha = c.alpha;
         kp.external_scores = 0;
         dim3 grid(kp.tiles_per_frame, n);
-        if (e->d_diffmaps) k_score<true><<<grid, K2_THREADS, 0, stream>>>(kp);
+        if (cams && e->d_diffmaps) k_score_cam<true><<<grid, K2_THREADS, 0, stream>>>(kp);
+        else if (cams) k_score_cam<false><<<grid, K2_THREADS, 0, stream>>>(kp);
+        else if (e->d_diffmaps) k_score<true><<<grid, K2_THREADS, 0, stream>>>(kp);
         else k_score<false><<<grid, K2_THREADS, 0, stream>>>(kp);
         e->launches++;
         CU(cudaGetLastError());
@@ -890,7 +966,7 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
         memset(&rp, 0, sizeof(rp));
         rp.coords = d_coords; rp.pix = d_pix; rp.pix_stride = pix_shared ? 0 : DSAC_N * 2;
         rp.perm = e->d_perm;
-        rp.f = c.focal; rp.cx = c.cx; rp.cy = c.cy;
+        rp.f = c.focal; rp.cx = c.cx; rp.cy = c.cy; rp.cams = cams;
         rp.thr = c.thr2d; rp.inlier_count = c.inlier_count; rp.ref_steps = c.ref_steps;
         rp.n_jobs = n;
         rp.job_init = e->d_avg + o * 6;
@@ -901,7 +977,7 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             rp.gt_jp = d_gt_jp;
             rp.loss = e->d_loss + o; rp.rot_err = e->d_rot_err + o; rp.t_err = e->d_t_err + o; rp.correct = e->d_correct + o;
         }
-        k_refine<<<n, K4_THREADS, 0, stream>>>(rp);
+        launch_refine(rp, (unsigned)n, stream);
         e->launches++;
         CU(cudaGetLastError());
     }
@@ -962,6 +1038,7 @@ int dsac_forward_device(dsac_engine* e, int32_t n, int64_t frame0, const int16_t
     if (n < 1 || n > e->cfg.max_frames) return fail(e, DSAC_ERR_CAPACITY, "n_frames %d exceeds engine capacity %d", n, e->cfg.max_frames);
     if (!d_coords || !d_pix) return fail(e, DSAC_ERR_ARG, "null input");
     CU(cudaSetDevice(e->cfg.device));
+    if (int rc = cameras_begin_pass(e, n, (cudaStream_t)stream_v)) return rc;
     e->cur_coords = d_coords;
     e->cur_pix = d_pix;
     e->cur_pix_shared = pix_shared;
@@ -1054,6 +1131,8 @@ static int forward_submit_impl(dsac_engine* e, int32_t n, int64_t frame0, const 
     if (n < 1 || n > e->cfg.max_frames) return fail(e, DSAC_ERR_CAPACITY, "n_frames %d exceeds engine capacity %d", n, e->cfg.max_frames);
     if (!coords || !pix) return fail(e, DSAC_ERR_ARG, "null input");
     CU(cudaSetDevice(e->cfg.device));
+    for (int c = 0; c < 4; c++)   // (every chunk's stream: DSAC_PIPE_CHUNKS)
+        if (int rc = cameras_begin_pass(e, n, e->pipe[c])) return rc;
     const size_t N = DSAC_N;
     e->cur_coords = e->d_coords;
     e->cur_pix = e->d_pix;
@@ -1161,6 +1240,7 @@ static int forward_dsac_run(dsac_engine* e, int32_t n, int64_t frame0, const int
     if (!d_coords || !d_pix) return fail(e, DSAC_ERR_ARG, "null input");
     const dsac_config& c = e->cfg;
     CU(cudaSetDevice(c.device));
+    if (int rc = cameras_begin_pass(e, n, stream)) return rc;
     const size_t N = DSAC_N, nn = (size_t)n, H = c.n_hyps, jobs = nn * H;
     // refine-all buffers: they grow together, and the job -> frame table is written whenever they do
     if (jobs > e->ra_jobs) {
@@ -1198,7 +1278,7 @@ static int forward_dsac_run(dsac_engine* e, int32_t n, int64_t frame0, const int
         memset(&rp, 0, sizeof(rp));
         rp.coords = d_coords; rp.pix = d_pix; rp.pix_stride = pix_shared ? 0 : DSAC_N * 2;
         rp.perm = e->d_perm;
-        rp.f = c.focal; rp.cx = c.cx; rp.cy = c.cy;
+        rp.f = c.focal; rp.cx = c.cx; rp.cy = c.cy; rp.cams = e->cams_n ? e->d_cams.get() : nullptr;
         rp.thr = c.thr2d; rp.inlier_count = c.inlier_count; rp.ref_steps = c.ref_steps;
         rp.n_jobs = (int)jobs;
         rp.job_frame = e->d_ra_frame;
@@ -1210,7 +1290,7 @@ static int forward_dsac_run(dsac_engine* e, int32_t n, int64_t frame0, const int
             rp.gt_jp = d_gt;
             rp.loss = e->d_ra_loss; rp.rot_err = e->d_ra_rot; rp.t_err = e->d_ra_t; rp.correct = e->d_ra_correct;
         }
-        k_refine<<<(unsigned)jobs, K4_THREADS, 0, stream>>>(rp);
+        launch_refine(rp, (unsigned)jobs, stream);
         e->launches++;
         CU(cudaGetLastError());
     }
@@ -1324,6 +1404,7 @@ int dsac_refined_jp6_device(dsac_engine* e, int32_t n, double* d_jp6, void* stre
     if (!e) return DSAC_ERR_ARG;
     if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_refined_jp6_device: a submitted pass has not been awaited (dsac_forward_wait)");
     if (!d_jp6) return fail(e, DSAC_ERR_ARG, "dsac_refined_jp6_device: null output");
+    if (int rc = cameras_unchanged(e, "dsac_refined_jp6_device")) return rc;
     const double* pose;
     size_t count;
     if (n >= 1 && e->cur_n == n && e->cur_coords) {   // soft-argmax pass: one refined pose per frame

@@ -11,6 +11,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include "camera.cuh"
 #include "pose_math.cuh"
 #include "sampler.cuh"
 
@@ -115,6 +116,7 @@ struct SampleParams {
     const int32_t* pix;      // [n or 1][N][2]
     int pix_stride;          // N*2 or 0 (shared grid)
     double f, cx, cy;
+    const Cam* cams;         // [n] or null: the camera of every frame is f, cx, cy
     int H, T, thr;
     uint32_t seed, skip;
     int max_candidates;
@@ -234,7 +236,13 @@ __device__ __forceinline__ int cand_parse_fast(const unsigned char* vals, int q,
 //   B  cheap conservative filter, one thread per candidate, no block barriers
 //   C  queue the ~2% that need the full fp64 P3P, in candidate order
 //   D  full solve + reprojection check on the queue, ordered compaction of the accepted
-__global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS) k_sample(SampleParams p) {
+// PER_FRAME: the camera of the CTA's frame comes from the per-frame table (SampleParams::cams) in place of p.f, p.cx, p.cy.
+template <bool PER_FRAME>
+__global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS) k_sample_t(SampleParams p) {
+    if constexpr (PER_FRAME) {
+        const Cam c = p.cams[blockIdx.y];
+        p.f = c.f; p.cx = c.cx; p.cy = c.cy;
+    }
     extern __shared__ __align__(16) unsigned char k1_smem_raw[];
     K1Smem& sm = *reinterpret_cast<K1Smem*>(k1_smem_raw);
 
@@ -681,6 +689,9 @@ __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS) k_sample(SamplePara
     }
 }
 
+constexpr auto k_sample = k_sample_t<false>;
+constexpr auto k_sample_cam = k_sample_t<true>;
+
 // ------------------------------------------------------------------ K2: fused scoring
 struct ScoreParams {
     const int16_t* coords;   // [n][N][3]
@@ -696,6 +707,7 @@ struct ScoreParams {
     unsigned int* frame_counter;  // [n] zero-initialised, self-resetting
     int H, tile, tiles_per_frame;
     float cxf, cyf;
+    const Cam* cams;         // [n] or null: the principal point of every frame is cxf, cyf (the focal length is inside hyp_P)
     float thr, kbeta;        // kbeta = beta * log2(e)
     double alpha;
     int external_scores;     // 1: scores come from the score hook, only the softmax tail runs
@@ -856,8 +868,8 @@ __device__ __noinline__ void score_tile_guarded(const float* s_P, int nh, const 
 #ifndef K2_MIN_BLOCKS
 #define K2_MIN_BLOCKS 3
 #endif
-template <bool WRITE_DM>
-__global__ void __launch_bounds__(K2_THREADS, K2_MIN_BLOCKS) k_score(ScoreParams p) {
+template <bool WRITE_DM, bool PER_FRAME>
+__device__ __forceinline__ void k_score_body(const ScoreParams& p) {
     __shared__ __align__(128) float s_P[K2_MAX_TILE * 12];
     __shared__ __align__(8) unsigned long long s_bar;
     __shared__ float s_part[K2_WARPS][K2_MAX_TILE];
@@ -875,6 +887,8 @@ __global__ void __launch_bounds__(K2_THREADS, K2_MIN_BLOCKS) k_score(ScoreParams
         {
             const int16_t* c = p.coords + (size_t)frame * DSAC_N_CONST * 3;
             const int2* px = reinterpret_cast<const int2*>(p.pix + (size_t)frame * p.pix_stride);
+            float cxf = p.cxf, cyf = p.cyf;
+            if constexpr (PER_FRAME) { cxf = (float)p.cams[frame].cx; cyf = (float)p.cams[frame].cy; }
 #pragma unroll
             for (int j = 0; j < K2_PTS; j++) {
                 const int pt = (j < 4) ? 4 * tid + j : 4 * K2_THREADS + tid;   // four adjacent cells + one: 16-byte stores of the error rows
@@ -882,8 +896,8 @@ __global__ void __launch_bounds__(K2_THREADS, K2_MIN_BLOCKS) k_score(ScoreParams
                 Y[j] = (float)__ldg(c + pt * 3 + 1);
                 Z[j] = (float)__ldg(c + pt * 3 + 2);
                 int2 q = __ldg(px + pt);
-                pu[j] = (float)q.x - p.cxf;
-                pv[j] = (float)q.y - p.cyf;
+                pu[j] = (float)q.x - cxf;
+                pv[j] = (float)q.y - cyf;
             }
         }
         // stage the tile's 3x4 projection rows (48 bytes per hypothesis, contiguous) in shared memory by TMA: one thread
@@ -924,5 +938,11 @@ __global__ void __launch_bounds__(K2_THREADS, K2_MIN_BLOCKS) k_score(ScoreParams
         softargmax_tail(p, frame, s_red);
     }
 }
+
+template <bool WRITE_DM>
+__global__ void __launch_bounds__(K2_THREADS, K2_MIN_BLOCKS) k_score(ScoreParams p) { k_score_body<WRITE_DM, false>(p); }
+// the same with the per-frame principal points (ScoreParams::cams)
+template <bool WRITE_DM>
+__global__ void __launch_bounds__(K2_THREADS, K2_MIN_BLOCKS) k_score_cam(ScoreParams p) { k_score_body<WRITE_DM, true>(p); }
 
 }  // namespace dsac

@@ -16,6 +16,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include "camera.cuh"
 #include "lm_math.cuh"
 #include "pose_math.cuh"
 
@@ -38,6 +39,7 @@ struct RefineParams {
     int pix_stride;
     const uint16_t* perm;       // [ref_steps][N]  (std::shuffle with default mt19937, cnn_softam.h:1104-1114)
     double f, cx, cy;
+    const Cam* cams;            // [n_frames] or null: the camera of every frame is f, cx, cy
     int thr, inlier_count, ref_steps;
     // jobs
     int n_jobs;
@@ -123,7 +125,8 @@ __device__ double max_loss_dev(const double R1[9], const double t1[3], const dou
 //            compute in its next CALC_J if the trial is accepted -- the same numbers); warp 0 reduces, decides,
 //            solves the damped 6x6 system in registers and builds the next R / dR/dr across its lanes.  Two block
 //            barriers per trial.
-__global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine(RefineParams p) {
+template <bool PER_FRAME>
+__device__ __forceinline__ void k_refine_body(const RefineParams& p) {
     // the frame's scene coordinates (int16 mm, this job's perturbation applied) and pixel positions, staged once per job:
     // every refinement step reads all of them for the inlier flags and the selected ones in each LM pass
     __shared__ short s_cX[DSAC_N_CONST], s_cY[DSAC_N_CONST], s_cZ[DSAC_N_CONST];
@@ -141,6 +144,7 @@ __global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine(RefinePara
     const int job = blockIdx.x;
     const int frame = p.job_frame ? p.job_frame[job] : job;
     if (frame < 0) return;  // unused job slot
+    const Cam cam = frame_cam<PER_FRAME>(p, frame);
     const int16_t* coords = p.coords + (size_t)frame * DSAC_N_CONST * 3;
     const int32_t* pix = p.pix + (size_t)frame * p.pix_stride;
     int pert_idx = -1, pert_delta = 0;
@@ -167,7 +171,7 @@ __global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine(RefinePara
     __syncthreads();
 
     const float thrf = (float)p.thr;
-    const float cxf = (float)p.cx, cyf = (float)p.cy, c_abs = fabsf(cxf) + fabsf(cyf);
+    const float cxf = (float)cam.cx, cyf = (float)cam.cy, c_abs = fabsf(cxf) + fabsf(cyf);
 
     // inlier flags of the current pose s_pose (getDiffMap, cnn_softam.h:319-362, reduced to "< threshold")
     auto inlier_flags = [&]() {
@@ -183,7 +187,7 @@ __global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine(RefinePara
             for (int k = 0; k < 12; k++) {
                 const int row = k >> 2, col = k & 3;
                 const double v = (col < 3) ? R[row * 3 + col] : pose[3 + row];
-                if (lane == k) s_Pf[k] = (float)(row < 2 ? p.f * v : v);
+                if (lane == k) s_Pf[k] = (float)(row < 2 ? cam.f * v : v);
             }
         }
         __syncthreads();
@@ -204,7 +208,7 @@ __global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine(RefinePara
 #pragma unroll
                     for (int k = 0; k < 9; k++) Rd[k] = s_Rd[k];
                     t[0] = s_pose[3]; t[1] = s_pose[4]; t[2] = s_pose[5];
-                    flag = reproj_error_exact(Rd, t, (double)X, (double)Y, (double)Z, p.f, p.cx, p.cy, fu, fv) < thrf;
+                    flag = reproj_error_exact(Rd, t, (double)X, (double)Y, (double)Z, cam.f, cam.cx, cam.cy, fu, fv) < thrf;
                 }
             }
             const uint32_t m = __ballot_sync(0xffffffffu, flag);
@@ -236,7 +240,7 @@ __global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine(RefinePara
         for (int k = 0; k < K4_PPT; k++)
             if (tid + k * K4_THREADS < n)
                 lm_point_contrib(s_R, s_J, s_param, (double)selX[k], (double)selY[k], (double)selZ[k], (double)selU[k], (double)selV[k],
-                                 p.f, p.cx, p.cy, v);
+                                 cam.f, cam.cx, cam.cy, v);
         // transposed butterfly: after the step with offset `off` every lane keeps half of its values; lane L ends with sum L
 #pragma unroll
         for (int half = 16, off = 16; half >= 1; half >>= 1, off >>= 1) {
@@ -361,6 +365,16 @@ __global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine(RefinePara
             p.correct[job] = (re < 5 && te < 50) ? 1 : 0;
         }
     }
+}
+
+__global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine(RefineParams p) { k_refine_body<false>(p); }
+// the same with the per-frame camera table (RefineParams::cams)
+__global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine_cam(RefineParams p) { k_refine_body<true>(p); }
+
+// one CTA per job, with the instantiation the parameters ask for
+inline void launch_refine(const RefineParams& p, unsigned jobs, cudaStream_t stream) {
+    if (p.cams) k_refine_cam<<<jobs, K4_THREADS, 0, stream>>>(p);
+    else k_refine<<<jobs, K4_THREADS, 0, stream>>>(p);
 }
 
 }  // namespace dsac

@@ -92,7 +92,8 @@ struct K1SplitParams {
 // steps), so one THREAD per stream does it here, all streams at once and next to the cell records, instead of thread 0 of
 // every k1_slot CTA with the other 255 threads waiting.  A warp seeds 32 streams in lockstep
 // and hands every 32 steps over through a shared-memory tile, so that the states reach HBM as 128-byte rows.
-__global__ void __launch_bounds__(256) k1_cells(K1SplitParams q, int n_frames, int seed_blocks) {
+template <bool PER_FRAME>
+__device__ __forceinline__ void k1_cells_body(const K1SplitParams& q, int n_frames, int seed_blocks) {
     const SampleParams& p = q.sp;
     __shared__ uint32_t tile[32][33];
     if ((int)blockIdx.x < seed_blocks) {
@@ -130,16 +131,20 @@ __global__ void __launch_bounds__(256) k1_cells(K1SplitParams q, int n_frames, i
     const int frame = i / DSAC_N_CONST, c = i - frame * DSAC_N_CONST;
     const int16_t* coords = p.coords + (size_t)frame * DSAC_N_CONST * 3;
     const int32_t* pix = p.pix + (size_t)frame * p.pix_stride;
-    const double inv_f = 1. / p.f, cx_f = p.cx * inv_f, cy_f = p.cy * inv_f;
+    const Cam cam = frame_cam<PER_FRAME>(p, frame);
+    const double inv_f = 1. / cam.f, cx_f = cam.cx * inv_f, cy_f = cam.cy * inv_f;
     CellRec r;
     r.X = __ldg(coords + c * 3); r.Y = __ldg(coords + c * 3 + 1); r.Z = __ldg(coords + c * 3 + 2); r.pad = 0;
-    r.xn = (float)(((double)__ldg(pix + c * 2) - p.cx) * inv_f);       // cv::undistortPoints rounds to float (p3p_pixel)
-    r.yn = (float)(((double)__ldg(pix + c * 2 + 1) - p.cy) * inv_f);
-    const double mu = r.xn * p.f + p.cx, mv = r.yn * p.f + p.cy;     // float * double
+    r.xn = (float)(((double)__ldg(pix + c * 2) - cam.cx) * inv_f);       // cv::undistortPoints rounds to float (p3p_pixel)
+    r.yn = (float)(((double)__ldg(pix + c * 2 + 1) - cam.cy) * inv_f);
+    const double mu = r.xn * cam.f + cam.cx, mv = r.yn * cam.f + cam.cy;     // float * double
     const double u = inv_f * mu - cx_f, v = inv_f * mv - cy_f;
     r.k = rsqrt(u * u + v * v + 1);
     q.celltab[i] = r;
 }
+__global__ void __launch_bounds__(256) k1_cells(K1SplitParams q, int n_frames, int seed_blocks) { k1_cells_body<false>(q, n_frames, seed_blocks); }
+// the same with the per-frame camera table (SampleParams::cams)
+__global__ void __launch_bounds__(256) k1_cells_cam(K1SplitParams q, int n_frames, int seed_blocks) { k1_cells_body<true>(q, n_frames, seed_blocks); }
 
 // ------------------------------------------------------------------ k1_slot
 template <int NW>
@@ -1231,13 +1236,20 @@ struct K1FSmem {
 // the global queue with one atomic per item.  A group barrier only when moving on to another frame's table.
 // The group: NTHREADS threads synchronising with barrier BAR_ID (0: the whole CTA of k1_filter; >= 1: the filter warps
 // of k1_fused); items first_item, first_item + item_stride, ...  The transaction barriers must have been initialised.
-template <int BAR_ID, int NTHREADS>
+// PER_FRAME: the camera is the frame's entry of SampleParams::cams instead of the engine's in the constant bank.  It
+// travels with the frame's cell table: the thread that issues the table's copy into buffer b first writes the camera and
+// the three values derived from it to camv[b][0..6) (shared memory), which the barrier's release / acquire makes visible
+// to everybody who waits for the table (camv is referenced by the per-frame instantiation only).  Every candidate reads
+// them from there: held in registers across the candidate loop they do not fit beside the filter's 128.
+template <int BAR_ID, int NTHREADS, bool PER_FRAME = false>
 __device__ __forceinline__ void k1_filter_body(const K1SplitParams& q, K1FSmem& sm, const int tid, const int first_item, const int item_stride) {
+    __shared__ double camv[2][6];
     const SampleParams& p = q.sp;
     const int lane = tid & 31, warp_id = tid >> 5;
     const int n_items = q.wq_n[q.qidx];
     const uint2* wq = q.wq + (size_t)q.qidx * q.wq_stride;
-    const double inv_f = 1. / p.f, cx_f = p.cx * inv_f, cy_f = p.cy * inv_f;
+    Cam cam = frame_cam<false>(p, 0);
+    double inv_f = 1. / cam.f, cx_f = cam.cx * inv_f, cy_f = cam.cy * inv_f;
     unsigned short* wl = sm.wlist[warp_id];
     constexpr uint32_t TABLE_BYTES = (uint32_t)(sizeof(CellRec) * DSAC_N_CONST);
     int cur = 0;
@@ -1245,9 +1257,18 @@ __device__ __forceinline__ void k1_filter_body(const K1SplitParams& q, K1FSmem& 
     uint32_t parity[2] = {0u, 0u};
     bool pending[2] = {false, false};    // a copy into buffer b has been issued and not yet waited for
     unsigned long long n_flagged = 0;
+    auto stage_cam = [&](int b, int frame) {   // (the issuing thread only)
+        if constexpr (PER_FRAME) {
+            const Cam c = p.cams[frame];
+            const double inv = 1. / c.f;
+            double* cv = camv[b];
+            cv[0] = c.f; cv[1] = c.cx; cv[2] = c.cy; cv[3] = inv; cv[4] = c.cx * inv; cv[5] = c.cy * inv;
+        }
+    };
     int item = first_item;
     if (item < n_items) {
         const int f0 = (int)(wq[item].x >> 7) / p.T;
+        if (tid == 0) stage_cam(0, f0);
         if (tid == 0) tma_load_1d(sm.cell[0], q.celltab + (size_t)f0 * DSAC_N_CONST, TABLE_BYTES, &sm.mbar[0]);
         frame_in[0] = f0;
         pending[0] = true;
@@ -1263,6 +1284,7 @@ __device__ __forceinline__ void k1_filter_body(const K1SplitParams& q, K1FSmem& 
         if (nxt < n_items) {
             nframe = (int)(wq[nxt].x >> 7) / p.T;
             if (nframe != frame && frame_in[cur ^ 1] != nframe) {
+                if (tid == 0) stage_cam(cur ^ 1, nframe);
                 if (tid == 0) tma_load_1d(sm.cell[cur ^ 1], q.celltab + (size_t)nframe * DSAC_N_CONST, TABLE_BYTES, &sm.mbar[cur ^ 1]);
                 frame_in[cur ^ 1] = nframe;
                 pending[cur ^ 1] = true;
@@ -1287,7 +1309,11 @@ __device__ __forceinline__ void k1_filter_body(const K1SplitParams& q, K1FSmem& 
             bool need = false;
             if (i < n_here) {
                 const int cells[4] = {(int)(c.x & 0xffffu), (int)(c.x >> 16), (int)(c.y & 0xffffu), (int)(c.y >> 16)};
-                need = k1_filter_candidate(cell, cells, p.f, p.cx, p.cy, inv_f, cx_f, cy_f, (double)p.thr);
+                if constexpr (PER_FRAME) {
+                    const volatile double* cv = camv[cur];   // (volatile: read for every candidate, not kept across the loop)
+                    cam.f = cv[0]; cam.cx = cv[1]; cam.cy = cv[2]; inv_f = cv[3]; cx_f = cv[4]; cy_f = cv[5];
+                }
+                need = k1_filter_candidate(cell, cells, cam.f, cam.cx, cam.cy, inv_f, cx_f, cy_f, (double)p.thr);
             }
             const uint32_t bits = __ballot_sync(0xffffffffu, need);
             if (need) wl[cnt + __popc(bits & ((1u << lane) - 1u))] = (unsigned short)(base + i);
@@ -1317,6 +1343,14 @@ __global__ void __maxnreg__(K1F_MAXREG) k1_filter(K1SplitParams q) {
     if (threadIdx.x == 0) { mbar_init(&sm.mbar[0]); mbar_init(&sm.mbar[1]); }
     __syncthreads();
     k1_filter_body<0, K1F_THREADS>(q, sm, threadIdx.x, blockIdx.x, gridDim.x);
+}
+// the same with the per-frame camera table (SampleParams::cams)
+__global__ void __maxnreg__(K1F_MAXREG) k1_filter_cam(K1SplitParams q) {
+    extern __shared__ __align__(128) unsigned char k1f_smem_raw[];
+    K1FSmem& sm = *reinterpret_cast<K1FSmem*>(k1f_smem_raw);
+    if (threadIdx.x == 0) { mbar_init(&sm.mbar[0]); mbar_init(&sm.mbar[1]); }
+    __syncthreads();
+    k1_filter_body<0, K1F_THREADS, true>(q, sm, threadIdx.x, blockIdx.x, gridDim.x);
 }
 
 // ------------------------------------------------------------------ k1_fused
@@ -1365,7 +1399,7 @@ __global__ void __launch_bounds__(K1X_THREADS, 1) k1_fused(K1SplitParams qf, K1S
 #ifndef K1V_MIN_BLOCKS
 #define K1V_MIN_BLOCKS 4
 #endif
-template <int GROUP>
+template <int GROUP, bool PER_FRAME = false>
 __device__ __forceinline__ void k1_solve_body(const K1SplitParams& q) {
     const SampleParams& p = q.sp;
     const int tid = threadIdx.x;
@@ -1379,11 +1413,13 @@ __device__ __forceinline__ void k1_solve_body(const K1SplitParams& q) {
         double e2 = 1.7976931348623157e308, R[9], t[3];
         float obj[12], img[8];
         int nsol = 0, slot = 0, ci = 0;
+        Cam cam = frame_cam<false>(p, 0);
         if (qi < n_q) {
             const uint32_t ent = q.fq[qi];
             slot = (int)(ent >> K1S_IDX_BITS);
             ci = (int)(ent & ((1u << K1S_IDX_BITS) - 1u));
             const int frame = slot / p.T;
+            if constexpr (PER_FRAME) cam = p.cams[frame];
             const uint2 c = q.cells[(size_t)slot * q.cap + ci];
             const int cells[4] = {(int)(c.x & 0xffffu), (int)(c.x >> 16), (int)(c.y & 0xffffu), (int)(c.y >> 16)};
             const CellRec* cell = q.celltab + (size_t)frame * DSAC_N_CONST;
@@ -1392,16 +1428,16 @@ __device__ __forceinline__ void k1_solve_body(const K1SplitParams& q) {
 #pragma unroll
             for (int j = 0; j < 4; j++) {
                 const CellRec r = cell[cells[j]];
-                pr.mu[j] = r.xn * p.f + p.cx;   // float * double
-                pr.mv[j] = r.yn * p.f + p.cy;
+                pr.mu[j] = r.xn * cam.f + cam.cx;   // float * double
+                pr.mv[j] = r.yn * cam.f + cam.cy;
                 pr.X[j][0] = (double)r.X; pr.X[j][1] = (double)r.Y; pr.X[j][2] = (double)r.Z;
                 obj[j * 3] = (float)pr.X[j][0]; obj[j * 3 + 1] = (float)pr.X[j][1]; obj[j * 3 + 2] = (float)pr.X[j][2];
                 img[j * 2] = (float)__ldg(pix + cells[j] * 2);
                 img[j * 2 + 1] = (float)__ldg(pix + cells[j] * 2 + 1);
             }
             P3PFront fr;
-            p3p_front(pr, p.f, p.cx, p.cy, fr);
-            nsol = p3p_full(pr, fr, p.f, p.cx, p.cy, R, t, &e2, sub * ROOTS, (sub + 1) * ROOTS);
+            p3p_front(pr, cam.f, cam.cx, cam.cy, fr);
+            nsol = p3p_full(pr, fr, cam.f, cam.cx, cam.cy, R, t, &e2, sub * ROOTS, (sub + 1) * ROOTS);
             if (nsol == 0) e2 = 1.7976931348623157e308;
         }
         // minimum over the group; ties go to the lower root index, as the sequential loop would
@@ -1414,7 +1450,7 @@ __device__ __forceinline__ void k1_solve_body(const K1SplitParams& q) {
             if (oe < be || (oe == be && ol < bl)) { be = oe; bl = ol; }
         }
         if (nsol > 0 && bl == sub)
-            ok = minimal_set_accept(obj, img, p.f, p.cx, p.cy, p.thr, R, t, e2, rvec, tvec, &fragile);
+            ok = minimal_set_accept(obj, img, cam.f, cam.cx, cam.cy, p.thr, R, t, e2, rvec, tvec, &fragile);
         if (fragile) atomicAdd(p.n_fragile, 1ull);
         if (ok) {
             double* po = q.pose_out + ((size_t)slot * q.cap + ci) * 6;
@@ -1430,5 +1466,24 @@ __device__ __forceinline__ void k1_solve_body(const K1SplitParams& q) {
 // candidate's chain, and the four roots are that chain's longest part)
 __global__ void __launch_bounds__(K1V_THREADS, K1V_MIN_BLOCKS) k1_solve(K1SplitParams q) { k1_solve_body<K1V_GROUP>(q); }
 __global__ void __launch_bounds__(K1V_THREADS, K1V_MIN_BLOCKS) k1_solve4(K1SplitParams q) { k1_solve_body<4>(q); }
+// the same with the per-frame camera table (SampleParams::cams)
+__global__ void __launch_bounds__(K1V_THREADS, K1V_MIN_BLOCKS) k1_solve_cam(K1SplitParams q) { k1_solve_body<K1V_GROUP, true>(q); }
+__global__ void __launch_bounds__(K1V_THREADS, K1V_MIN_BLOCKS) k1_solve4_cam(K1SplitParams q) { k1_solve_body<4, true>(q); }
+
+// The generator is camera-free: the selection of k1_slot writes the rows (fR0 ft0), (fR1 ft1) of hyp_P with the engine's
+// focal length.  With a per-frame camera table this kernel, launched after the sampler, writes them again from the
+// hypothesis pose with the frame's own focal length, in the selection's arithmetic.  One thread per (frame, hypothesis).
+__global__ void __launch_bounds__(256) k1_focal_rows_cam(SampleParams p, int n_frames) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_frames * p.H) return;
+    const double f = p.cams[i / p.H].f;
+    const double* hp = p.hyp_pose + (size_t)i * 6;
+    const double rvec[3] = {hp[0], hp[1], hp[2]}, tvec[2] = {hp[3], hp[4]};
+    double Rm[9];
+    rodrigues_v2m(rvec, Rm);
+    float4* P = reinterpret_cast<float4*>(p.hyp_P + (size_t)i * 12);
+    P[0] = make_float4((float)(f * Rm[0]), (float)(f * Rm[1]), (float)(f * Rm[2]), (float)(f * tvec[0]));
+    P[1] = make_float4((float)(f * Rm[3]), (float)(f * Rm[4]), (float)(f * Rm[5]), (float)(f * tvec[1]));
+}
 
 }  // namespace dsac

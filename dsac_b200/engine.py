@@ -19,7 +19,7 @@ ST_SAMPLER_EXHAUSTED, ST_REFINE_ABORTED = 1, 2
 # every symbol include/dsac_b200.h declares
 EXPORTS = [
     "dsac_default_config", "dsac_engine_create", "dsac_engine_destroy", "dsac_last_error", "dsac_engine_config",
-    "dsac_forward", "dsac_forward_submit", "dsac_forward_wait", "dsac_forward_device", "dsac_fetch", "dsac_device_view_get", "dsac_set_stages",
+    "dsac_forward", "dsac_forward_submit", "dsac_forward_wait", "dsac_forward_device", "dsac_fetch", "dsac_device_view_get", "dsac_set_cameras", "dsac_set_stages",
     "dsac_set_tail_split", "dsac_launch_count", "dsac_sampler_profile", "dsac_sampler_profile_read", "dsac_debug_spec_result", "dsac_set_score_hook", "dsac_set_score_backward_hook", "dsac_backward", "dsac_backward_device", "dsac_forward_dsac", "dsac_forward_dsac_device",
     "dsac_backward_dsac", "dsac_backward_dsac_device", "dsac_refined_jp6_device", "dsac_backward_pose_device",
     "dsac_backward_dsac_pose_device", "dsac_gather_patches_device", "dsac_coords_from_prediction_device", "dsac_kabsch",
@@ -160,6 +160,7 @@ def load(build_if_missing=True):
     lib.dsac_sampler_profile.argtypes = [C.c_void_p, C.c_int32]
     lib.dsac_sampler_profile_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     lib.dsac_debug_spec_result.argtypes = [C.c_void_p, C.c_void_p]
+    lib.dsac_set_cameras.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.dsac_set_stages.argtypes = [C.c_void_p, C.c_uint32]
     lib.dsac_set_tail_split.argtypes = [C.c_void_p, C.c_int32]
     lib.dsac_set_score_hook.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
@@ -368,6 +369,17 @@ class Engine:
         out = (C.c_int32 * 8)()
         self._check(self.lib.dsac_debug_spec_result(self.h, out))
         return [int(x) for x in out]
+
+    def set_cameras(self, cams, stream=None):
+        """dsac_set_cameras: cams float64 [n][3] = (focal, cx, cy) of frame i of the following passes (a host array or CPU
+        tensor), which must then have n frames; None: back to the config's camera.  stream: a cudaStream_t as int."""
+        if cams is None:
+            self._check(self.lib.dsac_set_cameras(self.h, 0, None, None))
+            return
+        cams = np.ascontiguousarray(cams, np.float64)
+        if cams.ndim != 2 or cams.shape[1] != 3:
+            raise ValueError("cameras must be float64 [n][3] (focal, cx, cy), got %s" % (cams.shape,))
+        self._check(self.lib.dsac_set_cameras(self.h, cams.shape[0], _p(cams), C.c_void_p(stream) if stream else None))
 
     def set_tail_split(self, mode):
         """0: off, 1: forward_device + blocking forward (default), 2: submitted passes too (scheduling only)."""

@@ -146,6 +146,26 @@ int dsac_forward_device(dsac_engine* e, int32_t n_frames, int64_t frame0, const 
 int dsac_fetch(dsac_engine* e, int32_t n_frames, dsac_forward_out* out, void* stream);
 int dsac_device_view_get(dsac_engine* e, dsac_device_view* view);
 
+/* Per-frame cameras: one batch may mix focal lengths and principal points (images of different sensors, SfM
+ * reconstructions, scale augmentation).  The reference has one camera per process (getCamMat(), properties.cpp:308-323);
+ * without this call so does the engine (dsac_config's). */
+typedef struct dsac_camera { double focal, cx, cy; } dsac_camera;   /* getCamMat(), per frame */
+
+/* Cameras of the frames of the following passes: cams[i] belongs to frame i of the call (local index, like coords --
+ * NOT the global frame0 + i).  cams is a HOST array of n entries; it is validated here (focal finite and > 0, cx / cy
+ * finite), staged in page-locked memory the engine owns and copied to an engine-owned device buffer on `stream`
+ * (a cudaStream_t, NULL = default), after the engine's last forward pass; the passes that follow wait for the copy on
+ * whichever stream they run.  The setting is sticky: every later forward on this engine (dsac_forward, _submit, _device,
+ * dsac_forward_dsac, _device) must have n_frames == n (else DSAC_ERR_ARG) until it is changed.  cams == NULL (n
+ * ignored): back to dsac_config's camera.
+ * DSAC_ERR_ARG, with the engine left as it was: n outside [1, max_frames], a bad entry (dsac_last_error names its
+ * index), or a submitted pass that has not been awaited.
+ * A backward pass, and dsac_refined_jp6_device, belong to the forward pass before them and so to its cameras: after a
+ * dsac_set_cameras they return DSAC_ERR_ARG until the next forward.
+ * dsac_score_maps_device and the pre-training data paths keep dsac_config's / dsac_rgbd_camera's single camera: their
+ * frame index is a dataset index, not a pass index.  No distortion and no separate fx / fy: the reference has neither. */
+int dsac_set_cameras(dsac_engine* e, int32_t n, const dsac_camera* cams, void* stream);
+
 /* Stage control for measurement: which stages dsac_forward_device runs. */
 #define DSAC_STAGE_SAMPLE 1u
 #define DSAC_STAGE_SCORE 2u
