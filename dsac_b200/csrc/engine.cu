@@ -8,6 +8,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdarg>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -29,6 +30,9 @@
 using namespace dsac;
 
 static_assert(sizeof(Cam) == sizeof(dsac_camera), "Cam mirrors dsac_camera");
+static_assert(sizeof(ObjCam) == sizeof(dsac_rgbd_camera) && offsetof(ObjCam, sensor_trans) == offsetof(dsac_rgbd_camera, sensor_trans) &&
+                  offsetof(ObjCam, raw_data) == offsetof(dsac_rgbd_camera, raw_data),
+              "ObjCam mirrors dsac_rgbd_camera");
 
 static std::string g_create_error;
 
@@ -128,6 +132,14 @@ struct dsac_engine {
     Event ev_cams;                  // recorded after that copy: the staging is rewritten, and a pass starts, only after it
     int cams_n = 0;
     unsigned long long cams_gen = 0, fwd_cams_gen = 0;   // generation of the setting, and the one the last forward ran with
+    // per-dataset cameras of the pre-training data paths (dsac_set_dataset_cameras), indexed by dataset frame; grow-only.
+    // ds_cams_n == 0: no table.  ds_cam0 is entry 0 on the host: the frame size and raw_data every entry shares.
+    DevMem<ObjCam> d_ds_cams;
+    PinnedMem<ObjCam> h_ds_cams;    // staging of the copy to d_ds_cams
+    Event ev_ds_cams;               // recorded after that copy: the staging is rewritten, and a reader starts, only after it
+    Event ev_ds_use;                // recorded after the last launch that read the table: a new table is copied after it
+    int ds_cams_n = 0;
+    ObjCam ds_cam0{};
     // state
     DevMem<uint16_t> d_perm;
     DevMem<double> d_hyp_pose;
@@ -387,6 +399,8 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
     CUC(e->d_cams.reserve(n * sizeof(Cam)));
     CUC(e->h_cams.reserve(n * sizeof(dsac_camera)));
     CUC(cudaEventCreateWithFlags(e->ev_cams.put(), cudaEventDisableTiming));
+    CUC(cudaEventCreateWithFlags(e->ev_ds_cams.put(), cudaEventDisableTiming));
+    CUC(cudaEventCreateWithFlags(e->ev_ds_use.put(), cudaEventDisableTiming));
     CUC(cudaMemset(e->d_frame_counter, 0, n * sizeof(unsigned int)));
     CUC(cudaMemset(e->d_fragile, 0, sizeof(unsigned long long)));
     if (getenv("DSAC_K1_TIMERS")) {
@@ -1498,6 +1512,62 @@ static bool obj_cam(dsac_engine* e, const dsac_rgbd_camera* c, ObjCam* o) {
     return true;
 }
 
+int dsac_set_dataset_cameras(dsac_engine* e, int32_t n_frames, const dsac_rgbd_camera* cams, void* stream_v) {
+    if (!e) return DSAC_ERR_ARG;
+    if (!cams) {
+        e->ds_cams_n = 0;
+        return DSAC_OK;
+    }
+    if (n_frames < 1) return fail(e, DSAC_ERR_ARG, "dsac_set_dataset_cameras: n_frames %d must be >= 1", n_frames);
+    const dsac_rgbd_camera& c0 = cams[0];
+    for (int32_t i = 0; i < n_frames; i++) {
+        const dsac_rgbd_camera& c = cams[i];
+        bool finite = std::isfinite(c.x_shift) && std::isfinite(c.y_shift) && std::isfinite(c.raw_x_shift) &&
+                      std::isfinite(c.raw_y_shift);
+        for (int k = 0; k < 16; k++) finite = finite && std::isfinite(c.sensor_trans[k]);
+        if (!std::isfinite(c.focal) || !(c.focal > 0) || (c.raw_data && (!std::isfinite(c.secondary_focal) || !(c.secondary_focal > 0))) ||
+            !finite)
+            return fail(e, DSAC_ERR_ARG, "dsac_set_dataset_cameras: camera %d is invalid (focal %g, and secondary focal %g with raw_data, "
+                        "must be finite and > 0; shifts and sensor_trans finite)", i, c.focal, c.secondary_focal);
+        if (c.width < 1 || c.height < 1 || c.width != c0.width || c.height != c0.height || !c.raw_data != !c0.raw_data)
+            return fail(e, DSAC_ERR_ARG, "dsac_set_dataset_cameras: camera %d is %dx%d with raw_data %d; every camera must be %dx%d "
+                        "with raw_data %d like camera 0", i, c.width, c.height, c.raw_data, c0.width, c0.height, c0.raw_data);
+    }
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    const size_t bytes = (size_t)n_frames * sizeof(ObjCam);
+    CU(cudaSetDevice(e->cfg.device));
+    CU(cudaEventSynchronize(e->ev_ds_cams));          // the previous copy has left the staging buffer
+    e->ds_cams_n = 0;                                  // (a failed copy leaves no table)
+    CU(e->h_ds_cams.reserve(bytes));
+    memcpy(e->h_ds_cams.get(), cams, bytes);
+    for (int32_t i = 0; i < n_frames; i++) e->h_ds_cams.get()[i].raw_data = cams[i].raw_data ? 1 : 0;
+    CU(cudaStreamWaitEvent(stream, e->ev_ds_use, 0));  // the last reader of the old table is done with it
+    CU(e->d_ds_cams.reserve(bytes));
+    CU(cudaMemcpyAsync(e->d_ds_cams.get(), e->h_ds_cams.get(), bytes, cudaMemcpyHostToDevice, stream));
+    CU(cudaEventRecord(e->ev_ds_cams, stream));
+    e->ds_cam0 = e->h_ds_cams.get()[0];
+    e->ds_cams_n = n_frames;
+    return DSAC_OK;
+}
+
+// The check of an entry point called with cam == NULL, which means the per-dataset table: a table is set and covers the
+// call's n frames.
+static int dataset_cameras_check(dsac_engine* e, const char* who, int32_t n) {
+    if (!e->ds_cams_n) return fail(e, DSAC_ERR_ARG, "%s: cam is NULL and no dataset cameras are set (dsac_set_dataset_cameras)", who);
+    if (n != e->ds_cams_n)
+        return fail(e, DSAC_ERR_ARG, "%s: %d frames, but the dataset cameras cover %d", who, n, e->ds_cams_n);
+    return DSAC_OK;
+}
+// Around the launches that read the table: `stream` waits for the table's copy, and the next copy waits for them.
+static int dataset_cameras_wait(dsac_engine* e, cudaStream_t stream) {
+    CU(cudaStreamWaitEvent(stream, e->ev_ds_cams, 0));
+    return DSAC_OK;
+}
+static int dataset_cameras_done(dsac_engine* e, cudaStream_t stream) {
+    CU(cudaEventRecord(e->ev_ds_use, stream));
+    return DSAC_OK;
+}
+
 static inline unsigned grid_of(size_t n, int threads) { return (unsigned)((n + threads - 1) / threads); }
 
 __global__ void k_dropped_status(int n, const int32_t* dropped, uint32_t* status) {
@@ -1509,19 +1579,30 @@ int dsac_register_depth_device(dsac_engine* e, const dsac_rgbd_camera* cam, int3
                                uint16_t* d_depth, int32_t* d_dropped, uint32_t* d_status, void* stream_v) {
     if (!e) return DSAC_ERR_ARG;
     ObjCam c;
-    if (!obj_cam(e, cam, &c)) return DSAC_ERR_ARG;
+    if (cam ? !obj_cam(e, cam, &c) : false) return DSAC_ERR_ARG;
+    if (!cam) {
+        if (int rc = dataset_cameras_check(e, "dsac_register_depth_device", n)) return rc;
+        c = e->ds_cam0;
+    }
     if (n < 1 || !d_raw || !d_depth || d_raw == d_depth || (d_status && !d_dropped))
         return fail(e, DSAC_ERR_ARG, "dsac_register_depth_device: bad arguments");
     CU(cudaSetDevice(e->cfg.device));
     cudaStream_t stream = (cudaStream_t)stream_v;
+    // cam == NULL: the per-dataset table; only a registration reads it (raw_data 0 passes the depth through)
+    const bool table = !cam && c.raw_data;
+    if (table)
+        if (int rc = dataset_cameras_wait(e, stream)) return rc;
     const size_t count = (size_t)n * c.width * c.height;
     if (d_dropped) CU(cudaMemsetAsync(d_dropped, 0, (size_t)n * sizeof(int32_t), stream));
     if (c.raw_data) {
         CU(e->d_reg_keys.reserve(count * sizeof(uint64_t)));
         CU(cudaMemsetAsync(e->d_reg_keys, 0, count * sizeof(uint64_t), stream));
     }
-    k_register_depth<<<grid_of(count, 256), 256, 0, stream>>>(c, n, d_raw, e->d_reg_keys, d_depth, d_dropped);
+    if (table) k_register_depth_cam<<<grid_of(count, 256), 256, 0, stream>>>(c, e->d_ds_cams, n, d_raw, e->d_reg_keys, d_depth, d_dropped);
+    else k_register_depth<<<grid_of(count, 256), 256, 0, stream>>>(c, n, d_raw, e->d_reg_keys, d_depth, d_dropped);
     e->launches++;
+    if (table)
+        if (int rc = dataset_cameras_done(e, stream)) return rc;
     if (c.raw_data) {
         k_register_finish<<<grid_of(count, 256), 256, 0, stream>>>(count, e->d_reg_keys, d_depth);
         e->launches++;
@@ -1538,12 +1619,23 @@ int dsac_obj_coords_device(dsac_engine* e, const dsac_rgbd_camera* cam, int32_t 
                            const uint16_t* d_depth, const double* d_poses, int16_t* d_coords, void* stream_v) {
     if (!e) return DSAC_ERR_ARG;
     ObjCam c;
-    if (!obj_cam(e, cam, &c)) return DSAC_ERR_ARG;
+    if (cam ? !obj_cam(e, cam, &c) : false) return DSAC_ERR_ARG;
+    if (!cam) {
+        if (int rc = dataset_cameras_check(e, "dsac_obj_coords_device", n_frames)) return rc;
+        c = e->ds_cam0;
+    }
     if (n < 1 || n_frames < 1 || (!d_idx && n > n_frames) || !d_depth || !d_poses || !d_coords)
         return fail(e, DSAC_ERR_ARG, "dsac_obj_coords_device: bad arguments");
     CU(cudaSetDevice(e->cfg.device));
+    cudaStream_t stream = (cudaStream_t)stream_v;
     const size_t count = (size_t)n * c.width * c.height;
-    k_obj_coords<<<grid_of(count, 256), 256, 0, (cudaStream_t)stream_v>>>(c, n_frames, n, d_idx, d_depth, d_poses, d_coords);
+    if (cam) {
+        k_obj_coords<<<grid_of(count, 256), 256, 0, stream>>>(c, n_frames, n, d_idx, d_depth, d_poses, d_coords);
+    } else {
+        if (int rc = dataset_cameras_wait(e, stream)) return rc;
+        k_obj_coords_cam<<<grid_of(count, 256), 256, 0, stream>>>(c, e->d_ds_cams, n_frames, n, d_idx, d_depth, d_poses, d_coords);
+        if (int rc = dataset_cameras_done(e, stream)) return rc;
+    }
     e->launches++;
     CU(cudaGetLastError());
     return DSAC_OK;
@@ -1565,7 +1657,11 @@ int dsac_obj_draw_device(dsac_engine* e, const dsac_rgbd_camera* cam, int32_t n_
                          uint32_t* d_status, void* stream_v) {
     if (!e) return DSAC_ERR_ARG;
     ObjDrawParams p;
-    if (!obj_cam(e, cam, &p.cam)) return DSAC_ERR_ARG;
+    if (cam ? !obj_cam(e, cam, &p.cam) : false) return DSAC_ERR_ARG;
+    if (!cam) {
+        if (int rc = dataset_cameras_check(e, "dsac_obj_draw_device", n_frames)) return rc;
+        p.cam = e->ds_cam0;   // the frame size of every entry
+    }
     if (p.cam.width <= UP_PATCH || p.cam.height <= UP_PATCH)
         return fail(e, DSAC_ERR_ARG, "a %dx%d frame holds no %d-pixel patch centre", p.cam.width, p.cam.height, UP_PATCH);
     if (n_frames < 1 || n_images < 1 || n_patches < 1 || n_streams < 1 || max_attempts < 32 || !d_depth || !d_poses ||
@@ -1576,7 +1672,16 @@ int dsac_obj_draw_device(dsac_engine* e, const dsac_rgbd_camera* cam, int32_t n_
     p.n_frames = n_frames; p.n_images = n_images; p.n_patches = n_patches; p.n_streams = n_streams;
     p.max_attempts = max_attempts; p.state = d_state;
     p.img = d_img; p.centre = d_centre; p.label = d_label; p.status = d_status;
-    k_obj_draw<<<grid_of(n_streams, OBJ_DRAW_WARPS), 32 * OBJ_DRAW_WARPS, 0, (cudaStream_t)stream_v>>>(p);
+    p.cams = nullptr;
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    if (cam) {
+        k_obj_draw<<<grid_of(n_streams, OBJ_DRAW_WARPS), 32 * OBJ_DRAW_WARPS, 0, stream>>>(p);
+    } else {
+        if (int rc = dataset_cameras_wait(e, stream)) return rc;
+        p.cams = e->d_ds_cams;
+        k_obj_draw_cam<<<grid_of(n_streams, OBJ_DRAW_WARPS), 32 * OBJ_DRAW_WARPS, 0, stream>>>(p);
+        if (int rc = dataset_cameras_done(e, stream)) return rc;
+    }
     e->launches++;
     CU(cudaGetLastError());
     return DSAC_OK;
@@ -1641,7 +1746,16 @@ int dsac_score_maps_device(dsac_engine* e, int32_t n_images, int32_t hyps_per_im
     p.hyps = hyps_per_image;
     p.f = e->cfg.focal; p.cxf = (float)e->cfg.cx; p.cyf = (float)e->cfg.cy; p.temperature = temperature;
     p.maps = d_maps; p.labels = d_labels; p.correct = d_correct;
-    k_score_maps<<<(unsigned)(n_images * hyps_per_image), SM_THREADS, 0, (cudaStream_t)stream_v>>>(p);
+    p.cams = nullptr; p.n_cams = 0;
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    if (!e->ds_cams_n) {
+        k_score_maps<<<(unsigned)(n_images * hyps_per_image), SM_THREADS, 0, stream>>>(p);
+    } else {   // the camera of frame img[i] (getCamMat of its dataset entry)
+        if (int rc = dataset_cameras_wait(e, stream)) return rc;
+        p.cams = e->d_ds_cams; p.n_cams = e->ds_cams_n;
+        k_score_maps_cam<<<(unsigned)(n_images * hyps_per_image), SM_THREADS, 0, stream>>>(p);
+        if (int rc = dataset_cameras_done(e, stream)) return rc;
+    }
     e->launches++;
     CU(cudaGetLastError());
     return DSAC_OK;

@@ -3,6 +3,8 @@
 //   * k_obj_coords:       Dataset::getObj (dataset.h:226-255): pxToEye (dataset.cpp:37-56) then Hypothesis::invTransform
 //   * k_obj_draw:         assembleData's random draw (train_obj.cpp:47-102): image index, then accepted patch centres
 //   * k_gather_patches_at: the patch gather of upstream.cuh at per-patch (frame, x, y) into a device-resident dataset
+// The first three have _cam instantiations that take each frame's camera from the per-dataset table
+// (dsac_set_dataset_cameras); the instantiations without it are the single-camera code.
 // The per-pixel arithmetic is in DSAC_HD functions, so that the host build (tests/host_shim) can be checked against the
 // numpy restatement on a machine without a GPU.  Every operation is spelled with a round-to-nearest intrinsic on the
 // device so that nvcc cannot contract it into an FMA the x86 reference never executes.
@@ -159,8 +161,12 @@ DSAC_HD uint32_t lemire_draw(uint32_t range, Next&& next) {
 // y inner, so the last source pixel in that order wins; the 64-bit key ((x * rows + y) << 16) | depth ordered by
 // atomicMax keeps exactly that one.  Targets outside the image (undefined behaviour in the reference) are dropped and
 // counted per frame.  With raw_data = 0 the depth passes through.
-__global__ void k_register_depth(ObjCam c, int n, const uint16_t* __restrict__ raw, uint64_t* __restrict__ keys,
-                                 uint16_t* __restrict__ out, int32_t* __restrict__ dropped) {
+// TABLE: the per-dataset camera table (dsac_set_dataset_cameras) gives each frame its own mapping; `c` still holds the
+// frame size and raw_data, which every entry shares.
+template <bool TABLE>
+__device__ __forceinline__ void register_depth_body(const ObjCam& c, const ObjCam* __restrict__ cams, int n,
+                                                    const uint16_t* __restrict__ raw, uint64_t* __restrict__ keys,
+                                                    uint16_t* __restrict__ out, int32_t* __restrict__ dropped) {
     const int W = c.width, H = c.height;
     const size_t plane = (size_t)W * H;
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -171,13 +177,22 @@ __global__ void k_register_depth(ObjCam c, int n, const uint16_t* __restrict__ r
     if (!c.raw_data) { out[i] = d; return; }
     if (d == 0) return;
     int nx, ny;
-    map_depth_to_rgb(c, x, y, d, &nx, &ny);
+    if constexpr (TABLE) map_depth_to_rgb(cams[f], x, y, d, &nx, &ny);
+    else map_depth_to_rgb(c, x, y, d, &nx, &ny);
     if (nx < 0 || ny < 0 || nx >= W || ny >= H) {
         if (dropped) atomicAdd(dropped + f, 1);
         return;
     }
     const unsigned long long key = ((unsigned long long)((uint32_t)x * (uint32_t)H + (uint32_t)y) << 16) | d;
     atomicMax(reinterpret_cast<unsigned long long*>(keys) + (size_t)f * plane + (size_t)ny * W + nx, key);
+}
+__global__ void k_register_depth(ObjCam c, int n, const uint16_t* __restrict__ raw, uint64_t* __restrict__ keys,
+                                 uint16_t* __restrict__ out, int32_t* __restrict__ dropped) {
+    register_depth_body<false>(c, nullptr, n, raw, keys, out, dropped);
+}
+__global__ void k_register_depth_cam(ObjCam c, const ObjCam* __restrict__ cams, int n, const uint16_t* __restrict__ raw,
+                                     uint64_t* __restrict__ keys, uint16_t* __restrict__ out, int32_t* __restrict__ dropped) {
+    register_depth_body<true>(c, cams, n, raw, keys, out, dropped);
 }
 
 // Pass 2: the registered depth is the winning key's low 16 bits (0 where nothing landed).
@@ -188,8 +203,11 @@ __global__ void k_register_finish(size_t count, const uint64_t* __restrict__ key
 
 // ----------------------------------------------------------------------------- getObj
 // A listed frame outside [0, n_frames) yields a zero image (the entry point documents it; RGBDScene refuses such lists).
-__global__ void k_obj_coords(ObjCam c, int n_frames, int n, const int32_t* __restrict__ idx, const uint16_t* __restrict__ depth,
-                             const double* __restrict__ poses, int16_t* __restrict__ out) {
+// TABLE: the camera of frame idx[k] from the per-dataset table, read only for a frame inside the dataset.
+template <bool TABLE>
+__device__ __forceinline__ void obj_coords_body(const ObjCam& c, const ObjCam* __restrict__ cams, int n_frames, int n,
+                                                const int32_t* __restrict__ idx, const uint16_t* __restrict__ depth,
+                                                const double* __restrict__ poses, int16_t* __restrict__ out) {
     const int W = c.width, H = c.height;
     const size_t plane = (size_t)W * H;
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -201,8 +219,17 @@ __global__ void k_obj_coords(ObjCam c, int n_frames, int n, const int32_t* __res
     ObjPose p;
     obj_pose(poses + (size_t)f * 12, &p);
     int16_t v[3];
-    obj_coord(c, p, x, y, depth[(size_t)f * plane + pix], v);
+    if constexpr (TABLE) obj_coord(cams[f], p, x, y, depth[(size_t)f * plane + pix], v);
+    else obj_coord(c, p, x, y, depth[(size_t)f * plane + pix], v);
     out[i * 3] = v[0]; out[i * 3 + 1] = v[1]; out[i * 3 + 2] = v[2];
+}
+__global__ void k_obj_coords(ObjCam c, int n_frames, int n, const int32_t* __restrict__ idx, const uint16_t* __restrict__ depth,
+                             const double* __restrict__ poses, int16_t* __restrict__ out) {
+    obj_coords_body<false>(c, nullptr, n_frames, n, idx, depth, poses, out);
+}
+__global__ void k_obj_coords_cam(ObjCam c, const ObjCam* __restrict__ cams, int n_frames, int n, const int32_t* __restrict__ idx,
+                                 const uint16_t* __restrict__ depth, const double* __restrict__ poses, int16_t* __restrict__ out) {
+    obj_coords_body<true>(c, cams, n_frames, n, idx, depth, poses, out);
 }
 
 // ----------------------------------------------------------------------------- ThreadRand state
@@ -216,7 +243,8 @@ __global__ void k_obj_rng_init(uint32_t seed, int T, uint32_t* __restrict__ stat
 
 // ----------------------------------------------------------------------------- assembleData's draw
 struct ObjDrawParams {
-    ObjCam cam;
+    ObjCam cam;                // the camera; with a table, its frame size (which every entry shares)
+    const ObjCam* cams;        // [n_frames] per-dataset cameras (k_obj_draw_cam only)
     const uint16_t* depth;     // [F][H][W] registered depth
     const double* poses;       // [F][12] jp poses
     int n_frames, n_images, n_patches, n_streams, max_attempts;
@@ -263,7 +291,10 @@ struct ObjStream {
 // pairing holds only while no word is a Lemire rejection; the first lane whose pair contains one ends the batch there and
 // the pair at that point is drawn sequentially (rejections are rare: threshold / 2^32 per word).  A patch that is still
 // unmet after max_attempts (>= 32) pairs ends its image with DSAC_ST_OBJ_DRAW_EXHAUSTED; the reference would loop forever.
-__global__ void __launch_bounds__(32 * OBJ_DRAW_WARPS) k_obj_draw(ObjDrawParams p) {
+// TABLE: once the warp has drawn an image's frame it loads that frame's camera for the labels; the words consumed are
+// the same.
+template <bool TABLE>
+__device__ __forceinline__ void obj_draw_body(const ObjDrawParams& p) {
     __shared__ uint32_t sbuf[OBJ_DRAW_WARPS][2][MT_N];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int t = blockIdx.x * OBJ_DRAW_WARPS + warp;
@@ -293,6 +324,13 @@ __global__ void __launch_bounds__(32 * OBJ_DRAW_WARPS) k_obj_draw(ObjDrawParams 
         const int f = (int)s.draw(&pos, (uint32_t)p.n_frames);
         ObjPose pose;
         obj_pose(p.poses + (size_t)f * 12, &pose);
+        ObjCam fc;   // TABLE: the fields getObj reads, of frame f
+        if constexpr (TABLE) {
+            const ObjCam* t = p.cams + f;
+            fc.focal = t->focal; fc.x_shift = t->x_shift; fc.y_shift = t->y_shift;
+            fc.width = c.width; fc.height = c.height;
+        }
+        const ObjCam& lc = TABLE ? fc : c;
         const uint16_t* dep = p.depth + (size_t)f * plane;
         const size_t out0 = (size_t)i * p.n_patches;
         int done = 0, attempts = 0;
@@ -309,7 +347,7 @@ __global__ void __launch_bounds__(32 * OBJ_DRAW_WARPS) k_obj_draw(ObjDrawParams 
             const bool rej = ((uint32_t)px < thx) || ((uint32_t)py < thy);
             const int x = (int)(px >> 32) + OBJ_HALF, y = (int)(py >> 32) + OBJ_HALF;
             int16_t v[3];
-            obj_coord(c, pose, x, y, dep[(size_t)y * c.width + x], v);
+            obj_coord(lc, pose, x, y, dep[(size_t)y * c.width + x], v);
             const bool acc = !rej && on_obj(v);
             const unsigned rmask = __ballot_sync(0xffffffffu, rej);
             const int r = rmask ? __ffs(rmask) - 1 : 32;
@@ -336,7 +374,7 @@ __global__ void __launch_bounds__(32 * OBJ_DRAW_WARPS) k_obj_draw(ObjDrawParams 
                 const int sy = (int)s.draw(&pos, ry) + OBJ_HALF;
                 attempts++;
                 int16_t w[3];
-                obj_coord(c, pose, sx, sy, dep[(size_t)sy * c.width + sx], w);
+                obj_coord(lc, pose, sx, sy, dep[(size_t)sy * c.width + sx], w);
                 if (on_obj(w)) {
                     if (lane == 0) emit(done, sx, sy, w);
                     done++;
@@ -360,6 +398,8 @@ __global__ void __launch_bounds__(32 * OBJ_DRAW_WARPS) k_obj_draw(ObjDrawParams 
     for (int k = lane; k < MT_N; k += 32) st[k] = b[k];
     if (lane == 0) st[MT_N] = (uint32_t)(second ? pos - MT_N : pos);
 }
+__global__ void __launch_bounds__(32 * OBJ_DRAW_WARPS) k_obj_draw(ObjDrawParams p) { obj_draw_body<false>(p); }
+__global__ void __launch_bounds__(32 * OBJ_DRAW_WARPS) k_obj_draw_cam(ObjDrawParams p) { obj_draw_body<true>(p); }
 
 // ----------------------------------------------------------------------------- patch gather at listed centres
 struct GatherAtParams {

@@ -3,7 +3,7 @@
 //                    (stochasticSubSample, cnn.h:348-374) and, per hypothesis, the drift level and getRandHyp (:48-72)
 //   * k_score_maps:  per (image, hypothesis) poseGT * getRandHyp, the 40x40 reprojection-error image of getDiffMap
 //                    (cnn.h:384-427) with K2's arithmetic, the label -temperature * max(angle deg, |dt| mm / 10) and the
-//                    5 deg / 50 mm flag
+//                    5 deg / 50 mm flag; k_score_maps_cam with each frame's getCamMat() camera from the per-dataset table
 // The random draws and the pose arithmetic are DSAC_HD functions, so that the host build (tests/host_shim/score_shim.cpp)
 // can be checked against the numpy restatement and against libstdc++'s own distributions on a machine without a GPU.
 // Every double operation of the draw is spelled with a round-to-nearest intrinsic on the device (objtrain.cuh's OT_*),
@@ -148,6 +148,18 @@ DSAC_HD void score_sample(const double* gt_jp, const double v[6], double f, floa
     out->P[11] = (float)t[2];
 }
 
+// The camera train_score.cpp projects with, getCamMat() (properties.cpp:308-311, train_score.cpp:178), of a dataset
+// camera: the focal length, and a principal point of the INTEGER width / 2 (and height / 2) plus the float shift, in
+// float.  getObj's principal point is width / 2.f + x_shift instead (dataset.cpp:51); the two differ on odd frame sizes
+// (DESIGN.md quirk Q27).  k_score_maps takes dsac_config's camera in the same form: f, and cx / cy rounded to float.
+struct ScoreCam {
+    double f;
+    float cx, cy;
+};
+DSAC_HD ScoreCam score_cam(const ObjCam& c) {
+    return ScoreCam{(double)c.focal, OT_FADD((float)(c.width / 2), c.x_shift), OT_FADD((float)(c.height / 2), c.y_shift)};
+}
+
 #if defined(__CUDACC__) && !defined(DSAC_HOST_ONLY)
 
 // ----------------------------------------------------------------------------- assembleData's draw
@@ -239,6 +251,8 @@ struct ScoreMapsParams {
     int hyps;
     double f;
     float cxf, cyf, temperature;
+    const ObjCam* cams;      // [n_cams] per-dataset cameras, indexed by img (k_score_maps_cam only)
+    int n_cams;
     float* maps;             // [n_images * hyps][1600]
     double* labels;          // [n_images * hyps]
     int32_t* correct;        // [n_images * hyps] or null
@@ -249,13 +263,32 @@ constexpr int SM_PTS = DSAC_N_CONST / SM_THREADS;
 
 // One CTA per (image, hypothesis): thread 0 builds the noisy pose, its label and its projection rows; every thread then
 // projects 5 of the 1600 cells with score_pair_error, the function K2 applies to the forward's diffmaps.
-__global__ void __launch_bounds__(SM_THREADS) k_score_maps(ScoreMapsParams p) {
+// TABLE: the camera is score_cam of frame img[i]'s entry in the per-dataset table; an img[i] outside the table is not
+// read and gives a NaN map and label and correct = 0.
+template <bool TABLE>
+__device__ __forceinline__ void score_maps_body(const ScoreMapsParams& p) {
     __shared__ float s_P[12];
     const size_t k = blockIdx.x;
     const int i = (int)(k / (size_t)p.hyps);
+    double f = p.f;
+    float cxf = p.cxf, cyf = p.cyf;
+    if constexpr (TABLE) {
+        const int fr = p.img[i];
+        if (fr < 0 || fr >= p.n_cams) {
+            float* out = p.maps + k * DSAC_N_CONST;
+            for (int pt = threadIdx.x; pt < DSAC_N_CONST; pt += SM_THREADS) out[pt] = __int_as_float(0x7fffffff);
+            if (threadIdx.x == 0) {
+                p.labels[k] = __longlong_as_double(0x7fffffffffffffffll);
+                if (p.correct) p.correct[k] = 0;
+            }
+            return;
+        }
+        const ScoreCam sc = score_cam(p.cams[fr]);
+        f = sc.f; cxf = sc.cx; cyf = sc.cy;
+    }
     if (threadIdx.x == 0) {
         ScoreSample smp;
-        score_sample(p.gt_jp + (size_t)p.img[i] * 12, p.noise + k * 6, p.f, p.temperature, &smp);
+        score_sample(p.gt_jp + (size_t)p.img[i] * 12, p.noise + k * 6, f, p.temperature, &smp);
         for (int j = 0; j < 12; j++) s_P[j] = smp.P[j];
         p.labels[k] = smp.label;
         if (p.correct) p.correct[k] = smp.correct;
@@ -271,9 +304,11 @@ __global__ void __launch_bounds__(SM_THREADS) k_score_maps(ScoreMapsParams p) {
         float az;
         out[pt] = score_pair_error<true>(s_P[0], s_P[1], s_P[2], s_P[3], s_P[4], s_P[5], s_P[6], s_P[7], s_P[8], s_P[9],
                                          s_P[10], s_P[11], (float)__ldg(c + pt * 3), (float)__ldg(c + pt * 3 + 1),
-                                         (float)__ldg(c + pt * 3 + 2), (float)q.x - p.cxf, (float)q.y - p.cyf, &az);
+                                         (float)__ldg(c + pt * 3 + 2), (float)q.x - cxf, (float)q.y - cyf, &az);
     }
 }
+__global__ void __launch_bounds__(SM_THREADS) k_score_maps(ScoreMapsParams p) { score_maps_body<false>(p); }
+__global__ void __launch_bounds__(SM_THREADS) k_score_maps_cam(ScoreMapsParams p) { score_maps_body<true>(p); }
 
 #endif  // device code
 

@@ -25,7 +25,7 @@ EXPORTS = [
     "dsac_backward_dsac_pose_device", "dsac_gather_patches_device", "dsac_coords_from_prediction_device", "dsac_kabsch",
     "dsac_stochastic_subsample",
     "dsac_synth_frames", "dsac_version",
-    "dsac_default_rgbd_camera", "dsac_register_depth_device", "dsac_obj_coords_device", "dsac_obj_rng_init_device",
+    "dsac_default_rgbd_camera", "dsac_set_dataset_cameras", "dsac_register_depth_device", "dsac_obj_coords_device", "dsac_obj_rng_init_device",
     "dsac_obj_draw_device", "dsac_gather_patches_at_device", "dsac_shuffle_permutation",
     "dsac_score_draw_device", "dsac_score_maps_device", "dsac_shuffle_permutations",
 ]
@@ -68,6 +68,14 @@ def default_rgbd_camera(**kw):
         else:
             setattr(cam, k, v)
     return cam
+
+
+def camera_table(cams):
+    """A sequence of RGBDCamera as the contiguous dsac_rgbd_camera array dsac_set_dataset_cameras reads (a ctypes array
+    of RGBDCamera is returned as it is)."""
+    if isinstance(cams, C.Array) and cams._type_ is RGBDCamera:
+        return cams
+    return (RGBDCamera * len(cams))(*cams)
 
 
 def shuffle_permutation(n, seed=5489):
@@ -188,6 +196,7 @@ def load(build_if_missing=True):
                                       C.c_int32, C.c_double, C.c_double, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p]
     lib.dsac_default_rgbd_camera.argtypes = [C.POINTER(RGBDCamera)]
+    lib.dsac_set_dataset_cameras.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.dsac_register_depth_device.argtypes = [C.c_void_p, C.POINTER(RGBDCamera), C.c_int32, C.c_void_p, C.c_void_p,
                                                C.c_void_p, C.c_void_p, C.c_void_p]
     lib.dsac_obj_coords_device.argtypes = [C.c_void_p, C.POINTER(RGBDCamera), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
@@ -329,6 +338,7 @@ class Engine:
             raise RuntimeError("dsac_engine_create failed (%d): %s" % (rc, self.lib.dsac_last_error(None).decode()))
         self.h = h
         self._hook = None
+        self._dataset_cameras = None   # bytes of the dataset camera table installed by set_dataset_cameras, or None
         self.passes = 0   # forward passes started on this engine: the engine holds one pass, autograd.py checks it is still its own
 
     def close(self):
@@ -575,11 +585,35 @@ class Engine:
         return R.reshape(n, 3, 3), t
 
     # ------------------------------------------------------------------ coordinate-CNN pre-training data path
-    # Raw device pointers as ints; `cam` is an RGBDCamera; stream: a cudaStream_t as int or None.
+    # Raw device pointers as ints; `cam` is an RGBDCamera, or None for the dataset camera table (set_dataset_cameras);
+    # stream: a cudaStream_t as int or None.
+
+    def set_dataset_cameras(self, cams, stream=None):
+        """dsac_set_dataset_cameras: cams, a sequence of RGBDCamera, one per dataset frame, becomes the table that
+        cam=None means in the pre-training calls and that score_maps_device projects with; None clears it."""
+        if cams is None:
+            self._check(self.lib.dsac_set_dataset_cameras(self.h, 0, None, None))
+            self._dataset_cameras = None
+            return
+        table = camera_table(cams)
+        self._check(self.lib.dsac_set_dataset_cameras(self.h, len(cams), C.cast(table, C.c_void_p),
+                                                      C.c_void_p(stream) if stream else None))
+        self._dataset_cameras = bytes(table)
+
+    def use_dataset_cameras(self, cams, stream=None):
+        """set_dataset_cameras(cams) unless this wrapper installed the same table last (None: no table), so that
+        several scenes can take turns on one engine without copying their tables on every call."""
+        key = None if cams is None else bytes(camera_table(cams))
+        if key != self._dataset_cameras:
+            self.set_dataset_cameras(cams, stream)
+
+    @staticmethod
+    def _cam(cam):
+        return C.byref(cam) if cam is not None else None
 
     def register_depth_device(self, cam, n, d_raw, d_depth, d_dropped=None, d_status=None, stream=None):
         """dsac_register_depth_device: raw depth [n][H][W] uint16 -> depth registered to the RGB camera."""
-        self._check(self.lib.dsac_register_depth_device(self.h, C.byref(cam), n, C.c_void_p(d_raw), C.c_void_p(d_depth),
+        self._check(self.lib.dsac_register_depth_device(self.h, self._cam(cam), n, C.c_void_p(d_raw), C.c_void_p(d_depth),
                                                         C.c_void_p(d_dropped) if d_dropped else None,
                                                         C.c_void_p(d_status) if d_status else None,
                                                         C.c_void_p(stream) if stream else None))
@@ -587,7 +621,7 @@ class Engine:
     def obj_coords_device(self, cam, n_frames, n, d_depth, d_poses, d_coords, d_idx=None, stream=None):
         """dsac_obj_coords_device: getObj images [n][H][W][3] int16 (mm) of frames d_idx[0..n) (None: 0..n) of a
         dataset of n_frames frames."""
-        self._check(self.lib.dsac_obj_coords_device(self.h, C.byref(cam), n_frames, n, C.c_void_p(d_idx) if d_idx else None,
+        self._check(self.lib.dsac_obj_coords_device(self.h, self._cam(cam), n_frames, n, C.c_void_p(d_idx) if d_idx else None,
                                                     C.c_void_p(d_depth), C.c_void_p(d_poses), C.c_void_p(d_coords),
                                                     C.c_void_p(stream) if stream else None))
 
@@ -599,7 +633,7 @@ class Engine:
     def obj_draw_device(self, cam, n_frames, d_depth, d_poses, n_images, n_patches, n_streams, max_attempts, d_state,
                         d_img, d_centre, d_label, d_status, stream=None):
         """dsac_obj_draw_device: one round of assembleData's draw."""
-        self._check(self.lib.dsac_obj_draw_device(self.h, C.byref(cam), n_frames, C.c_void_p(d_depth), C.c_void_p(d_poses),
+        self._check(self.lib.dsac_obj_draw_device(self.h, self._cam(cam), n_frames, C.c_void_p(d_depth), C.c_void_p(d_poses),
                                                   n_images, n_patches, n_streams, max_attempts, C.c_void_p(d_state),
                                                   C.c_void_p(d_img), C.c_void_p(d_centre), C.c_void_p(d_label),
                                                   C.c_void_p(d_status), C.c_void_p(stream) if stream else None))
@@ -626,7 +660,8 @@ class Engine:
     def score_maps_device(self, n_images, hyps_per_image, d_img, d_gt_jp, d_coords, d_pix, d_noise, temperature, d_maps,
                           d_labels, d_correct=None, stream=None):
         """dsac_score_maps_device: reprojection-error images [n][1600], labels [n] and the 5 deg / 50 mm flags of a
-        draw's perturbed ground-truth poses against the coordinate CNN's grids."""
+        draw's perturbed ground-truth poses against the coordinate CNN's grids; with a dataset camera table installed,
+        image i is projected with the camera of frame img[i] (getCamMat), else with the config's camera."""
         self._check(self.lib.dsac_score_maps_device(self.h, n_images, hyps_per_image, C.c_void_p(d_img), C.c_void_p(d_gt_jp),
                                                     C.c_void_p(d_coords), C.c_void_p(d_pix), C.c_void_p(d_noise),
                                                     C.c_float(temperature), C.c_void_p(d_maps), C.c_void_p(d_labels),

@@ -39,18 +39,33 @@ def read_sensor_trans(path):
 
 class RGBDScene:
     """A training set in device memory: bgr [F][H][W][3] uint8, raw depth [F][H][W] uint16 (as the depth PNGs hold it),
-    gt_jp [F][12] (the jp pose as dsac_forward takes it: row-major rotation, translation in mm) and an RGBDCamera whose
-    width / height are the frame size.  The depth is registered to the RGB camera once, here (with cam.raw_data = 0 it is
-    used as given)."""
+    gt_jp [F][12] (the jp pose as dsac_forward takes it: row-major rotation, translation in mm) and its camera: one
+    RGBDCamera for every frame, or a sequence of F, one per frame (frames with their own intrinsics), all with the frame
+    size as width / height and the same raw_data.  The depth is registered to the RGB camera once, here (with raw_data = 0
+    it is used as given).
+
+    cam is the single camera (None with per-frame cameras); cams is the per-frame table (None with one camera).  A scene
+    with per-frame cameras installs its table on the engine (Engine.use_dataset_cameras) before each of its calls if
+    another one is installed, so several scenes can share an engine."""
 
     def __init__(self, engine, bgr, raw_depth, gt_jp, cam=None, device="cuda"):
         self.engine, self.device = engine, device
-        self.cam = cam if cam is not None else E.default_rgbd_camera()
         raw = raw_depth.cpu().numpy() if isinstance(raw_depth, torch.Tensor) else np.asarray(raw_depth)
         raw = np.ascontiguousarray(raw.astype(np.uint16)).view(np.int16)   # the bits; torch has no uint16 arithmetic
         self.n_frames, self.height, self.width = raw.shape
-        if (self.width, self.height) != (self.cam.width, self.cam.height):
-            raise ValueError("frames are %dx%d, the camera %dx%d" % (self.width, self.height, self.cam.width, self.cam.height))
+        if cam is None or isinstance(cam, E.RGBDCamera):
+            self.cam = cam if cam is not None else E.default_rgbd_camera()
+            self.cams = None
+            shapes = [(self.cam.width, self.cam.height)]
+        else:
+            self.cam = None
+            self.cams = E.camera_table(list(cam))
+            if len(self.cams) != self.n_frames:
+                raise ValueError("%d cameras for %d frames" % (len(self.cams), self.n_frames))
+            shapes = {(c.width, c.height) for c in self.cams}
+        for w, h in shapes:
+            if (self.width, self.height) != (w, h):
+                raise ValueError("frames are %dx%d, a camera %dx%d" % (self.width, self.height, w, h))
         self.bgr = _dev(bgr, torch.uint8, device)
         if tuple(self.bgr.shape) != (self.n_frames, self.height, self.width, 3):
             raise ValueError("bgr must be [F][H][W][3] uint8 like the depth")
@@ -59,8 +74,16 @@ class RGBDScene:
         self.depth = torch.empty_like(self.raw_depth)
         self.dropped = torch.zeros(self.n_frames, dtype=torch.int32, device=device)
         self.status = torch.zeros(self.n_frames, dtype=torch.int32, device=device)
-        engine.register_depth_device(self.cam, self.n_frames, self.raw_depth.data_ptr(), self.depth.data_ptr(),
+        engine.register_depth_device(self.camera_arg(), self.n_frames, self.raw_depth.data_ptr(), self.depth.data_ptr(),
                                      self.dropped.data_ptr(), self.status.data_ptr(), stream=_stream())
+
+    def camera_arg(self):
+        """The `cam` argument of the engine's data-path calls on this scene: its camera, or None (the dataset camera
+        table) after installing its per-frame table on the engine where another one is installed."""
+        if self.cams is None:
+            return self.cam
+        self.engine.use_dataset_cameras(self.cams, stream=_stream())
+        return None
 
     def depth_u16(self):
         """The registered depth as a host uint16 array."""
@@ -74,7 +97,7 @@ class RGBDScene:
             raise IndexError("frame indices must lie in [0, %d)" % self.n_frames)
         ids = torch.as_tensor(ids, dtype=torch.int32, device=self.device)
         out = torch.empty((len(ids), self.height, self.width, 3), dtype=torch.int16, device=self.device)
-        self.engine.obj_coords_device(self.cam, self.n_frames, len(ids), self.depth.data_ptr(), self.gt_jp.data_ptr(),
+        self.engine.obj_coords_device(self.camera_arg(), self.n_frames, len(ids), self.depth.data_ptr(), self.gt_jp.data_ptr(),
                                       out.data_ptr(),
                                       d_idx=ids.data_ptr(), stream=_stream())
         return out[0] if one else out
@@ -100,7 +123,7 @@ class ObjRound:
         self.centre = torch.empty((n, 2), dtype=torch.int32, device=dev)
         self.label = torch.empty((n, 3), dtype=torch.float32, device=dev)
         self.status = torch.empty(n_images, dtype=torch.int32, device=dev)
-        s.engine.obj_draw_device(s.cam, s.n_frames, s.depth.data_ptr(), s.gt_jp.data_ptr(), n_images, n_patches,
+        s.engine.obj_draw_device(s.camera_arg(), s.n_frames, s.depth.data_ptr(), s.gt_jp.data_ptr(), n_images, n_patches,
                                  self.n_streams, self.max_attempts, self.state.data_ptr(), self.img.data_ptr(),
                                  self.centre.data_ptr(), self.label.data_ptr(), self.status.data_ptr(), stream=_stream())
         return self.img, self.centre, self.label, self.status

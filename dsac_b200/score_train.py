@@ -32,9 +32,12 @@ class ScoreRound:
     """assembleData's rounds on a scene: bgr [F][H][W][3] uint8 and gt_jp [F][12] (the jp pose as dsac_forward takes it:
     row-major rotation, translation in mm) on the device, e.g. an obj_train.RGBDScene's .bgr and .gt_jp.  pipe is a
     coord_cnn.CoordPipeline.  state: [n_streams][625] int32 holding the uint32 words and positions of the OpenMP threads'
-    std::mt19937 engines; every draw continues from it, as ThreadRand's generators do across the reference's rounds."""
+    std::mt19937 engines; every draw continues from it, as ThreadRand's generators do across the reference's rounds.
+    cameras: None projects the error images with the engine's config camera; a sequence of F RGBDCamera (e.g. an
+    RGBDScene's .cams) projects image i with frame img[i]'s camera as getCamMat() gives it, installed on the engine as its
+    dataset camera table before each draw's error images."""
 
-    def __init__(self, engine, bgr, gt_jp, pipe, seed=DEFAULT_THREADRAND_SEED, n_streams=1):
+    def __init__(self, engine, bgr, gt_jp, pipe, seed=DEFAULT_THREADRAND_SEED, n_streams=1, cameras=None):
         self.engine, self.pipe, self.n_streams = engine, pipe, n_streams
         self.bgr = bgr
         self.device = bgr.device
@@ -42,6 +45,9 @@ class ScoreRound:
         if tuple(bgr.shape) != (self.n_frames, self.height, self.width, 3) or bgr.dtype != torch.uint8:
             raise ValueError("bgr must be [F][H][W][3] uint8")
         self.gt_jp = _dev(gt_jp, torch.float64, self.device).reshape(self.n_frames, 12)
+        self.cameras = None if cameras is None else E.camera_table(list(cameras))
+        if self.cameras is not None and len(self.cameras) != self.n_frames:
+            raise ValueError("%d cameras for %d frames" % (len(self.cameras), self.n_frames))
         self.state = torch.empty((n_streams, E.OBJ_STATE_WORDS), dtype=torch.int32, device=self.device)
         engine.obj_rng_init_device(seed, n_streams, self.state.data_ptr(), stream=_stream())
         self.img = self.pix = self.drift = self.noise = self.coords = None
@@ -62,6 +68,7 @@ class ScoreRound:
         maps = torch.empty((n, 1, E.GRID, E.GRID), dtype=torch.float32, device=dev)
         labels = torch.empty(n, dtype=torch.float64, device=dev)
         correct = torch.empty(n, dtype=torch.int32, device=dev)
+        e.use_dataset_cameras(self.cameras, stream=_stream())
         e.score_maps_device(n_images, hyps_per_image, self.img.data_ptr(), self.gt_jp.data_ptr(), self.coords.data_ptr(),
                             self.pix.data_ptr(), self.noise.data_ptr(), temperature, maps.data_ptr(), labels.data_ptr(),
                             correct.data_ptr(), stream=_stream())
@@ -73,17 +80,17 @@ class ScorePretrainer:
     permutation of one continuing std::mt19937(perm_seed) and takes batches of `batch`, one Torch7Adam update per batch
     on nn.AbsCriterion (the mean absolute error) of the network's output on maps - 45 against the labels in float32; the
     learning rate halves after every lr_interval updates.  log: (update, loss) per update, as
-    score_training_loss_*.txt holds it."""
+    score_training_loss_*.txt holds it.  cameras: as ScoreRound's (None: the engine's config camera)."""
 
     def __init__(self, engine, bgr, gt_jp, pipe, model=None, seed=DEFAULT_THREADRAND_SEED, n_streams=1, n_images=100,
                  hyps_per_image=16, batch=64, lr=1e-4, lr_interval=5000, temperature=TEMPERATURE,
-                 perm_seed=DEFAULT_PERM_SEED):
-        self.engine, self.bgr, self.gt_jp, self.pipe = engine, bgr, gt_jp, pipe
+                 perm_seed=DEFAULT_PERM_SEED, cameras=None):
+        self.engine, self.bgr, self.gt_jp, self.pipe, self.cameras = engine, bgr, gt_jp, pipe, cameras
         self.n_images, self.hyps, self.batch, self.lr_interval = n_images, hyps_per_image, batch, lr_interval
         self.temperature, self.perm_seed = temperature, perm_seed
         self.model = (model if model is not None else score_cnn.build_model()).to(bgr.device).train()
         self.opt = Torch7Adam(self.model.parameters(), lr=lr)
-        self.round = ScoreRound(engine, bgr, gt_jp, pipe, seed=seed, n_streams=n_streams)
+        self.round = ScoreRound(engine, bgr, gt_jp, pipe, seed=seed, n_streams=n_streams, cameras=cameras)
         self.rounds = 0
         self.updates = 0
         self.log = []
@@ -124,7 +131,7 @@ class ScorePretrainer:
     def evaluate(self, n_images=100, hyps_per_image=64, seed=DEFAULT_THREADRAND_SEED + 1000):
         """The reference's (compiled-out) validation pass on a fresh draw: batches of `batch` in data order, mean of the
         per-batch losses and the ratio of batches whose selectBest is correct.  Evaluation mode."""
-        r = ScoreRound(self.engine, self.bgr, self.gt_jp, self.pipe, seed=seed)
+        r = ScoreRound(self.engine, self.bgr, self.gt_jp, self.pipe, seed=seed, cameras=self.cameras)
         maps, labels, _ = r.draw(n_images, hyps_per_image, self.temperature)
         self.model.eval()
         losses, best = [], []

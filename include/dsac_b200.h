@@ -162,8 +162,9 @@ typedef struct dsac_camera { double focal, cx, cy; } dsac_camera;   /* getCamMat
  * index), or a submitted pass that has not been awaited.
  * A backward pass, and dsac_refined_jp6_device, belong to the forward pass before them and so to its cameras: after a
  * dsac_set_cameras they return DSAC_ERR_ARG until the next forward.
- * dsac_score_maps_device and the pre-training data paths keep dsac_config's / dsac_rgbd_camera's single camera: their
- * frame index is a dataset index, not a pass index.  No distortion and no separate fx / fy: the reference has neither. */
+ * dsac_score_maps_device and the pre-training data paths do not use this table: their frame index is a dataset index, not
+ * a pass index, and their per-frame cameras come from dsac_set_dataset_cameras.  No distortion and no separate fx / fy:
+ * the reference has neither. */
 int dsac_set_cameras(dsac_engine* e, int32_t n, const dsac_camera* cams, void* stream);
 
 /* Stage control for measurement: which stages dsac_forward_device runs. */
@@ -363,7 +364,21 @@ typedef struct dsac_rgbd_camera {
 /* The reference's defaults, which the shipped 7-Scenes default.config repeats: focal 525, secondary focal 585, no shifts,
  * raw_data 1, 640 x 480; sensor_trans identity (the reference's value when sensorTrans.dat is absent). */
 int dsac_default_rgbd_camera(dsac_rgbd_camera* cam);
-/* getDepth for n frames: raw [n][H][W] uint16 -> depth [n][H][W] uint16 (raw_data 0: a copy).  Where several depth
+/* Per-frame cameras of a dataset (frames with their own intrinsics: SfM reconstructions, several sensors), indexed by
+ * DATASET frame -- unlike dsac_set_cameras' table, which is indexed by the frame of a forward pass; the two are separate.
+ * cams: HOST array [n_frames], one RGB-D camera per dataset frame; NULL clears the table (n_frames ignored).  Validated
+ * here: n_frames >= 1; focal finite and > 0; secondary_focal finite and > 0 where raw_data is set; the shifts and
+ * sensor_trans finite; width, height and raw_data the same in every entry (the dataset arrays are [F][H][W]).  On failure
+ * DSAC_ERR_ARG, dsac_last_error names the index, and the table in force stays as it was.  The table is staged in
+ * page-locked memory and copied to an engine-owned device buffer on `stream` (a cudaStream_t, NULL = default), after the
+ * last call that read the previous table; the calls that read it wait for the copy on whichever stream they run.
+ * With a table set:
+ *   - dsac_register_depth_device, dsac_obj_coords_device and dsac_obj_draw_device take cam == NULL to mean the table;
+ *     their n / n_frames must then equal its size (else DSAC_ERR_ARG, as for cam == NULL without a table);
+ *   - dsac_score_maps_device projects image i with the camera of frame img[i] (see there). */
+int dsac_set_dataset_cameras(dsac_engine* e, int32_t n_frames, const dsac_rgbd_camera* cams, void* stream);
+/* getDepth for n frames: raw [n][H][W] uint16 -> depth [n][H][W] uint16 (raw_data 0: a copy).  cam == NULL: frame f
+ * is registered with dataset camera f (dsac_set_dataset_cameras; n must equal the table's size).  Where several depth
  * pixels land on one RGB pixel the last in the reference's order (x outer, y inner) wins.  Targets outside the image are
  * dropped; dropped [n] (nullable) counts them and status [n] (nullable; needs dropped) gets DSAC_ST_DEPTH_DROPPED.
  * With raw_data the scatter uses a per-pixel buffer the engine owns and grows on demand (growing frees the old one,
@@ -373,7 +388,8 @@ int dsac_register_depth_device(dsac_engine* e, const dsac_rgbd_camera* cam, int3
                                uint16_t* d_depth, int32_t* d_dropped, uint32_t* d_status, void* stream);
 /* getObj: registered depth [n_frames][H][W] and jp poses [n_frames][12] (dsac_forward's gt_jp: row-major rotation,
  * translation in mm; taken through float as jp::info_t holds it) -> int16 scene coordinates [n][H][W][3] in mm of
- * frames idx[0..n) (idx NULL: frames 0..n, n <= n_frames).  A listed index outside [0, n_frames) gives a zero image. */
+ * frames idx[0..n) (idx NULL: frames 0..n, n <= n_frames).  A listed index outside [0, n_frames) gives a zero image.
+ * cam == NULL: frame idx[k] uses dataset camera idx[k] (n_frames must equal the table's size). */
 int dsac_obj_coords_device(dsac_engine* e, const dsac_rgbd_camera* cam, int32_t n_frames, int32_t n, const int32_t* d_idx,
                            const uint16_t* d_depth, const double* d_poses, int16_t* d_coords, void* stream);
 /* ThreadRand::init(seed) for n_streams threads: state [n_streams][625] = std::mt19937(seed + t) words and position. */
@@ -383,7 +399,8 @@ int dsac_obj_rng_init_device(dsac_engine* e, uint32_t seed, int32_t n_streams, u
  * n_patches], centre [..][2], label [..][3] (metres, Vec3f /= 1000) and status [n_images].  state is read and advanced,
  * so consecutive calls continue like the reference's rounds.  A patch not found within max_attempts (>= 32) pairs ends
  * its image: the remaining centres are (-1, -1) and status gets DSAC_ST_OBJ_DRAW_EXHAUSTED.  The frame must exceed 42 px
- * in both dimensions. */
+ * in both dimensions.  cam == NULL: an image's labels use the dataset camera of the frame it drew (n_frames must equal
+ * the table's size); the random words consumed are the same. */
 int dsac_obj_draw_device(dsac_engine* e, const dsac_rgbd_camera* cam, int32_t n_frames, const uint16_t* d_depth,
                          const double* d_poses, int32_t n_images, int32_t n_patches, int32_t n_streams,
                          int32_t max_attempts, uint32_t* d_state, int32_t* d_img, int32_t* d_centre, float* d_label,
@@ -414,7 +431,11 @@ int dsac_score_draw_device(dsac_engine* e, int32_t n_frames, int32_t width, int3
  * is its reprojection-error image against coords [i][1600][3] (mm, the coordinate CNN's grid at pix [i]) with the
  * engine's camera (config focal / cx / cy), clamped at 100 and computed like the forward's diffmaps; labels [k] =
  * -temperature * max(angular error in degrees, translation error in mm / 10); correct [k] (nullable) = 1 where the
- * errors are below 5 degrees and 50 mm.  img must index gt_jp (as dsac_score_draw_device writes it). */
+ * errors are below 5 degrees and 50 mm.  img must index gt_jp (as dsac_score_draw_device writes it).
+ * With a dataset camera table set (dsac_set_dataset_cameras), image i uses the camera of frame img[i] as train_score.cpp
+ * takes it from getCamMat(): focal, cx = float(width / 2 + x_shift) with the INTEGER width / 2, cy likewise (not
+ * getObj's width / 2.f; DESIGN.md quirk Q27).  An img[i] outside the table is not read: its maps and labels are NaN and
+ * correct 0. */
 int dsac_score_maps_device(dsac_engine* e, int32_t n_images, int32_t hyps_per_image, const int32_t* d_img,
                            const double* d_gt_jp, const int16_t* d_coords, const int32_t* d_pix, const double* d_noise,
                            float temperature, float* d_maps, double* d_labels, int32_t* d_correct, void* stream);
