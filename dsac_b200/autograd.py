@@ -23,6 +23,16 @@ own camera: it is applied with Engine.set_cameras before the forward, on the cur
 engine.  None leaves the engine's setting alone.  Changing the cameras between a loss and its backward() makes that
 backward() raise.
 
+`sampling_logits` (float32 [n][1600] on the engine's device, cell y*40+x) draws the pass's minimal sets from
+softmax(logits) instead of uniformly (guided sampling, INTEGRATION.md): the engine reads a detached copy, applied before
+the forward on the current stream, and the setting stays in force on the engine; None leaves it alone.
+sampling_log_prob(engine, logits) is then the log-probability of that draw, float64 [n], differentiable with respect to
+the logits, for a REINFORCE-style gradient:
+
+    loss = softam_loss(engine, pred, pix, gt_jp, frame0=g0, sampling_logits=logits)
+    logp = sampling_log_prob(engine, logits)
+    (loss + (loss.detach() - baseline) * logp).sum().backward()
+
 Everything stays on the device, on torch.cuda.current_stream().  The engine holds one pass: a forward on the same engine
 between a loss and its backward() makes that backward() raise.
 """
@@ -53,6 +63,21 @@ def _check_inputs(engine, prediction, pix, gt_jp, need_gt=True):
 def _set_cameras(engine, prediction, cameras):
     if cameras is not None:
         engine.set_cameras(cameras, torch.cuda.current_stream(prediction.device).cuda_stream)
+
+
+def _set_sampling(engine, prediction, logits):
+    if logits is None:
+        return
+    n = prediction.shape[0]
+    if logits.dtype != torch.float32 or tuple(logits.shape) != (n, _E.N) or logits.device != prediction.device:
+        raise ValueError("sampling_logits must be float32 [%d][%d] on %s, got %s %s on %s"
+                         % (n, _E.N, prediction.device, logits.dtype, tuple(logits.shape), logits.device))
+    copy = logits.detach().contiguous()
+    stream = torch.cuda.current_stream(prediction.device)
+    engine.set_sampling_logits_device(n, copy.data_ptr(), stream.cuda_stream)
+    copy.record_stream(stream)
+    # the pass that follows is sampled with this tensor as it is now (sampling_log_prob checks identity and version)
+    engine._sampling_key = (id(logits), logits._version, engine.passes + 1)
 
 
 def _coords(engine, prediction, stream):
@@ -162,30 +187,67 @@ class _DsacHypotheses(torch.autograd.Function):
         return grad, None, None, None, None, None
 
 
-def softam_loss(engine, prediction, pix, gt_jp, frame0=0, clamp=0.1, cameras=None):
+def softam_loss(engine, prediction, pix, gt_jp, frame0=0, clamp=0.1, cameras=None, sampling_logits=None):
     """Per-frame loss of the soft-argmax pipeline (train_ransac_softam.cpp) on `prediction`, float64 [n]; differentiable
     with respect to `prediction`.  frame0: global index of the first frame (keys the sampler streams)."""
     _set_cameras(engine, prediction, cameras)
+    _set_sampling(engine, prediction, sampling_logits)
     return _SoftamLoss.apply(prediction, engine, pix, gt_jp, int(frame0), float(clamp))
 
 
-def dsac_expected_loss(engine, prediction, pix, gt_jp, frame0=0, random_draw=True, clamp=0.1, cameras=None):
+def dsac_expected_loss(engine, prediction, pix, gt_jp, frame0=0, random_draw=True, clamp=0.1, cameras=None,
+                       sampling_logits=None):
     """Per-frame expected loss of the DSAC / RANSAC variant (train_ransac.cpp) on `prediction`, float64 [n];
     differentiable with respect to `prediction`."""
     _set_cameras(engine, prediction, cameras)
+    _set_sampling(engine, prediction, sampling_logits)
     return _DsacExpectedLoss.apply(prediction, engine, pix, gt_jp, int(frame0), bool(random_draw), float(clamp))
 
 
-def softam_pose(engine, prediction, pix, frame0=0, clamp=0.1, cameras=None):
+def softam_pose(engine, prediction, pix, frame0=0, clamp=0.1, cameras=None, sampling_logits=None):
     """Refined pose of every frame of the soft-argmax pipeline as a jp 6-vector [rodrigues(R); t in mm], float64 [n][6];
     differentiable with respect to `prediction`.  Needs no ground truth."""
     _set_cameras(engine, prediction, cameras)
+    _set_sampling(engine, prediction, sampling_logits)
     return _SoftamPose.apply(prediction, engine, pix, int(frame0), float(clamp))
 
 
-def dsac_hypotheses(engine, prediction, pix, frame0=0, random_draw=True, clamp=0.1, cameras=None):
+def dsac_hypotheses(engine, prediction, pix, frame0=0, random_draw=True, clamp=0.1, cameras=None, sampling_logits=None):
     """(sf [n][H], refined jp 6-vectors [n][H][6]) of the DSAC / RANSAC variant, both float64 and differentiable with
     respect to `prediction`.  The gradient through the poses covers the hypotheses with sf > 1e-4 whose incoming
     gradient is nonzero; an output that receives no gradient costs nothing in the backward."""
     _set_cameras(engine, prediction, cameras)
+    _set_sampling(engine, prediction, sampling_logits)
     return _DsacHypotheses.apply(prediction, engine, pix, int(frame0), bool(random_draw), float(clamp))
+
+
+class _SamplingLogProb(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, logits, engine):
+        n = logits.shape[0]
+        stream = torch.cuda.current_stream(logits.device).cuda_stream
+        logp = torch.empty(n, dtype=torch.float64, device=logits.device)
+        engine.sampling_log_prob_device(n, logp.data_ptr(), stream)
+        ctx.engine, ctx.pass_id, ctx.n = engine, engine.passes, n
+        return logp
+
+    @staticmethod
+    def backward(ctx, grad_logp):
+        if ctx.engine.passes != ctx.pass_id:
+            raise RuntimeError("the engine ran another forward pass after this log-probability was computed")
+        g = grad_logp.detach().to(torch.float64).contiguous()
+        grad = torch.empty((ctx.n, _E.N), dtype=torch.float32, device=g.device)
+        ctx.engine.sampling_log_prob_backward_device(ctx.n, g.data_ptr(), grad.data_ptr(), torch.cuda.current_stream(g.device).cuda_stream)
+        return grad, None
+
+
+def sampling_log_prob(engine, logits):
+    """Log-probability of the minimal sets the engine's last pass drew, float64 [n]: per frame the sum over every
+    candidate up to each stream's last accepted one (accepted and rejected alike) of the log-probability of its four
+    cells in draw order.  Differentiable with respect to `logits`, which must be the tensor that pass was sampled with
+    (sampling_logits=), unmodified since."""
+    key = getattr(engine, "_sampling_key", None)
+    if key is None or key[0] != id(logits) or key[1] != logits._version or key[2] != engine.passes:
+        raise RuntimeError("the engine's last pass was not sampled with this logits tensor as it is now "
+                           "(pass it as sampling_logits= to the forward, and do not modify it in between)")
+    return _SamplingLogProb.apply(logits, engine)

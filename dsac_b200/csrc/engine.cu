@@ -22,6 +22,7 @@
 #include "kernels.cuh"
 #include "refine.cuh"
 #include "sampler_split.cuh"
+#include "guided.cuh"
 #include "train.cuh"
 #include "upstream.cuh"
 #include "objtrain.cuh"
@@ -132,6 +133,16 @@ struct dsac_engine {
     Event ev_cams;                  // recorded after that copy: the staging is rewritten, and a pass starts, only after it
     int cams_n = 0;
     unsigned long long cams_gen = 0, fwd_cams_gen = 0;   // generation of the setting, and the one the last forward ran with
+    // guided sampling (dsac_set_sampling_logits_device): per-frame tables sized once for max_frames on first use; g_n == 0:
+    // the reference's uniform sampler
+    DevMem<double> d_g_w;            // [max_frames][N] softmax of the logits
+    DevMem<uint32_t> d_g_q, d_g_cum; // [max_frames][N] integer weights and their inclusive prefix sums
+    DevMem<uint32_t> d_g_bad;        // [max_frames] DSAC_ST_BAD_WEIGHTS
+    Event ev_g;                      // recorded after the table kernel: a pass starts only after it
+    int g_n = 0;
+    unsigned long long g_gen = 0, fwd_g_gen = 0;   // generation of the setting, and the one the last forward ran with
+    int fwd_g_n = 0;                 // frames of the last forward if it was guided, else 0
+    uint32_t fwd_seed = 0;
     // per-dataset cameras of the pre-training data paths (dsac_set_dataset_cameras), indexed by dataset frame; grow-only.
     // ds_cams_n == 0: no table.  ds_cam0 is entry 0 on the host: the frame size and raw_data every entry shares.
     DevMem<ObjCam> d_ds_cams;
@@ -191,7 +202,7 @@ struct dsac_engine {
     int k1_rounds = 3, k1_cap = 0;   // rounds 0..2 finish every stream of the benchmark batches; a straggler continues in k_sample (resume). 5 rounds = 6 empty launches per pass
     bool k1_rounds_fixed = false;   // DSAC_K1_ROUNDS given
     int k1_filter_grid = 0, k1_solve_grid = 0;
-    unsigned long long k1_calls = 0;
+    unsigned long long k1_calls[2] = {0, 0};     // passes by sampler: [0] uniform, [1] guided (parity selects the statistics block)
     DevMem<K1SlotState> d_k1_state;
     DevMem<CellRec> d_k1_celltab;
     DevMem<uint2> d_k1_cells;
@@ -201,7 +212,9 @@ struct dsac_engine {
     DevMem<uint2> d_k1_wq;
     DevMem<uint32_t> d_k1_fq;
     DevMem<int> d_k1_counters;                    // wq_n[K1S_MAX_ROUNDS], fq_n[K1S_MAX_ROUNDS]
-    DevMem<unsigned long long> d_k1_stats;        // [2][2]: candidates / hypotheses of finished streams, by call parity
+    DevMem<unsigned long long> d_k1_stats;        // [2][2][2]: candidates / hypotheses of finished streams, by sampler (uniform,
+                                                  // guided) and call parity: the first round of a pass is sized from the last
+                                                  // pass of the same sampler, whose rate can differ from the other's many times over
     DevMem<unsigned long long> d_k1_dbg;          // [K1S_MAX_ROUNDS][4] (DSAC_K1_DEBUG=1 or dsac_sampler_profile), else null
     // dsac_sampler_profile: CUDA events between the sampler's launches of the last forward pass
     int k1_profile = 0;
@@ -221,7 +234,7 @@ struct dsac_engine {
         Event ev_filt[K1S_MAX_SETS], ev_solve[K1S_MAX_SETS], ev_gen[K1S_MAX_SETS], ev_round;
         DevMem<int> counters;
         DevMem<unsigned long long> stats;
-        unsigned long long calls = 0;
+        unsigned long long calls[2] = {0, 0};
     } lane1;
     int k1_lanes = 1;                             // DSAC_K1_LANES: 0 = never split a batch into two lanes
     int k1_overlap = 1;
@@ -519,8 +532,8 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
             }
             CUC(cudaEventCreateWithFlags(L.ev_round.put(), cudaEventDisableTiming));
             CUC(L.counters.reserve(2 * K1S_MAX_SETS * sizeof(int)));
-            CUC(L.stats.reserve(4 * sizeof(unsigned long long)));
-            CUC(cudaMemset(L.stats, 0, 4 * sizeof(unsigned long long)));
+            CUC(L.stats.reserve(8 * sizeof(unsigned long long)));
+            CUC(cudaMemset(L.stats, 0, 8 * sizeof(unsigned long long)));
             if (const char* ln = getenv("DSAC_K1_LANES")) e->k1_lanes = atoi(ln);
         }
         if (const char* ov = getenv("DSAC_K1_OVERLAP")) { e->k1_overlap = atoi(ov); e->k1_overlap_fixed = true; }
@@ -529,8 +542,8 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
         if (const char* s4 = getenv("DSAC_K1_SOLVE4")) e->k1_solve_group4 = atoi(s4);
         if (const char* sb = getenv("DSAC_K1_SOLVE_BATCH")) e->k1_solve_batch = atoi(sb);
         CUC(cudaFuncSetAttribute(k1_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1XSmem)));
-        CUC(e->d_k1_stats.reserve(4 * sizeof(unsigned long long)));
-        CUC(cudaMemset(e->d_k1_stats, 0, 4 * sizeof(unsigned long long)));
+        CUC(e->d_k1_stats.reserve(8 * sizeof(unsigned long long)));
+        CUC(cudaMemset(e->d_k1_stats, 0, 8 * sizeof(unsigned long long)));
         if (getenv("DSAC_K1_DEBUG")) CUC(e->d_k1_dbg.reserve(K1S_MAX_ROUNDS * 4 * sizeof(unsigned long long)));
         CUC(cudaFuncSetAttribute(k1_filter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1FSmem)));
         CUC(cudaFuncSetAttribute(k1_filter_cam, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1FSmem)));
@@ -551,6 +564,7 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
         CUC(cudaEventCreateWithFlags(e->ev_fork.put(), cudaEventDisableTiming));
         CUC(cudaEventCreateWithFlags(e->ev_join.put(), cudaEventDisableTiming));
         CUC(cudaEventCreateWithFlags(e->ev_fwd.put(), cudaEventDisableTiming));
+        CUC(cudaEventCreateWithFlags(e->ev_g.put(), cudaEventDisableTiming));
         if (const char* ts = getenv("DSAC_TAIL_SPLIT")) e->tail_split = atoi(ts);
     }
 #undef CUC
@@ -605,8 +619,86 @@ static int cameras_begin_pass(dsac_engine* e, int32_t n, cudaStream_t stream) {
     if (e->cams_n && n != e->cams_n)
         return fail(e, DSAC_ERR_ARG, "n_frames %d differs from the %d cameras set by dsac_set_cameras", n, e->cams_n);
     if (e->cams_n) CU(cudaStreamWaitEvent(stream, e->ev_cams, 0));
+    if (e->g_n && n != e->g_n)
+        return fail(e, DSAC_ERR_ARG, "n_frames %d differs from the %d frames of the sampling logits (dsac_set_sampling_logits_device)", n, e->g_n);
+    if (e->g_n && !e->k1_mode) return fail(e, DSAC_ERR_ARG, "guided sampling needs the split sampler (DSAC_K1_MODE unset)");
+    if (e->g_n) CU(cudaStreamWaitEvent(stream, e->ev_g, 0));
     e->fwd_cams_gen = e->cams_gen;
+    e->fwd_g_gen = e->g_gen;
+    e->fwd_g_n = e->g_n;
+    e->fwd_seed = e->cfg.seed;
     return DSAC_OK;
+}
+
+int dsac_set_sampling_logits_device(dsac_engine* e, int32_t n, const float* d_logits, void* stream_v) {
+    if (!e) return DSAC_ERR_ARG;
+    if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_set_sampling_logits_device: a submitted pass has not been awaited (dsac_forward_wait)");
+    if (!d_logits) {
+        if (e->g_n) e->g_gen++;
+        e->g_n = 0;
+        return DSAC_OK;
+    }
+    if (n < 1 || n > e->cfg.max_frames)
+        return fail(e, DSAC_ERR_ARG, "dsac_set_sampling_logits_device: n %d out of range [1,%d]", n, e->cfg.max_frames);
+    if (!e->k1_mode) return fail(e, DSAC_ERR_ARG, "guided sampling needs the split sampler (DSAC_K1_MODE unset)");
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    CU(cudaSetDevice(e->cfg.device));
+    const size_t cells = (size_t)e->cfg.max_frames * DSAC_N;
+    CU(e->d_g_w.reserve(cells * sizeof(double)));
+    CU(e->d_g_q.reserve(cells * sizeof(uint32_t)));
+    CU(e->d_g_cum.reserve(cells * sizeof(uint32_t)));
+    CU(e->d_g_bad.reserve((size_t)e->cfg.max_frames * sizeof(uint32_t)));
+    CU(cudaStreamWaitEvent(stream, e->ev_fwd, 0));   // the last forward pass may still read the tables
+    e->g_n = 0;                                       // (a failed launch leaves the uniform sampler in force)
+    e->g_gen++;
+    k_guided_table<<<(unsigned)n, KG_THREADS, 0, stream>>>(d_logits, e->d_g_w, e->d_g_q, e->d_g_cum, e->d_g_bad);
+    e->launches++;
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(e->ev_g, stream));
+    e->g_n = n;
+    return DSAC_OK;
+}
+
+int dsac_sampling_table_device(dsac_engine* e, int32_t n, uint32_t* d_q) {
+    if (!e || !d_q) return DSAC_ERR_ARG;
+    if (!e->g_n) return fail(e, DSAC_ERR_ARG, "dsac_sampling_table_device: no sampling logits are set");
+    if (n != e->g_n) return fail(e, DSAC_ERR_ARG, "dsac_sampling_table_device: n %d differs from the %d frames of the setting", n, e->g_n);
+    CU(cudaSetDevice(e->cfg.device));
+    CU(cudaEventSynchronize(e->ev_g));
+    CU(cudaMemcpy(d_q, e->d_g_q, (size_t)n * DSAC_N * sizeof(uint32_t), cudaMemcpyDeviceToDevice));
+    return DSAC_OK;
+}
+
+// dsac_sampling_log_prob_device / _backward_device: the last pass must have been guided by the setting still in force.
+static int sampling_log_prob_run(dsac_engine* e, const char* who, int32_t n, double* d_logp, const double* d_grad_logp, float* d_grad,
+                                 void* stream_v) {
+    if (!e) return DSAC_ERR_ARG;
+    if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "%s: a submitted pass has not been awaited (dsac_forward_wait)", who);
+    if (!e->fwd_g_n) return fail(e, DSAC_ERR_ARG, "%s: the last forward pass was not guided", who);
+    if (n != e->fwd_g_n) return fail(e, DSAC_ERR_ARG, "%s: n %d differs from the %d frames of the last pass", who, n, e->fwd_g_n);
+    if (e->fwd_g_gen != e->g_gen) return fail(e, DSAC_ERR_ARG, "%s: the sampling logits were changed after the last pass", who);
+    if ((!d_logp && !d_grad_logp) || (d_grad_logp && !d_grad)) return fail(e, DSAC_ERR_ARG, "%s: null output", who);
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    CU(cudaSetDevice(e->cfg.device));
+    CU(cudaStreamWaitEvent(stream, e->ev_fwd, 0));
+    GuidedLogpParams g;
+    g.w = e->d_g_w; g.cum = e->d_g_cum; g.bad = e->d_g_bad; g.stream_ncand = e->d_stream_ncand;
+    g.T = e->cfg.n_streams; g.seed = e->fwd_seed; g.frame0 = e->cur_frame0;
+    g.logp = d_logp; g.grad_logp = d_grad_logp; g.grad_logits = d_grad;
+    k_guided_logp<<<(unsigned)n, KG_THREADS, 0, stream>>>(g);
+    e->launches++;
+    CU(cudaGetLastError());
+    return DSAC_OK;
+}
+
+int dsac_sampling_log_prob_device(dsac_engine* e, int32_t n, double* d_logp, void* stream) {
+    if (!d_logp) return e ? fail(e, DSAC_ERR_ARG, "dsac_sampling_log_prob_device: null output") : DSAC_ERR_ARG;
+    return sampling_log_prob_run(e, "dsac_sampling_log_prob_device", n, d_logp, nullptr, nullptr, stream);
+}
+
+int dsac_sampling_log_prob_backward_device(dsac_engine* e, int32_t n, const double* d_grad_logp, float* d_grad_logits, void* stream) {
+    if (!d_grad_logp || !d_grad_logits) return e ? fail(e, DSAC_ERR_ARG, "dsac_sampling_log_prob_backward_device: null argument") : DSAC_ERR_ARG;
+    return sampling_log_prob_run(e, "dsac_sampling_log_prob_backward_device", n, nullptr, d_grad_logp, d_grad_logits, stream);
 }
 
 // A backward pass differentiates the forward before it, which ran with the cameras in force then.
@@ -714,6 +806,8 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
     const dsac_config& c = e->cfg;
     const size_t o = (size_t)off, Hh = (size_t)c.n_hyps, Nn = DSAC_N;
     const Cam* cams = e->cams_n ? e->d_cams + o : nullptr;   // per-frame cameras: those of this range's frames
+    const bool guided = e->g_n > 0;                           // guided sampling: this range's frames of the tables
+    const GuidedGen gg{guided ? e->d_g_cum + o * DSAC_N : nullptr, guided ? e->d_g_bad + o : nullptr};
 
     if (e->stages & DSAC_STAGE_SAMPLE) {
         CU(cudaMemsetAsync(e->d_status + o, 0, (size_t)n * sizeof(uint32_t), stream));
@@ -743,8 +837,8 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             const Event* k_ev_gen = lane ? e->lane1.ev_gen : e->k1_ev_gen;
             cudaEvent_t k_ev_round = lane ? e->lane1.ev_round : e->k1_ev_round;
             int* k_counters = lane ? e->lane1.counters : e->d_k1_counters;
-            unsigned long long* k_stats = lane ? e->lane1.stats : e->d_k1_stats;
-            unsigned long long& k_calls = lane ? e->lane1.calls : e->k1_calls;
+            unsigned long long* k_stats = (lane ? e->lane1.stats : e->d_k1_stats) + (guided ? 4 : 0);
+            unsigned long long& k_calls = (lane ? e->lane1.calls : e->k1_calls)[guided ? 1 : 0];
             K1SplitParams q;
             q.sp = sp;
             q.state = e->d_k1_state + o * T; q.celltab = e->d_k1_celltab + o * Nn;
@@ -802,12 +896,13 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             if (e->k1_slot_threads > 0) slot_threads = e->k1_slot_threads;
             auto launch_slot = [&](const K1SplitParams& qq) {
                 const dim3 g(c.n_streams, n);
-                if (slot_threads == 1024) k1_slot_t<1024><<<g, 1024, 0, stream>>>(qq);
+                if (guided) k1_gslot<<<g, K1S_THREADS, 0, stream>>>(qq, gg);
+                else if (slot_threads == 1024) k1_slot_t<1024><<<g, 1024, 0, stream>>>(qq);
                 else if (slot_threads == 512) k1_slot_t<512><<<g, 512, 0, stream>>>(qq);
                 else k1_slot<<<g, K1S_THREADS, 0, stream>>>(qq);
             };
             // with the profile on everything runs on one stream so that the event intervals are the kernels' own durations
-            const bool fused = e->k1_fused != 0 && !cams;   // (k1_fused has no per-frame instantiation; the schedule does not change results)
+            const bool fused = e->k1_fused != 0 && !cams && !guided;   // (k1_fused has no per-frame instantiation; the schedule does not change results)
             // streams: generator on `stream`, filter (and solve) on a side stream; with a batch that does not fill the GPU several
             // times over the solve gets a stream of its own, so that the filter of set k+1 need not wait for the solve of set k
             // (DSAC_K1_OVERLAP=1 / 2 compares them; on an H100 SXM at 700 W: 128 frames 0.856 / 0.862 ms, 1024 frames 3.09 / 3.10 ms)
@@ -818,7 +913,8 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             const size_t n_slots_cap = (size_t)e->cfg.max_frames * c.n_streams * (size_t)e->k1_cap;
             mark(-1);
             {
-                const int cell_blocks = (int)(((size_t)n * Nn + 255) / 256), seed_blocks = (int)((n_slots + 31) / 32);
+                // (guided passes read no MT19937 stream: nothing to seed)
+                const int cell_blocks = (int)(((size_t)n * Nn + 255) / 256), seed_blocks = guided ? 0 : (int)((n_slots + 31) / 32);
                 if (cams) k1_cells_cam<<<(unsigned)(cell_blocks + seed_blocks), 256, 0, stream>>>(q, n, seed_blocks);
                 else k1_cells<<<(unsigned)(cell_blocks + seed_blocks), 256, 0, stream>>>(q, n, seed_blocks);
             }
@@ -834,11 +930,11 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             // speculative first round (k1_spec / k1_stitch): one stream generated window by window on many SMs; pays when a
             // stream's first round is several windows long (>= 64 hypotheses per stream) and the GPU is otherwise idle
             const int quota_max = (c.n_hyps + c.n_streams - 1) / c.n_streams;
-            const bool use_spec = few && off == 0 && n_slots <= e->k1_spec_slots && quota_max >= 64 && c.max_candidates >= (1 << 16) && !fused_req;   // (the candidate bound cannot fall inside the speculative round)
+            const bool use_spec = few && off == 0 && n_slots <= e->k1_spec_slots && quota_max >= 64 && c.max_candidates >= (1 << 16) && !fused_req && !guided;   // (the candidate bound cannot fall inside the speculative round)
             // chained generator (k1_pipe): K CTAs per stream, all of them resident at once
             const int pipe_K = (int)std::min<long long>(8, e->k1_slot_capacity / std::max<long long>(1, n_slots));
             const bool use_pipe = e->k1_pipe && !use_spec && pipe_K >= 3 && n_slots >= 9 && quota_max >= 64 && c.max_candidates >= (1 << 16) &&
-                                  !fused_req && !e->k1_profile;
+                                  !fused_req && !e->k1_profile && !guided;
             const int n_rounds = (few && !e->k1_rounds_fixed) ? std::min(e->k1_rounds, 2) : e->k1_rounds;
             for (int r = 0; r < n_rounds; r++) {
                 // portions only pay when the generator has the whole GPU to fill (many streams); a few streams (single-frame
@@ -931,7 +1027,9 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             launch_slot(q);
             mark(0);
             sp.resume = q.state;   // streams the rounds left unfinished (normally none) continue in the monolithic kernel
-            if (cams) k_sample_cam<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
+            if (guided && cams) k1_gtail_cam<<<dim3(c.n_streams, n), KG_THREADS, 0, stream>>>(q, gg);   // ... or in guided steps
+            else if (guided) k1_gtail<<<dim3(c.n_streams, n), KG_THREADS, 0, stream>>>(q, gg);
+            else if (cams) k_sample_cam<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
             else k_sample<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
             mark(3);
             e->launches += 2;

@@ -22,9 +22,47 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include "guided_rng.cuh"
 #include "kernels.cuh"
 
 namespace dsac {
+
+// Guided sampling (guided.cuh): the candidate source of k1_gslot and k1_gtail in place of MT19937.
+struct GuidedGen {
+    const uint32_t* cum;   // [n][N] inclusive prefix sums of the integer weights
+    const uint32_t* bad;   // [n] 1: DSAC_ST_BAD_WEIGHTS, nothing is sampled
+};
+
+// One accepted hypothesis to the pass's outputs (k1_slot's selection, k1_gtail's accepts).  getDiffMap -> cv::projectPoints
+// rebuilds R from rvec, so hyp_P does too.
+__device__ __forceinline__ void k1_write_hyp(const SampleParams& p, size_t hi, const double rvec[3], const double tvec[3], const int cells[4],
+                                             long long cand) {
+    double* hp = p.hyp_pose + hi * 6;
+    hp[0] = rvec[0]; hp[1] = rvec[1]; hp[2] = rvec[2];
+    hp[3] = tvec[0]; hp[4] = tvec[1]; hp[5] = tvec[2];
+    double Rm[9];
+    rodrigues_v2m(rvec, Rm);
+    float4* P = reinterpret_cast<float4*>(p.hyp_P + hi * 12);
+    P[0] = make_float4((float)(p.f * Rm[0]), (float)(p.f * Rm[1]), (float)(p.f * Rm[2]), (float)(p.f * tvec[0]));
+    P[1] = make_float4((float)(p.f * Rm[3]), (float)(p.f * Rm[4]), (float)(p.f * Rm[5]), (float)(p.f * tvec[1]));
+    P[2] = make_float4((float)Rm[6], (float)Rm[7], (float)Rm[8], (float)tvec[2]);
+    *reinterpret_cast<int4*>(p.img_idx + hi * 4) = make_int4(cells[0], cells[1], cells[2], cells[3]);
+    p.cand_idx[hi] = (int32_t)cand;
+}
+
+// Hypotheses [h, h + count) of `frame` as an exhausted stream leaves them (zero pose, k_sample's value encoding).
+__device__ __forceinline__ void k1_empty_hyps(const SampleParams& p, int frame, int h, int count, int tid, int nt) {
+    for (int r = tid; r < count; r += nt) {
+        const size_t hi = (size_t)frame * p.H + h + r;
+        for (int k = 0; k < 6; k++) p.hyp_pose[hi * 6 + k] = 0.0;
+        float4* P = reinterpret_cast<float4*>(p.hyp_P + hi * 12);
+        P[0] = make_float4((float)p.f, 0.f, 0.f, 0.f);
+        P[1] = make_float4(0.f, (float)p.f, 0.f, 0.f);
+        P[2] = make_float4(0.f, 0.f, 1.f, 0.f);
+        for (int k = 0; k < 4; k++) p.img_idx[hi * 4 + k] = -1;
+        p.cand_idx[hi] = -1;
+    }
+}
 
 #define K1S_THREADS_DEF 256
 constexpr int K1S_THREADS = K1S_THREADS_DEF;     // k1_slot
@@ -193,9 +231,12 @@ __device__ __forceinline__ int k1_round_size(int quota, int acc, long long cand_
 // (0: the whole CTA of the k1_slot kernel; >= 1: the generator warps inside k1_fused).  tid: index within the group.
 // TW3: regeneration through mt_twist3 (own words in registers, branch-free: fastest for a lone CTA, but ten
 // instructions more per thread, which the issue-bound full batch pays for)
-template <int BAR_ID, int BAR_N, int NT, bool TW3 = (NT > 256)>
+// GUIDED (k1_gslot): the candidates come from guided_draw with the frame's table gg instead of MT19937, one per thread;
+// selection, round sizing and hand-over are the same code.  A guided candidate's stream position (endw) is the stream's
+// starting word: the pass consumes nothing of the MT19937 streams.
+template <int BAR_ID, int BAR_N, int NT, bool TW3 = (NT > 256), bool GUIDED = false>
 __device__ __forceinline__ void k1_slot_body(const K1SplitParams& q, K1GSmemT<NT / 32>& sm, const int tid, const int s, const int frame,
-                                             const int slot_ov = -1) {
+                                             const int slot_ov = -1, const GuidedGen gg = GuidedGen{}) {
     constexpr int NW = NT / 32, SEL_WORDS = K1S_MAX_CAP / 32 / NT;   // warps of the group; accept-bit words per thread in the selection
     static_assert(SEL_WORDS >= 1 && K1S_LEFT_CAP % NT == 0, "k1_slot_body: thread count");
     const SampleParams& p = q.sp;
@@ -220,7 +261,7 @@ __device__ __forceinline__ void k1_slot_body(const K1SplitParams& q, K1GSmemT<NT
         cand_base = S.cand_base;
         pos = S.pos;
         gen = S.gen;
-        {
+        if constexpr (!GUIDED) {
             uint32_t* half = sm.st + ((gen / MT_N) & 1u) * MT_N;
             for (int k = tid; k < MT_N; k += NT) half[k] = S.mt[k];
             const int ln = S.left_n;
@@ -237,8 +278,21 @@ __device__ __forceinline__ void k1_slot_body(const K1SplitParams& q, K1GSmemT<NT
             }
             return;
         }
-        // stream s of global frame g: mt19937(seed + g*T + s)   (thread_rand.cpp:52 for g = 0)
-        for (int k = tid; k < MT_N; k += NT) sm.st[k] = S.mt[k];   // seeded by k1_cells
+        if constexpr (GUIDED) {
+            if (gg.bad[frame]) {   // DSAC_ST_BAD_WEIGHTS: nothing is sampled, the hypotheses of an exhausted stream
+                k1_empty_hyps(p, frame, h0, quota, tid, NT);
+                if (tid == 0) {
+                    S.done = 1; S.acc = 0; S.n_round = 0; S.target = 0; S.cand_base = 0; S.left_n = 0; S.any_reject = 0; S.overflow = 0; S.pos = 0; S.gen = 0;
+                    p.stream_ncand[slot] = 0;
+                    p.stream_endpos[slot] = (s == 0) ? p.skip : 0u;
+                    atomicOr(p.status + frame, 32u /* DSAC_ST_BAD_WEIGHTS */);
+                }
+                return;
+            }
+        } else {
+            // stream s of global frame g: mt19937(seed + g*T + s)   (thread_rand.cpp:52 for g = 0)
+            for (int k = tid; k < MT_N; k += NT) sm.st[k] = S.mt[k];   // seeded by k1_cells
+        }
         pos = (s == 0) ? p.skip : 0u;
         gen = 0;
         acc = 0;
@@ -281,20 +335,10 @@ __device__ __forceinline__ void k1_slot_body(const K1SplitParams& q, K1GSmemT<NT
             const int i = sm.acc_list[k];
             const size_t hi = (size_t)frame * p.H + h0 + acc + k;
             const double* po = q.pose_out + (cbase + i) * 6;
-            double rvec[3] = {po[0], po[1], po[2]}, tvec[3] = {po[3], po[4], po[5]};
-            double* hp = p.hyp_pose + hi * 6;
-            hp[0] = rvec[0]; hp[1] = rvec[1]; hp[2] = rvec[2];
-            hp[3] = tvec[0]; hp[4] = tvec[1]; hp[5] = tvec[2];
-            double Rm[9];
-            rodrigues_v2m(rvec, Rm);  // getDiffMap -> cv::projectPoints rebuilds R from rvec
-            float4* P = reinterpret_cast<float4*>(p.hyp_P + hi * 12);
-            P[0] = make_float4((float)(p.f * Rm[0]), (float)(p.f * Rm[1]), (float)(p.f * Rm[2]), (float)(p.f * tvec[0]));
-            P[1] = make_float4((float)(p.f * Rm[3]), (float)(p.f * Rm[4]), (float)(p.f * Rm[5]), (float)(p.f * tvec[1]));
-            P[2] = make_float4((float)Rm[6], (float)Rm[7], (float)Rm[8], (float)tvec[2]);
+            const double rvec[3] = {po[0], po[1], po[2]}, tvec[3] = {po[3], po[4], po[5]};
             const uint2 cc = q.cells[cbase + i];
-            *reinterpret_cast<int4*>(p.img_idx + hi * 4) =
-                make_int4((int)(cc.x & 0xffffu), (int)(cc.x >> 16), (int)(cc.y & 0xffffu), (int)(cc.y >> 16));
-            p.cand_idx[hi] = (int32_t)(cand_base + i);
+            const int cells[4] = {(int)(cc.x & 0xffffu), (int)(cc.x >> 16), (int)(cc.y & 0xffffu), (int)(cc.y >> 16)};
+            k1_write_hyp(p, hi, rvec, tvec, cells, cand_base + i);
             if (acc + k == quota - 1) {
                 p.stream_ncand[slot] = cand_base + i + 1;
                 p.stream_endpos[slot] = (unsigned long long)q.endw[cbase + i];
@@ -318,7 +362,7 @@ __device__ __forceinline__ void k1_slot_body(const K1SplitParams& q, K1GSmemT<NT
         // ---------------- restore the generator
         pos = S.pos;
         gen = S.gen;
-        {
+        if constexpr (!GUIDED) {
             uint32_t* half = sm.st + ((gen / MT_N) & 1u) * MT_N;
             for (int k = tid; k < MT_N; k += NT) half[k] = S.mt[k];
             const int ln = S.left_n;
@@ -346,12 +390,29 @@ __device__ __forceinline__ void k1_slot_body(const K1SplitParams& q, K1GSmemT<NT
     }
     const int n_round = min(q.portion, round_total - already);   // candidates this launch generates
 
+    int produced = 0;
+    if constexpr (GUIDED) {
+        // ---------------- guided generation: candidate cand_base + already + i by thread i mod NT, the frame's prefix sums
+        // in shared memory (vals holds stream words only in the MT19937 generator)
+        uint32_t* cum = reinterpret_cast<uint32_t*>(sm.vals);
+        static_assert(sizeof(sm.vals) >= DSAC_N_CONST * sizeof(uint32_t), "k1_slot_body: guided table");
+        for (int k = tid; k < DSAC_N_CONST; k += NT) cum[k] = gg.cum[(size_t)frame * DSAC_N_CONST + k];
+        group_barrier<BAR_ID, BAR_N>();
+        const unsigned long long z = (unsigned long long)((p.frame0 + frame) * (long long)p.T + s);
+        const uint32_t pos0 = (s == 0) ? p.skip : 0u;
+        for (int i = tid; i < n_round; i += NT) {
+            int cells[4];
+            guided_draw(cum, p.seed, z, (uint32_t)(cand_base + already + i), cells);
+            q.cells[cbase + already + i] = make_uint2((uint32_t)cells[0] | ((uint32_t)cells[1] << 16), (uint32_t)cells[2] | ((uint32_t)cells[3] << 16));
+            q.endw[cbase + already + i] = pos0;
+        }
+        produced = n_round;
+    } else {
     // ---------------- generation: windows of up to K1S_SR candidates (phases A1, A2 and E of k_sample)
     // development aid (DSAC_K1_TIMERS=1): thread-0 cycles per phase of the generator -> phase_cycles[8..13]
     const bool timed = p.phase_cycles != nullptr && tid == 0;
     long long t_mark = timed ? clock64() : 0, t_ph[6] = {0, 0, 0, 0, 0, 0};
 #define K1S_PHASE(k) do { if (timed) { const long long t_now = clock64(); t_ph[k] += t_now - t_mark; t_mark = t_now; } } while (0)
-    int produced = 0;
     uint32_t st_par = (gen / MT_N) & 1u;   // which half of sm.st holds the current state
     while (produced < n_round) {
         const int n_target = min(K1S_SR, n_round - produced);
@@ -600,13 +661,16 @@ __device__ __forceinline__ void k1_slot_body(const K1SplitParams& q, K1GSmemT<NT
     if (timed)
         for (int k = 0; k < 6; k++) atomicAdd(p.phase_cycles + 8 + k, (unsigned long long)t_ph[k]);
 #undef K1S_PHASE
+    }
 
     // ---------------- hand the portion over: state, work items, cleared accept bits
     {
-        const int left = min((int)(gen - pos), K1S_LEFT_CAP);
-        const uint32_t* half = sm.st + ((gen / MT_N) & 1u) * MT_N;
-        for (int k = tid; k < MT_N; k += NT) S.mt[k] = half[k];
-        for (int k = tid; k < left; k += NT) S.left[k] = sm.vals[k];
+        const int left = GUIDED ? 0 : min((int)(gen - pos), K1S_LEFT_CAP);
+        if constexpr (!GUIDED) {
+            const uint32_t* half = sm.st + ((gen / MT_N) & 1u) * MT_N;
+            for (int k = tid; k < MT_N; k += NT) S.mt[k] = half[k];
+            for (int k = tid; k < left; k += NT) S.left[k] = sm.vals[k];
+        }
         if (!q.spec) {
             uint32_t* ab = q.accbits + (size_t)slot * (q.cap >> 5) + (already >> 5);   // `already` is a multiple of the chunk size
             for (int k = tid; k < ((produced + 31) >> 5); k += NT) ab[k] = 0u;
@@ -614,7 +678,7 @@ __device__ __forceinline__ void k1_slot_body(const K1SplitParams& q, K1GSmemT<NT
         if (tid == 0) {
             S.pos = pos; S.gen = gen; S.acc = acc; S.cand_base = cand_base; S.n_round = already + produced; S.done = 0;
             if (!q.gen_only) S.target = round_total;
-            S.left_n = left; S.any_reject = sm.any_reject;
+            S.left_n = left; S.any_reject = GUIDED ? 0 : sm.any_reject;
             if (q.round == 0 && !q.gen_only) S.overflow = 0;
             const int n_items = q.spec ? 0 : (produced + q.chunk - 1) / q.chunk;
             if (n_items > 0) {
@@ -646,6 +710,11 @@ __global__ void __launch_bounds__(NT, (NT == K1S_THREADS) ? K1S_MIN_BLOCKS : 102
 __global__ void __launch_bounds__(K1S_THREADS, K1S_MIN_BLOCKS) k1_slot(K1SplitParams q) {
     __shared__ K1GSmem sm;
     k1_slot_body<0, 0, K1S_THREADS>(q, sm, threadIdx.x, blockIdx.x, blockIdx.y);
+}
+// the same with guided candidates (guided.cuh)
+__global__ void __launch_bounds__(K1S_THREADS, K1S_MIN_BLOCKS) k1_gslot(K1SplitParams q, GuidedGen gg) {
+    __shared__ K1GSmem sm;
+    k1_slot_body<0, 0, K1S_THREADS, false, true>(q, sm, threadIdx.x, blockIdx.x, blockIdx.y, -1, gg);
 }
 
 // ------------------------------------------------------------------ k1_spec / k1_stitch: one stream generated by many CTAs

@@ -15,6 +15,7 @@ GRID = 40
 N = GRID * GRID
 STAGE_SAMPLE, STAGE_SCORE, STAGE_REFINE, STAGE_EVAL, STAGE_ALL = 1, 2, 4, 8, 15
 ST_SAMPLER_EXHAUSTED, ST_REFINE_ABORTED = 1, 2
+ST_BAD_WEIGHTS = 32          # DSAC_ST_BAD_WEIGHTS
 
 # every symbol include/dsac_b200.h declares
 EXPORTS = [
@@ -28,6 +29,8 @@ EXPORTS = [
     "dsac_default_rgbd_camera", "dsac_set_dataset_cameras", "dsac_register_depth_device", "dsac_obj_coords_device", "dsac_obj_rng_init_device",
     "dsac_obj_draw_device", "dsac_gather_patches_at_device", "dsac_shuffle_permutation",
     "dsac_score_draw_device", "dsac_score_maps_device", "dsac_shuffle_permutations",
+    "dsac_set_sampling_logits_device", "dsac_sampling_table_device", "dsac_sampling_log_prob_device",
+    "dsac_sampling_log_prob_backward_device",
 ]
 
 ST_OBJ_DRAW_EXHAUSTED = 8    # DSAC_ST_OBJ_DRAW_EXHAUSTED
@@ -170,6 +173,10 @@ def load(build_if_missing=True):
     lib.dsac_debug_spec_result.argtypes = [C.c_void_p, C.c_void_p]
     lib.dsac_set_cameras.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.dsac_set_stages.argtypes = [C.c_void_p, C.c_uint32]
+    lib.dsac_set_sampling_logits_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.dsac_sampling_table_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
+    lib.dsac_sampling_log_prob_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.dsac_sampling_log_prob_backward_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.dsac_set_tail_split.argtypes = [C.c_void_p, C.c_int32]
     lib.dsac_set_score_hook.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     lib.dsac_set_score_backward_hook.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
@@ -390,6 +397,25 @@ class Engine:
         if cams.ndim != 2 or cams.shape[1] != 3:
             raise ValueError("cameras must be float64 [n][3] (focal, cx, cy), got %s" % (cams.shape,))
         self._check(self.lib.dsac_set_cameras(self.h, cams.shape[0], _p(cams), C.c_void_p(stream) if stream else None))
+
+    def set_sampling_logits_device(self, n, d_logits, stream=None):
+        """dsac_set_sampling_logits_device: float32 [n][1600] logits on the device (raw pointer as int) guide the sampler of
+        the following passes, which must then have n frames; d_logits None: back to the reference's uniform sampler."""
+        self._check(self.lib.dsac_set_sampling_logits_device(self.h, n if d_logits else 0, C.c_void_p(d_logits) if d_logits else None,
+                                                             C.c_void_p(stream) if stream else None))
+
+    def sampling_table_device(self, n, d_q):
+        """dsac_sampling_table_device: the integer weights [n][1600] (uint32) the sampler draws from."""
+        self._check(self.lib.dsac_sampling_table_device(self.h, n, C.c_void_p(d_q)))
+
+    def sampling_log_prob_device(self, n, d_logp, stream=None):
+        """dsac_sampling_log_prob_device: float64 [n] log-probability of the last (guided) pass's draw."""
+        self._check(self.lib.dsac_sampling_log_prob_device(self.h, n, C.c_void_p(d_logp), C.c_void_p(stream) if stream else None))
+
+    def sampling_log_prob_backward_device(self, n, d_grad_logp, d_grad_logits, stream=None):
+        """dsac_sampling_log_prob_backward_device: float32 [n][1600] = d_grad_logp[f] * d log p_f / d logits_f."""
+        self._check(self.lib.dsac_sampling_log_prob_backward_device(self.h, n, C.c_void_p(d_grad_logp), C.c_void_p(d_grad_logits),
+                                                                    C.c_void_p(stream) if stream else None))
 
     def set_tail_split(self, mode):
         """0: off, 1: forward_device + blocking forward (default), 2: submitted passes too (scheduling only)."""

@@ -47,6 +47,7 @@ extern "C" {
 #define DSAC_ST_REFINE_ABORTED 2u         /* refinement stopped early (<50 inliers / NaN), cnn_softam.h:1136,1147 */
 #define DSAC_ST_OBJ_DRAW_EXHAUSTED 8u     /* dsac_obj_draw_device: a patch found no valid centre within max_attempts */
 #define DSAC_ST_DEPTH_DROPPED 16u         /* dsac_register_depth_device: registration targets outside the image were dropped */
+#define DSAC_ST_BAD_WEIGHTS 32u           /* guided sampling: a NaN or +inf logit, or fewer than 4 cells with weight > 0; nothing sampled */
 
 typedef struct dsac_engine dsac_engine;
 
@@ -166,6 +167,31 @@ typedef struct dsac_camera { double focal, cx, cy; } dsac_camera;   /* getCamMat
  * a pass index, and their per-frame cameras come from dsac_set_dataset_cameras.  No distortion and no separate fx / fy:
  * the reference has neither. */
 int dsac_set_cameras(dsac_engine* e, int32_t n, const dsac_camera* cams, void* stream);
+
+/* Guided sampling (Neural-Guided RANSAC, Brachmann & Rother, ICCV 2019): the minimal sets of the following passes are drawn
+ * from learned per-cell weights instead of uniformly.  d_logits: DEVICE float32 [n][1600], cell y*40+x, read on `stream`
+ * into engine-owned tables (sized once for max_frames); the buffer may be reused once `stream` has passed this call.  Per frame w = softmax(logits) in fp64 and the sampler draws from the integer
+ * weights q_j = floor(w_j 2^31): each point of a candidate is cell j with probability q_j / (Q - sum of the q already in the
+ * candidate), Q = sum q; the random numbers are Philox4x32-10, key (seed, 0), counter (block, candidate index, lo32(z),
+ * hi32(z)) for slot z = global frame * n_streams + stream (INTEGRATION.md, "Guided sampling").  -inf logits are allowed
+ * (q = 0); a NaN or +inf logit, or fewer than 4 cells with q > 0, gives the frame DSAC_ST_BAD_WEIGHTS and no hypotheses
+ * (zero poses, img_idx -1).  Acceptance, quotas and every later stage are the uniform path's; the DSAC variant's random
+ * draw reads MT19937 stream 0 of the frame right after stream_skip.  Sticky like dsac_set_cameras: later passes must have
+ * n frames; d_logits == NULL (n ignored) returns to the reference sampler.  The redraw of a repeated cell is unbounded as
+ * in the reference: weights with nearly all mass on <= 3 cells and tiny nonzero weights elsewhere make a frame run for a
+ * long time (INTEGRATION.md).  DSAC_ERR_ARG, with the engine left as it was:
+ * n outside [1, max_frames], or a submitted pass that has not been awaited. */
+int dsac_set_sampling_logits_device(dsac_engine* e, int32_t n, const float* d_logits, void* stream);
+/* The integer weights q [n][1600] of the setting in force (DEVICE uint32), the distribution the sampler draws from.
+ * Waits for the setting's table; n must equal its frame count. */
+int dsac_sampling_table_device(dsac_engine* e, int32_t n, uint32_t* d_q);
+/* Log-probability of the last pass's draw, d_logp DEVICE float64 [n]: per frame the sum over the used candidates (stream s:
+ * candidates 0 .. the one of its last accepted hypothesis, or all it drew if it ran out; accepted and rejected alike) of
+ * sum_k [log w_{c_k} - log(1 - sum_{i<k} w_{c_i})].  _backward_device: d_grad_logits [n][1600] float32 = d_grad_logp[f] *
+ * d log p_f / d logits_f, deterministic.  Both recompute the candidates from their counters.  DSAC_ERR_ARG if the last
+ * pass was not guided, n differs from its frame count, the logits were set again since, or a submitted pass is pending. */
+int dsac_sampling_log_prob_device(dsac_engine* e, int32_t n, double* d_logp, void* stream);
+int dsac_sampling_log_prob_backward_device(dsac_engine* e, int32_t n, const double* d_grad_logp, float* d_grad_logits, void* stream);
 
 /* Stage control for measurement: which stages dsac_forward_device runs. */
 #define DSAC_STAGE_SAMPLE 1u
