@@ -33,6 +33,11 @@ the logits, for a REINFORCE-style gradient:
     logp = sampling_log_prob(engine, logits)
     (loss + (loss.detach() - baseline) * logp).sum().backward()
 
+`cell_depth` (float32 [n][1600] on the engine's device, depth in mm at each cell's grid pixel; cell_depth() gathers it
+from registered depth maps) makes the pass an RGB-D pass (INTEGRATION.md, "RGB-D localisation"): hypotheses and
+refinement are Kabsch fits of scene to eye coordinates.  Like sampling_logits, the engine reads a detached copy applied on
+the current stream, and None leaves the setting alone.  The gradient goes to `prediction` only: depth is not differentiated.
+
 Everything stays on the device, on torch.cuda.current_stream().  The engine holds one pass: a forward on the same engine
 between a loss and its backward() makes that backward() raise.
 """
@@ -78,6 +83,37 @@ def _set_sampling(engine, prediction, logits):
     copy.record_stream(stream)
     # the pass that follows is sampled with this tensor as it is now (sampling_log_prob checks identity and version)
     engine._sampling_key = (id(logits), logits._version, engine.passes + 1)
+
+
+def _set_depth(engine, prediction, depth):
+    if depth is None:
+        return
+    n = prediction.shape[0]
+    if depth.dtype != torch.float32 or tuple(depth.shape) != (n, _E.N) or depth.device != prediction.device:
+        raise ValueError("cell_depth must be float32 [%d][%d] on %s, got %s %s on %s"
+                         % (n, _E.N, prediction.device, depth.dtype, tuple(depth.shape), depth.device))
+    copy = depth.detach().contiguous()
+    stream = torch.cuda.current_stream(prediction.device)
+    engine.set_cell_depth_device(n, copy.data_ptr(), stream.cuda_stream)
+    copy.record_stream(stream)
+
+
+def cell_depth(depth, pix):
+    """Per-cell depth float32 [n][1600] (mm) for cell_depth=: the registered uint16 depth maps `depth` [n][H][W] (mm, on
+    the RGB camera, e.g. dsac_register_depth_device's output) at the cells' grid pixels `pix` (int32 [1600][2] shared or
+    [n][1600][2], (x, y)).  0 and 65535 (7-Scenes' invalid value, DESIGN.md Q13) are missing depth (NaN), as are pixels
+    outside the map."""
+    if depth.dim() != 3 or depth.dtype.is_floating_point or depth.dtype == torch.bool:
+        raise ValueError("depth must be uint16 [n][H][W], got %s %s" % (depth.dtype, tuple(depth.shape)))
+    n, Hh, W = depth.shape
+    p = pix.reshape(-1, _E.N, 2).to(torch.int64).expand(n, _E.N, 2)
+    x, y = p[..., 0], p[..., 1]
+    inside = (x >= 0) & (x < W) & (y >= 0) & (y < Hh)
+    flat = depth.reshape(n, -1).to(torch.int64) & 0xffff   # (int16 storage holds the uint16 values too)
+    d = torch.gather(flat, 1, (y.clamp(0, Hh - 1) * W + x.clamp(0, W - 1)))
+    out = d.to(torch.float32)
+    bad = ~inside | (d == 0) | (d == 65535)
+    return torch.where(bad, torch.full_like(out, float("nan")), out)
 
 
 def _coords(engine, prediction, stream):
@@ -187,37 +223,42 @@ class _DsacHypotheses(torch.autograd.Function):
         return grad, None, None, None, None, None
 
 
-def softam_loss(engine, prediction, pix, gt_jp, frame0=0, clamp=0.1, cameras=None, sampling_logits=None):
+def softam_loss(engine, prediction, pix, gt_jp, frame0=0, clamp=0.1, cameras=None, sampling_logits=None, cell_depth=None):
     """Per-frame loss of the soft-argmax pipeline (train_ransac_softam.cpp) on `prediction`, float64 [n]; differentiable
     with respect to `prediction`.  frame0: global index of the first frame (keys the sampler streams)."""
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
+    _set_depth(engine, prediction, cell_depth)
     return _SoftamLoss.apply(prediction, engine, pix, gt_jp, int(frame0), float(clamp))
 
 
 def dsac_expected_loss(engine, prediction, pix, gt_jp, frame0=0, random_draw=True, clamp=0.1, cameras=None,
-                       sampling_logits=None):
+                       sampling_logits=None, cell_depth=None):
     """Per-frame expected loss of the DSAC / RANSAC variant (train_ransac.cpp) on `prediction`, float64 [n];
     differentiable with respect to `prediction`."""
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
+    _set_depth(engine, prediction, cell_depth)
     return _DsacExpectedLoss.apply(prediction, engine, pix, gt_jp, int(frame0), bool(random_draw), float(clamp))
 
 
-def softam_pose(engine, prediction, pix, frame0=0, clamp=0.1, cameras=None, sampling_logits=None):
+def softam_pose(engine, prediction, pix, frame0=0, clamp=0.1, cameras=None, sampling_logits=None, cell_depth=None):
     """Refined pose of every frame of the soft-argmax pipeline as a jp 6-vector [rodrigues(R); t in mm], float64 [n][6];
     differentiable with respect to `prediction`.  Needs no ground truth."""
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
+    _set_depth(engine, prediction, cell_depth)
     return _SoftamPose.apply(prediction, engine, pix, int(frame0), float(clamp))
 
 
-def dsac_hypotheses(engine, prediction, pix, frame0=0, random_draw=True, clamp=0.1, cameras=None, sampling_logits=None):
+def dsac_hypotheses(engine, prediction, pix, frame0=0, random_draw=True, clamp=0.1, cameras=None, sampling_logits=None,
+                    cell_depth=None):
     """(sf [n][H], refined jp 6-vectors [n][H][6]) of the DSAC / RANSAC variant, both float64 and differentiable with
     respect to `prediction`.  The gradient through the poses covers the hypotheses with sf > 1e-4 whose incoming
     gradient is nonzero; an output that receives no gradient costs nothing in the backward."""
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
+    _set_depth(engine, prediction, cell_depth)
     return _DsacHypotheses.apply(prediction, engine, pix, int(frame0), bool(random_draw), float(clamp))
 
 

@@ -15,6 +15,7 @@
 
 #include "pose_math.cuh"
 #include "refine.cuh"
+#include "rigid.cuh"
 
 struct dsac_engine;
 struct dsac_backward_out;
@@ -200,6 +201,28 @@ __global__ void k_dsac_job_p3p(DsacBwParams p) {
     } else {
         for (int k = 0; k < 6; k++) pose[k] = 0;   // safeSolvePnP leaves a zero pose (cnn.h:66-71)
     }
+    for (int k = 0; k < 6; k++) p.job_init[(size_t)j * 6 + k] = pose[k];
+}
+
+// The same for an RGB-D pass: the initial pose of a job that perturbs a minimal-set point is the Kabsch fit of the
+// perturbed points 0..2 to their eye points (eye [n][N][3]).  Depth is not perturbed: the gradient is the scene's.
+__global__ void k_dsac_job_kabsch(DsacBwParams p, const double* __restrict__ eye) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= p.n_jobs) return;
+    const int hyp = p.job_p3p[j * 3];
+    if (hyp < 0) return;
+    const int frame = p.job_frame[j];
+    const int16_t* coords = p.coords + (size_t)frame * DSAC_N_CONST * 3;
+    const double* ey = eye + (size_t)frame * DSAC_N_CONST * 3;
+    const int32_t* idx = p.img_idx + (size_t)hyp * 4;
+    double a[9], b[9];
+    for (int q = 0; q < 3; q++)
+        for (int k = 0; k < 3; k++) { a[q * 3 + k] = (double)coords[idx[q] * 3 + k]; b[q * 3 + k] = ey[idx[q] * 3 + k]; }
+    const int pc = p.job_p3p[j * 3 + 1];
+    if (pc < 9) a[pc] += (double)p.job_p3p[j * 3 + 2];
+    double R[9], pose[6];
+    kabsch_fit(3, a, b, R, pose + 3);
+    rodrigues_m2v(R, pose);
     for (int k = 0; k < 6; k++) p.job_init[(size_t)j * 6 + k] = pose[k];
 }
 
@@ -478,6 +501,71 @@ __global__ void __launch_bounds__(192) k_dpnp(BwParams p) {
     }
 }
 
+// ---- dPNP of an RGB-D pass: the same central differences (eps 0.1 on the float coordinates, the reference's serial
+// perturb / restore) of the 3-point Kabsch hypothesis, scene to eye (eye [n][N][3]); the columns of the 4th point are
+// zero, since the fit does not use it.  Also the jp pose + Rodrigues Jacobian of every hypothesis for k_dscore.
+__global__ void __launch_bounds__(192) k_dkabsch(BwParams p, const double* __restrict__ eye) {
+    const int frame = blockIdx.y;
+    const int h = blockIdx.x * 16 + threadIdx.x / 12, col = threadIdx.x % 12;
+    __shared__ int s_nan[16];
+    if (threadIdx.x < 16) s_nan[threadIdx.x] = 0;
+    __syncthreads();
+    const bool active = h < p.H;
+    double colv[6] = {0, 0, 0, 0, 0, 0};
+    if (active && col < 9) {
+        const int16_t* coords = p.coords + (size_t)frame * DSAC_N_CONST * 3;
+        const double* ey = eye + (size_t)frame * DSAC_N_CONST * 3;
+        const int32_t* idx = p.img_idx + ((size_t)frame * p.H + h) * 4;
+        float obj[9];
+        double b[9];
+        bool valid = true;
+        for (int j = 0; j < 3; j++) {
+            int c = idx[j];
+            if (c < 0) { valid = false; c = 0; }
+            for (int k = 0; k < 3; k++) { obj[j * 3 + k] = (float)coords[c * 3 + k]; b[j * 3 + k] = ey[c * 3 + k]; }
+        }
+        const float eps = 0.1f;
+        for (int q = 0; q < col; q++) {
+            obj[q] += eps;
+            obj[q] -= 2 * eps;
+            obj[q] += eps;
+        }
+        double fS[6], bS[6];
+        for (int side = 0; side < 2; side++) {
+            obj[col] += side ? -2 * eps : eps;
+            double a[9], R[9], pose[6] = {0, 0, 0, 0, 0, 0};
+            for (int k = 0; k < 9; k++) a[k] = (double)obj[k];
+            if (valid) {
+                kabsch_fit(3, a, b, R, pose + 3);
+                rodrigues_m2v(R, pose);
+            }
+            jp6_from_cv_dev(pose, side ? bS : fS);
+        }
+        bool nan = false;
+        for (int k = 0; k < 6; k++) {
+            colv[k] = (fS[k] - bS[k]) / (2 * eps);
+            if (colv[k] != colv[k]) nan = true;
+        }
+        if (nan) s_nan[threadIdx.x / 12] = 1;
+    }
+    __syncthreads();
+    if (active) {
+        const bool zero = s_nan[threadIdx.x / 12] != 0;
+        double* out = p.s.dpnp + ((size_t)frame * p.H + h) * 72;
+        for (int k = 0; k < 6; k++) out[k * 12 + col] = zero ? 0.0 : colv[k];
+        if (col == 0) {
+            double* hj = p.s.hypjp + ((size_t)frame * p.H + h) * 39;
+            double R[9], t[3], rod[3], Rt[9], J[27];
+            cv2our_dev(p.hyp_pose + ((size_t)frame * p.H + h) * 6, R, t);
+            rodrigues_m2v(R, rod);
+            rodrigues_jac(rod, Rt, J);
+            for (int k = 0; k < 9; k++) hj[k] = R[k];
+            for (int k = 0; k < 3; k++) hj[9 + k] = t[k];
+            for (int k = 0; k < 27; k++) hj[12 + k] = J[k];
+        }
+    }
+}
+
 // ---- per frame (one warp): row += dLdAvg . sum_h sf_h dPNP_h scattered to the support points
 //      (train_ransac_softam.cpp:340-353); hypotheses in order, so the sums are reproducible
 __global__ void k_bw_scatter_pnp(BwParams p, int n) {
@@ -658,97 +746,14 @@ __global__ void __launch_bounds__(K5_THREADS) k_dscore(BwParams p) {
     }
 }
 
-// ---- batched Kabsch (Hypothesis::calcRigidBodyTransform, Hypothesis.cpp:145-200): thread = problem.
-// b ~ R a + t with R = V diag(1,1,sign) U^T from the SVD of sum (a-ca)(b-cb)^T.
-__device__ void sym_eig3(const double S[9], double w[3], double V[9]) {
-    double A[9];
-    for (int i = 0; i < 9; i++) { A[i] = S[i]; V[i] = (i % 4 == 0) ? 1.0 : 0.0; }
-    for (int sweep = 0; sweep < 40; sweep++) {
-        double off = fabs(A[1]) + fabs(A[2]) + fabs(A[5]);
-        if (off == 0.0) break;
-        for (int pq = 0; pq < 3; pq++) {
-            const int p = pq == 2 ? 1 : 0, q = pq == 0 ? 1 : 2;
-            double apq = A[p * 3 + q];
-            if (apq == 0.0) continue;
-            double theta = (A[q * 3 + q] - A[p * 3 + p]) / (2.0 * apq);
-            double t = (theta >= 0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
-            double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
-            for (int k = 0; k < 3; k++) {
-                double akp = A[k * 3 + p], akq = A[k * 3 + q];
-                A[k * 3 + p] = c * akp - s * akq;
-                A[k * 3 + q] = s * akp + c * akq;
-            }
-            for (int k = 0; k < 3; k++) {
-                double apk = A[p * 3 + k], aqk = A[q * 3 + k];
-                A[p * 3 + k] = c * apk - s * aqk;
-                A[q * 3 + k] = s * apk + c * aqk;
-            }
-            A[p * 3 + q] = A[q * 3 + p] = 0.0;
-            for (int k = 0; k < 3; k++) {
-                double vkp = V[k * 3 + p], vkq = V[k * 3 + q];
-                V[k * 3 + p] = c * vkp - s * vkq;
-                V[k * 3 + q] = s * vkp + c * vkq;
-            }
-        }
-    }
-    w[0] = A[0]; w[1] = A[4]; w[2] = A[8];
-}
-
+// ---- batched Kabsch (Hypothesis::calcRigidBodyTransform, Hypothesis.cpp:145-200): thread = problem (kabsch_fit, rigid.cuh).
 __global__ void k_kabsch(int n, int m, const double* __restrict__ a, const double* __restrict__ b, double* R, double* t) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const double* pa = a + (size_t)i * m * 3;
-    const double* pb = b + (size_t)i * m * 3;
-    double cA[3] = {0, 0, 0}, cB[3] = {0, 0, 0};
-    for (int k = 0; k < m; k++)
-        for (int d = 0; d < 3; d++) { cA[d] += pa[k * 3 + d]; cB[d] += pb[k * 3 + d]; }
-    for (int d = 0; d < 3; d++) { cA[d] *= 1.0 / (double)m; cB[d] *= 1.0 / (double)m; }
-    double C[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};   // pointsA * pointsB^T
-    for (int k = 0; k < m; k++)
-        for (int r = 0; r < 3; r++)
-            for (int c = 0; c < 3; c++) C[r * 3 + c] += (pa[k * 3 + r] - cA[r]) * (pb[k * 3 + c] - cB[c]);
-    // SVD C = U diag(s) V^T through the eigen-decomposition of C^T C (V) and U = C V / s
-    double S[9], w[3], V[9];
-    for (int r = 0; r < 3; r++)
-        for (int c = 0; c < 3; c++) S[r * 3 + c] = C[0 * 3 + r] * C[0 * 3 + c] + C[1 * 3 + r] * C[1 * 3 + c] + C[2 * 3 + r] * C[2 * 3 + c];
-    sym_eig3(S, w, V);
-    // order eigenvalues descending
-    int o[3] = {0, 1, 2};
-    if (w[o[0]] < w[o[1]]) { int x = o[0]; o[0] = o[1]; o[1] = x; }
-    if (w[o[1]] < w[o[2]]) { int x = o[1]; o[1] = o[2]; o[2] = x; }
-    if (w[o[0]] < w[o[1]]) { int x = o[0]; o[0] = o[1]; o[1] = x; }
-    double Vs[9], U[9];
-    for (int j = 0; j < 3; j++)
-        for (int k = 0; k < 3; k++) Vs[k * 3 + j] = V[k * 3 + o[j]];
-    for (int j = 0; j < 2; j++) {
-        double u[3], nn = 0;
-        for (int k = 0; k < 3; k++) { u[k] = C[k * 3] * Vs[0 * 3 + j] + C[k * 3 + 1] * Vs[1 * 3 + j] + C[k * 3 + 2] * Vs[2 * 3 + j]; nn += u[k] * u[k]; }
-        nn = nn > 0 ? 1.0 / sqrt(nn) : 0.0;
-        for (int k = 0; k < 3; k++) U[k * 3 + j] = u[k] * nn;
-    }
-    // third left vector: C v3 / s3 when s3 is well above rounding, else completes the right-handed frame
-    {
-        double u[3], nn = 0;
-        for (int k = 0; k < 3; k++) { u[k] = C[k * 3] * Vs[0 * 3 + 2] + C[k * 3 + 1] * Vs[1 * 3 + 2] + C[k * 3 + 2] * Vs[2 * 3 + 2]; nn += u[k] * u[k]; }
-        double cr[3] = {U[3] * U[7] - U[6] * U[4], U[6] * U[1] - U[0] * U[7], U[0] * U[4] - U[3] * U[1]};
-        if (nn > 1e-24 * (w[o[0]] > 0 ? w[o[0]] : 1.0)) {
-            nn = 1.0 / sqrt(nn);
-            for (int k = 0; k < 3; k++) U[k * 3 + 2] = u[k] * nn;
-        } else {
-            for (int k = 0; k < 3; k++) U[k * 3 + 2] = cr[k];
-        }
-    }
-    // sign = det(V U^T) < 0 ? -1 : 1 ; R = V diag(1,1,sign) U^T
-    double VUt[9];
-    for (int r = 0; r < 3; r++)
-        for (int c = 0; c < 3; c++) VUt[r * 3 + c] = Vs[r * 3] * U[c * 3] + Vs[r * 3 + 1] * U[c * 3 + 1] + Vs[r * 3 + 2] * U[c * 3 + 2];
-    double det = VUt[0] * (VUt[4] * VUt[8] - VUt[5] * VUt[7]) - VUt[1] * (VUt[3] * VUt[8] - VUt[5] * VUt[6]) + VUt[2] * (VUt[3] * VUt[7] - VUt[4] * VUt[6]);
-    double sign = det < 0 ? -1.0 : 1.0;
-    double Ro[9];
-    for (int r = 0; r < 3; r++)
-        for (int c = 0; c < 3; c++) Ro[r * 3 + c] = Vs[r * 3] * U[c * 3] + Vs[r * 3 + 1] * U[c * 3 + 1] + sign * Vs[r * 3 + 2] * U[c * 3 + 2];
+    double Ro[9], to[3];
+    kabsch_fit(m, a + (size_t)i * m * 3, b + (size_t)i * m * 3, Ro, to);
     for (int k = 0; k < 9; k++) R[(size_t)i * 9 + k] = Ro[k];
-    for (int r = 0; r < 3; r++) t[(size_t)i * 3 + r] = -(Ro[r * 3] * cA[0] + Ro[r * 3 + 1] * cA[1] + Ro[r * 3 + 2] * cA[2]) + cB[r];
+    for (int r = 0; r < 3; r++) t[(size_t)i * 3 + r] = to[r];
 }
 
 }  // namespace dsac

@@ -23,6 +23,7 @@
 #include "refine.cuh"
 #include "sampler_split.cuh"
 #include "guided.cuh"
+#include "rgbd.cuh"
 #include "train.cuh"
 #include "upstream.cuh"
 #include "objtrain.cuh"
@@ -139,10 +140,18 @@ struct dsac_engine {
     DevMem<uint32_t> d_g_q, d_g_cum; // [max_frames][N] integer weights and their inclusive prefix sums
     DevMem<uint32_t> d_g_bad;        // [max_frames] DSAC_ST_BAD_WEIGHTS
     Event ev_g;                      // recorded after the table kernel: a pass starts only after it
+    Event ev_depth;                  // recorded after the copy of the cell depth: a pass starts only after it
     int g_n = 0;
     unsigned long long g_gen = 0, fwd_g_gen = 0;   // generation of the setting, and the one the last forward ran with
     int fwd_g_n = 0;                 // frames of the last forward if it was guided, else 0
     uint32_t fwd_seed = 0;
+    // RGB-D localisation (dsac_set_cell_depth_device): buffers sized once for max_frames on first use; depth_n == 0: RGB
+    DevMem<float> d_depth;           // [max_frames][N] the setting's per-cell depth (mm)
+    DevMem<double> d_eye;            // [max_frames][N][3] eye coordinates of the pass's cells, NaN without depth
+    DevMem<uint32_t> d_rgbd_skip;    // [max_frames] status bits of frames that sample nothing (DSAC_ST_NO_DEPTH, ...)
+    int depth_n = 0;
+    unsigned long long depth_gen = 0, fwd_depth_gen = 0;   // generation of the setting, and the one the last forward ran with
+    bool fwd_rgbd = false;           // the last forward was an RGB-D pass
     // per-dataset cameras of the pre-training data paths (dsac_set_dataset_cameras), indexed by dataset frame; grow-only.
     // ds_cams_n == 0: no table.  ds_cam0 is entry 0 on the host: the frame size and raw_data every entry shares.
     DevMem<ObjCam> d_ds_cams;
@@ -445,11 +454,15 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
     }
     CUC(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1Smem)));
     CUC(cudaFuncSetAttribute(k_sample_cam, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1Smem)));
+    CUC(cudaFuncSetAttribute(k_sample_rgbd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1Smem)));
+    CUC(cudaFuncSetAttribute(k_sample_rgbd_cam, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1Smem)));
     // k_refine wants 8 CTAs x 26 KB of shared memory per SM: ask for the carve-out explicitly (the default heuristic
     // need not pick the split the launch bounds were written for).  k_sample is left to the default: it spills to
     // local memory, so it wants the L1 that the largest carve-out would take away (DSAC_K1_CARVEOUT overrides).
     CUC(cudaFuncSetAttribute(k_refine, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
     CUC(cudaFuncSetAttribute(k_refine_cam, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    CUC(cudaFuncSetAttribute(k_refine_rgbd, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+    CUC(cudaFuncSetAttribute(k_refine_rgbd_cam, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
     if (const char* co = getenv("DSAC_K1_CARVEOUT")) {
         CUC(cudaFuncSetAttribute(k_sample, cudaFuncAttributePreferredSharedMemoryCarveout, atoi(co)));
         CUC(cudaFuncSetAttribute(k_sample_cam, cudaFuncAttributePreferredSharedMemoryCarveout, atoi(co)));
@@ -565,6 +578,7 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
         CUC(cudaEventCreateWithFlags(e->ev_join.put(), cudaEventDisableTiming));
         CUC(cudaEventCreateWithFlags(e->ev_fwd.put(), cudaEventDisableTiming));
         CUC(cudaEventCreateWithFlags(e->ev_g.put(), cudaEventDisableTiming));
+        CUC(cudaEventCreateWithFlags(e->ev_depth.put(), cudaEventDisableTiming));
         if (const char* ts = getenv("DSAC_TAIL_SPLIT")) e->tail_split = atoi(ts);
     }
 #undef CUC
@@ -623,7 +637,12 @@ static int cameras_begin_pass(dsac_engine* e, int32_t n, cudaStream_t stream) {
         return fail(e, DSAC_ERR_ARG, "n_frames %d differs from the %d frames of the sampling logits (dsac_set_sampling_logits_device)", n, e->g_n);
     if (e->g_n && !e->k1_mode) return fail(e, DSAC_ERR_ARG, "guided sampling needs the split sampler (DSAC_K1_MODE unset)");
     if (e->g_n) CU(cudaStreamWaitEvent(stream, e->ev_g, 0));
+    if (e->depth_n && n != e->depth_n)
+        return fail(e, DSAC_ERR_ARG, "n_frames %d differs from the %d frames of the cell depth (dsac_set_cell_depth_device)", n, e->depth_n);
+    if (e->depth_n) CU(cudaStreamWaitEvent(stream, e->ev_depth, 0));
     e->fwd_cams_gen = e->cams_gen;
+    e->fwd_depth_gen = e->depth_gen;
+    e->fwd_rgbd = e->depth_n > 0;
     e->fwd_g_gen = e->g_gen;
     e->fwd_g_n = e->g_n;
     e->fwd_seed = e->cfg.seed;
@@ -677,6 +696,7 @@ static int sampling_log_prob_run(dsac_engine* e, const char* who, int32_t n, dou
     if (!e->fwd_g_n) return fail(e, DSAC_ERR_ARG, "%s: the last forward pass was not guided", who);
     if (n != e->fwd_g_n) return fail(e, DSAC_ERR_ARG, "%s: n %d differs from the %d frames of the last pass", who, n, e->fwd_g_n);
     if (e->fwd_g_gen != e->g_gen) return fail(e, DSAC_ERR_ARG, "%s: the sampling logits were changed after the last pass", who);
+    if (e->fwd_depth_gen != e->depth_gen) return fail(e, DSAC_ERR_ARG, "%s: the cell depth was changed after the last pass", who);
     if ((!d_logp && !d_grad_logp) || (d_grad_logp && !d_grad)) return fail(e, DSAC_ERR_ARG, "%s: null output", who);
     cudaStream_t stream = (cudaStream_t)stream_v;
     CU(cudaSetDevice(e->cfg.device));
@@ -701,10 +721,37 @@ int dsac_sampling_log_prob_backward_device(dsac_engine* e, int32_t n, const doub
     return sampling_log_prob_run(e, "dsac_sampling_log_prob_backward_device", n, nullptr, d_grad_logp, d_grad_logits, stream);
 }
 
-// A backward pass differentiates the forward before it, which ran with the cameras in force then.
+int dsac_set_cell_depth_device(dsac_engine* e, int32_t n, const float* d_depth, void* stream_v) {
+    if (!e) return DSAC_ERR_ARG;
+    if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_set_cell_depth_device: a submitted pass has not been awaited (dsac_forward_wait)");
+    if (!d_depth) {
+        if (e->depth_n) e->depth_gen++;
+        e->depth_n = 0;
+        return DSAC_OK;
+    }
+    if (n < 1 || n > e->cfg.max_frames)
+        return fail(e, DSAC_ERR_ARG, "dsac_set_cell_depth_device: n %d out of range [1,%d]", n, e->cfg.max_frames);
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    CU(cudaSetDevice(e->cfg.device));
+    const size_t cells = (size_t)e->cfg.max_frames * DSAC_N;
+    CU(e->d_depth.reserve(cells * sizeof(float)));
+    CU(e->d_eye.reserve(cells * 3 * sizeof(double)));
+    CU(e->d_rgbd_skip.reserve((size_t)e->cfg.max_frames * sizeof(uint32_t)));
+    CU(cudaStreamWaitEvent(stream, e->ev_fwd, 0));   // the last forward pass may still read the buffer
+    e->depth_n = 0;                                   // (a failed copy leaves RGB in force)
+    e->depth_gen++;
+    CU(cudaMemcpyAsync(e->d_depth.get(), d_depth, (size_t)n * DSAC_N * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+    CU(cudaEventRecord(e->ev_depth, stream));
+    e->depth_n = n;
+    return DSAC_OK;
+}
+
+// A backward pass differentiates the forward before it, which ran with the cameras and the cell depth in force then.
 static int cameras_unchanged(dsac_engine* e, const char* who) {
     if (e->fwd_cams_gen != e->cams_gen)
         return fail(e, DSAC_ERR_ARG, "%s: the cameras were changed (dsac_set_cameras) after the forward pass", who);
+    if (e->fwd_depth_gen != e->depth_gen)
+        return fail(e, DSAC_ERR_ARG, "%s: the cell depth was changed (dsac_set_cell_depth_device) after the forward pass", who);
     return DSAC_OK;
 }
 
@@ -808,9 +855,19 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
     const Cam* cams = e->cams_n ? e->d_cams + o : nullptr;   // per-frame cameras: those of this range's frames
     const bool guided = e->g_n > 0;                           // guided sampling: this range's frames of the tables
     const GuidedGen gg{guided ? e->d_g_cum + o * DSAC_N : nullptr, guided ? e->d_g_bad + o : nullptr};
+    const bool rgbd = e->depth_n > 0;                         // RGB-D pass: this range's frames of the eye coordinates
+    const double* eye = rgbd ? e->d_eye + o * Nn * 3 : nullptr;
 
     if (e->stages & DSAC_STAGE_SAMPLE) {
         CU(cudaMemsetAsync(e->d_status + o, 0, (size_t)n * sizeof(uint32_t), stream));
+        if (rgbd) {
+            const int ps = pix_shared ? 0 : DSAC_N * 2;
+            const Cam cam0{c.focal, c.cx, c.cy};
+            const uint32_t* gbad = guided ? gg.bad : nullptr;
+            if (cams) k_rgbd_eye_cam<<<(unsigned)n, KE_THREADS, 0, stream>>>(e->d_depth + o * Nn, d_pix, ps, cam0, cams, gbad, e->d_eye + o * Nn * 3, e->d_rgbd_skip + o);
+            else k_rgbd_eye<<<(unsigned)n, KE_THREADS, 0, stream>>>(e->d_depth + o * Nn, d_pix, ps, cam0, nullptr, gbad, e->d_eye + o * Nn * 3, e->d_rgbd_skip + o);
+            e->launches++;
+        }
         SampleParams sp;
         sp.coords = d_coords; sp.pix = d_pix; sp.pix_stride = pix_shared ? 0 : DSAC_N * 2;
         sp.f = c.focal; sp.cx = c.cx; sp.cy = c.cy; sp.cams = cams;
@@ -822,8 +879,11 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
         sp.phase_cycles = e->d_phase;
         { const char* g = getenv("DSAC_K1_A2_GENERIC"); sp.a2_generic = (g && g[0] == '1') ? 1 : 0; }
         sp.resume = nullptr;
+        sp.eye = eye; sp.skip_frame = rgbd ? e->d_rgbd_skip + o : nullptr;
         if (!e->k1_mode) {
-            if (cams) k_sample_cam<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
+            if (rgbd && cams) k_sample_rgbd_cam<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
+            else if (rgbd) k_sample_rgbd<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
+            else if (cams) k_sample_cam<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
             else k_sample<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
             e->launches++;
             CU(cudaGetLastError());
@@ -896,20 +956,22 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             if (e->k1_slot_threads > 0) slot_threads = e->k1_slot_threads;
             auto launch_slot = [&](const K1SplitParams& qq) {
                 const dim3 g(c.n_streams, n);
-                if (guided) k1_gslot<<<g, K1S_THREADS, 0, stream>>>(qq, gg);
+                if (rgbd && guided) k1_gslot_rgbd<<<g, K1S_THREADS, 0, stream>>>(qq, gg);
+                else if (rgbd) k1_slot_rgbd<<<g, K1S_THREADS, 0, stream>>>(qq);
+                else if (guided) k1_gslot<<<g, K1S_THREADS, 0, stream>>>(qq, gg);
                 else if (slot_threads == 1024) k1_slot_t<1024><<<g, 1024, 0, stream>>>(qq);
                 else if (slot_threads == 512) k1_slot_t<512><<<g, 512, 0, stream>>>(qq);
                 else k1_slot<<<g, K1S_THREADS, 0, stream>>>(qq);
             };
             // with the profile on everything runs on one stream so that the event intervals are the kernels' own durations
-            const bool fused = e->k1_fused != 0 && !cams && !guided;   // (k1_fused has no per-frame instantiation; the schedule does not change results)
+            const bool fused = e->k1_fused != 0 && !cams && !guided && !rgbd;   // (k1_fused has no per-frame instantiation; the schedule does not change results)
             // streams: generator on `stream`, filter (and solve) on a side stream; with a batch that does not fill the GPU several
             // times over the solve gets a stream of its own, so that the filter of set k+1 need not wait for the solve of set k
             // (DSAC_K1_OVERLAP=1 / 2 compares them; on an H100 SXM at 700 W: 128 frames 0.856 / 0.862 ms, 1024 frames 3.09 / 3.10 ms)
             const int ov_mode = e->k1_overlap_fixed ? e->k1_overlap : (n_slots <= 768 ? 2 : 1);
             const bool overlap = ov_mode && !e->k1_profile && !fused;
             cudaStream_t side = overlap ? k_side : stream;
-            cudaStream_t solve_side = (overlap && ov_mode >= 2) ? k_side2 : side;
+            cudaStream_t solve_side = (overlap && ov_mode >= 2 && !rgbd) ? k_side2 : side;   // (k1_kabsch: no solve)
             const size_t n_slots_cap = (size_t)e->cfg.max_frames * c.n_streams * (size_t)e->k1_cap;
             mark(-1);
             {
@@ -930,11 +992,11 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             // speculative first round (k1_spec / k1_stitch): one stream generated window by window on many SMs; pays when a
             // stream's first round is several windows long (>= 64 hypotheses per stream) and the GPU is otherwise idle
             const int quota_max = (c.n_hyps + c.n_streams - 1) / c.n_streams;
-            const bool use_spec = few && off == 0 && n_slots <= e->k1_spec_slots && quota_max >= 64 && c.max_candidates >= (1 << 16) && !fused_req && !guided;   // (the candidate bound cannot fall inside the speculative round)
+            const bool use_spec = few && off == 0 && n_slots <= e->k1_spec_slots && quota_max >= 64 && c.max_candidates >= (1 << 16) && !fused_req && !guided && !rgbd;   // (the candidate bound cannot fall inside the speculative round)
             // chained generator (k1_pipe): K CTAs per stream, all of them resident at once
             const int pipe_K = (int)std::min<long long>(8, e->k1_slot_capacity / std::max<long long>(1, n_slots));
             const bool use_pipe = e->k1_pipe && !use_spec && pipe_K >= 3 && n_slots >= 9 && quota_max >= 64 && c.max_candidates >= (1 << 16) &&
-                                  !fused_req && !e->k1_profile && !guided;
+                                  !fused_req && !e->k1_profile && !guided && !rgbd;
             const int n_rounds = (few && !e->k1_rounds_fixed) ? std::min(e->k1_rounds, 2) : e->k1_rounds;
             for (int r = 0; r < n_rounds; r++) {
                 // portions only pay when the generator has the whole GPU to fill (many streams); a few streams (single-frame
@@ -1002,6 +1064,13 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
                         CU(cudaStreamWaitEvent(side, k_ev_gen[set], 0));
                         if (!batch && solve_side != side && set >= 2) CU(cudaStreamWaitEvent(side, k_ev_solve[set - 2], 0));   // the flag-queue region is free again
                     }
+                    if (rgbd) {   // the acceptance test writes the accept bits itself: no flag queue, no solve
+                        if (cams) k1_kabsch_cam<<<fgrid, K1F_THREADS, 0, side>>>(q);
+                        else k1_kabsch<<<fgrid, K1F_THREADS, 0, side>>>(q);
+                        if (!overlap) mark(1);
+                        e->launches += 2;
+                        continue;
+                    }
                     if (cams) k1_filter_cam<<<fgrid, K1F_THREADS, sizeof(K1FSmem), side>>>(q);
                     else k1_filter<<<fgrid, K1F_THREADS, sizeof(K1FSmem), side>>>(q);
                     if (!overlap) mark(1);
@@ -1027,7 +1096,11 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             launch_slot(q);
             mark(0);
             sp.resume = q.state;   // streams the rounds left unfinished (normally none) continue in the monolithic kernel
-            if (guided && cams) k1_gtail_cam<<<dim3(c.n_streams, n), KG_THREADS, 0, stream>>>(q, gg);   // ... or in guided steps
+            if (rgbd && guided && cams) k1_gtail_rgbd_cam<<<dim3(c.n_streams, n), KG_THREADS, 0, stream>>>(q, gg);
+            else if (rgbd && guided) k1_gtail_rgbd<<<dim3(c.n_streams, n), KG_THREADS, 0, stream>>>(q, gg);
+            else if (rgbd && cams) k_sample_rgbd_cam<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
+            else if (rgbd) k_sample_rgbd<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
+            else if (guided && cams) k1_gtail_cam<<<dim3(c.n_streams, n), KG_THREADS, 0, stream>>>(q, gg);   // ... or in guided steps
             else if (guided) k1_gtail<<<dim3(c.n_streams, n), KG_THREADS, 0, stream>>>(q, gg);
             else if (cams) k_sample_cam<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
             else k_sample<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
@@ -1089,7 +1162,7 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             rp.gt_jp = d_gt_jp;
             rp.loss = e->d_loss + o; rp.rot_err = e->d_rot_err + o; rp.t_err = e->d_t_err + o; rp.correct = e->d_correct + o;
         }
-        launch_refine(rp, (unsigned)n, stream);
+        launch_refine(rp, (unsigned)n, stream, eye);
         e->launches++;
         CU(cudaGetLastError());
     }
@@ -1402,7 +1475,7 @@ static int forward_dsac_run(dsac_engine* e, int32_t n, int64_t frame0, const int
             rp.gt_jp = d_gt;
             rp.loss = e->d_ra_loss; rp.rot_err = e->d_ra_rot; rp.t_err = e->d_ra_t; rp.correct = e->d_ra_correct;
         }
-        launch_refine(rp, (unsigned)jobs, stream);
+        launch_refine(rp, (unsigned)jobs, stream, e->depth_n ? e->d_eye.get() : nullptr);
         e->launches++;
         CU(cudaGetLastError());
     }

@@ -84,7 +84,8 @@ __global__ void __launch_bounds__(KG_THREADS) k_guided_table(const float* logits
 // solved and accepted exactly as in the rounds, the first accepted ones in candidate order, until the stream has its
 // quota or max_candidates candidates.  An exhausted stream gets the uniform path's empty hypotheses.  Normally no stream
 // is left: the kernel then returns after one look at the state.
-template <bool PER_FRAME>
+// RGBD: the candidates are accepted by rgbd_accept instead.
+template <bool PER_FRAME, bool RGBD = false>
 __global__ void __launch_bounds__(KG_THREADS) k1_gtail_t(K1SplitParams q, GuidedGen gg) {
     __shared__ uint32_t cum[DSAC_N_CONST];
     __shared__ int warp[2][KG_THREADS / 32];
@@ -114,7 +115,12 @@ __global__ void __launch_bounds__(KG_THREADS) k1_gtail_t(K1SplitParams q, Guided
         int cells[4];
         if (ci < cand_max) {
             guided_draw(cum, p.seed, z, (uint32_t)ci, cells);
-            if (k1_filter_candidate(cell, cells, cam.f, cam.cx, cam.cy, inv_f, cx_f, cy_f, (double)p.thr)) {
+            if constexpr (RGBD) {
+                bool fragile = false;
+                ok = rgbd_accept_cells(p.coords + (size_t)frame * DSAC_N_CONST * 3, p.eye + (size_t)frame * DSAC_N_CONST * 3, pix, cells,
+                                       cam.f, cam.cx, cam.cy, p.thr, rvec, tvec, &fragile);
+                if (fragile) atomicAdd(p.n_fragile, 1ull);
+            } else if (k1_filter_candidate(cell, cells, cam.f, cam.cx, cam.cy, inv_f, cx_f, cy_f, (double)p.thr)) {
                 P3PProblem pr;
                 float obj[12], img[8];
 #pragma unroll
@@ -160,6 +166,8 @@ __global__ void __launch_bounds__(KG_THREADS) k1_gtail_t(K1SplitParams q, Guided
 }
 constexpr auto k1_gtail = k1_gtail_t<false>;
 constexpr auto k1_gtail_cam = k1_gtail_t<true>;
+constexpr auto k1_gtail_rgbd = k1_gtail_t<false, true>;
+constexpr auto k1_gtail_rgbd_cam = k1_gtail_t<true, true>;
 
 struct GuidedLogpParams {
     const double* w;                 // [n][N] softmax of the logits

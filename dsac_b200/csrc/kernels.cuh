@@ -13,6 +13,7 @@
 
 #include "camera.cuh"
 #include "pose_math.cuh"
+#include "rigid.cuh"
 #include "sampler.cuh"
 
 namespace dsac {
@@ -132,6 +133,9 @@ struct SampleParams {
     unsigned long long* phase_cycles;  // [8] or null: thread-0 cycles per phase (development aid)
     int a2_generic;                    // 1: always take the general boundary path (test aid, DSAC_K1_A2_GENERIC=1)
     const K1SlotState* resume;         // null: streams start at their seed; else continue the split sampler's streams
+    // RGB-D passes (dsac_set_cell_depth_device, rigid.cuh): minimal sets are accepted by rgbd_accept
+    const double* eye;                 // [n][N][3] eye coordinates (mm), NaN without depth
+    const uint32_t* skip_frame;        // [n] status bits of a frame that samples nothing (DSAC_ST_NO_DEPTH), else 0
 };
 
 #ifndef K1_THREADS_DEF
@@ -237,7 +241,8 @@ __device__ __forceinline__ int cand_parse_fast(const unsigned char* vals, int q,
 //   C  queue the ~2% that need the full fp64 P3P, in candidate order
 //   D  full solve + reprojection check on the queue, ordered compaction of the accepted
 // PER_FRAME: the camera of the CTA's frame comes from the per-frame table (SampleParams::cams) in place of p.f, p.cx, p.cy.
-template <bool PER_FRAME>
+// RGBD: every candidate goes to phase D, where one lane per candidate runs rgbd_accept in place of the four P3P lanes.
+template <bool PER_FRAME, bool RGBD = false>
 __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS) k_sample_t(SampleParams p) {
     if constexpr (PER_FRAME) {
         const Cam c = p.cams[blockIdx.y];
@@ -260,6 +265,26 @@ __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS) k_sample_t(SamplePa
 
     const K1SlotState* rs = p.resume ? p.resume + ((size_t)frame * p.T + s) : nullptr;
     if (rs && rs->done) return;
+    if constexpr (RGBD) {
+        if (const uint32_t bits = p.skip_frame[frame]) {   // DSAC_ST_NO_DEPTH: nothing is sampled, the hypotheses of an exhausted stream
+            for (int r = tid; r < quota; r += K1_THREADS) {
+                const size_t hi = (size_t)frame * p.H + h0 + r;
+                for (int k = 0; k < 6; k++) p.hyp_pose[hi * 6 + k] = 0.0;
+                float4* P = reinterpret_cast<float4*>(p.hyp_P + hi * 12);
+                P[0] = make_float4((float)p.f, 0.f, 0.f, 0.f);
+                P[1] = make_float4(0.f, (float)p.f, 0.f, 0.f);
+                P[2] = make_float4(0.f, 0.f, 1.f, 0.f);
+                for (int k = 0; k < 4; k++) p.img_idx[hi * 4 + k] = -1;
+                p.cand_idx[hi] = -1;
+            }
+            if (tid == 0) {
+                p.stream_ncand[(size_t)frame * p.T + s] = 0;
+                p.stream_endpos[(size_t)frame * p.T + s] = (s == 0) ? p.skip : 0u;
+                atomicOr(p.status + frame, bits);
+            }
+            return;
+        }
+    }
     if (rs && rs->overflow) rs = nullptr;   // the leftover of a round did not fit the state (cannot happen with the window sizes used): redo the stream from its seed
     // stream s of global frame g: mt19937(seed + g*T + s)   (thread_rand.cpp:52 for g = 0)
     if (!rs && tid == 0) mt_seed(sm.st, p.seed + (uint32_t)((p.frame0 + frame) * (long long)p.T + s));
@@ -309,6 +334,7 @@ __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS) k_sample_t(SamplePa
     };
     // the filter's inputs straight from the cell table: bearings of points 0..2 from the stored 1/|(u, v, 1)|
     auto filter_candidate = [&](const int cells[4]) -> bool {
+        if constexpr (RGBD) return true;
         double bear[3][3], X[4][3], mu3 = 0, mv3 = 0;
 #pragma unroll
         for (int j = 0; j < 4; j++) {
@@ -577,6 +603,11 @@ __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS) k_sample_t(SamplePa
                 ci_keep = ci;
                 cand_parse_fast(sm.vals, sm.cand_start[ci], w_avail, cells);
                 cand = cand_base + ci;
+                if constexpr (RGBD) {
+                    if (sub == 0)
+                        ok = rgbd_accept_cells(coords, p.eye + (size_t)frame * DSAC_N_CONST * 3, pix, cells, p.f, p.cx, p.cy, p.thr, rvec,
+                                               tvec, &fragile);
+                } else {
                 P3PProblem pr;
                 load_problem(cells, pr);
 #pragma unroll
@@ -589,7 +620,9 @@ __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS) k_sample_t(SamplePa
                 p3p_front(pr, p.f, p.cx, p.cy, fr);
                 nsol = p3p_full(pr, fr, p.f, p.cx, p.cy, R, t, &e2, sub, sub + 1);
                 if (nsol == 0) e2 = 1.7976931348623157e308;
+                }
             }
+            if constexpr (!RGBD) {
             // minimum over the group; ties go to the lower root index, as the sequential loop would
             double be = e2;
             int bl = sub;
@@ -601,6 +634,7 @@ __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS) k_sample_t(SamplePa
             }
             if (nsol > 0 && bl == sub)
                 ok = minimal_set_accept(obj, img, p.f, p.cx, p.cy, p.thr, R, t, e2, rvec, tvec, &fragile);
+            }
             if (fragile) atomicAdd(p.n_fragile, 1ull);
             int tot;
             int rank = acc + block_excl_scan<K1_WARPS>(ok ? 1 : 0, &tot, sm.warp[par]);
@@ -691,6 +725,8 @@ __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS) k_sample_t(SamplePa
 
 constexpr auto k_sample = k_sample_t<false>;
 constexpr auto k_sample_cam = k_sample_t<true>;
+constexpr auto k_sample_rgbd = k_sample_t<false, true>;
+constexpr auto k_sample_rgbd_cam = k_sample_t<true, true>;
 
 // ------------------------------------------------------------------ K2: fused scoring
 struct ScoreParams {

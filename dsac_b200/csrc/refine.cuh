@@ -19,6 +19,7 @@
 #include "camera.cuh"
 #include "lm_math.cuh"
 #include "pose_math.cuh"
+#include "rigid.cuh"
 
 namespace dsac {
 
@@ -125,8 +126,10 @@ __device__ double max_loss_dev(const double R1[9], const double t1[3], const dou
 //            compute in its next CALC_J if the trial is accepted -- the same numbers); warp 0 reduces, decides,
 //            solves the damped 6x6 system in registers and builds the next R / dR/dr across its lanes.  Two block
 //            barriers per trial.
-template <bool PER_FRAME>
-__device__ __forceinline__ void k_refine_body(const RefineParams& p) {
+// RGBD (k_refine_rgbd): the selection takes the first inlier_count flagged cells that have depth (eye [n_frames][N][3], NaN
+// without), and the pose update is the Kabsch fit of the selected cells, scene to eye (kabsch_fit), in place of LM.
+template <bool PER_FRAME, bool RGBD = false>
+__device__ __forceinline__ void k_refine_body(const RefineParams& p, const double* eye = nullptr) {
     // the frame's scene coordinates (int16 mm, this job's perturbation applied) and pixel positions, staged once per job:
     // every refinement step reads all of them for the inlier flags and the selected ones in each LM pass
     __shared__ short s_cX[DSAC_N_CONST], s_cY[DSAC_N_CONST], s_cZ[DSAC_N_CONST];
@@ -268,7 +271,8 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p) {
             int count = 0;
             for (int k0 = 0; k0 < DSAC_N_CONST && count < p.inlier_count; k0 += 32) {
                 const int c = __ldg(perm + k0 + lane);
-                const bool flag = (s_bits[c >> 5] >> (c & 31)) & 1u;
+                bool flag = (s_bits[c >> 5] >> (c & 31)) & 1u;
+                if constexpr (RGBD) flag = flag && __ldg(eye + ((size_t)frame * DSAC_N_CONST + c) * 3 + 2) > 0.0;   // (NaN: no depth)
                 const uint32_t m = __ballot_sync(0xffffffffu, flag);
                 const int rank = count + __popc(m & ((1u << lane) - 1u));
                 if (flag && rank < p.inlier_count) {
@@ -283,6 +287,25 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p) {
         const int count = s_count;
         if (count < 50) break;  // cnn_softam.h:1136
 
+        if constexpr (RGBD) {
+            // ---- Kabsch fit of the selected cells: gathered in selection order, one thread fits
+            __shared__ double s_ka[K4_MAX_INLIERS * 3], s_kb[K4_MAX_INLIERS * 3];
+            for (int i = tid; i < count; i += K4_THREADS) {
+                const int c = s_sel[i];
+                const double* e = eye + ((size_t)frame * DSAC_N_CONST + c) * 3;
+                s_ka[i * 3] = (double)s_cX[c]; s_ka[i * 3 + 1] = (double)s_cY[c]; s_ka[i * 3 + 2] = (double)s_cZ[c];
+                s_kb[i * 3] = e[0]; s_kb[i * 3 + 1] = e[1]; s_kb[i * 3 + 2] = e[2];
+            }
+            __syncthreads();
+            if (tid == 0) {
+                double R[9], t[3], r[3];
+                kabsch_fit(count, s_ka, s_kb, R, t);
+                rodrigues_m2v(R, r);
+                s_param[0] = r[0]; s_param[1] = r[1]; s_param[2] = r[2];
+                s_param[3] = t[0]; s_param[4] = t[1]; s_param[5] = t[2];
+            }
+            __syncthreads();
+        } else {
         // ---- Levenberg-Marquardt, CvLevMarq(6, 2n, max_iter 20, eps FLT_EPSILON)
         load_selected(count);
         // (state used by warp 0 only, uniform across its lanes; trial / base parameter vectors live in s_param / s_prev)
@@ -325,6 +348,7 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p) {
                 if (lane == 0) s_ctl = (action == LM_DONE) ? 1 : 0;
             }
             __syncthreads();
+        }
         }
         // NaN -> abort without accepting (cnn_softam.h:1147)
         bool nan = false;
@@ -371,9 +395,15 @@ __global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine(RefinePara
 // the same with the per-frame camera table (RefineParams::cams)
 __global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine_cam(RefineParams p) { k_refine_body<true>(p); }
 
-// one CTA per job, with the instantiation the parameters ask for
-inline void launch_refine(const RefineParams& p, unsigned jobs, cudaStream_t stream) {
-    if (p.cams) k_refine_cam<<<jobs, K4_THREADS, 0, stream>>>(p);
+// the same for RGB-D passes: eye [n_frames][N][3] eye coordinates of the cells (rgbd.cuh)
+__global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine_rgbd(RefineParams p, const double* eye) { k_refine_body<false, true>(p, eye); }
+__global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine_rgbd_cam(RefineParams p, const double* eye) { k_refine_body<true, true>(p, eye); }
+
+// one CTA per job, with the instantiation the parameters ask for; eye != null: an RGB-D pass
+inline void launch_refine(const RefineParams& p, unsigned jobs, cudaStream_t stream, const double* eye = nullptr) {
+    if (eye && p.cams) k_refine_rgbd_cam<<<jobs, K4_THREADS, 0, stream>>>(p, eye);
+    else if (eye) k_refine_rgbd<<<jobs, K4_THREADS, 0, stream>>>(p, eye);
+    else if (p.cams) k_refine_cam<<<jobs, K4_THREADS, 0, stream>>>(p);
     else k_refine<<<jobs, K4_THREADS, 0, stream>>>(p);
 }
 

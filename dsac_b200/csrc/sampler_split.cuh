@@ -234,7 +234,9 @@ __device__ __forceinline__ int k1_round_size(int quota, int acc, long long cand_
 // GUIDED (k1_gslot): the candidates come from guided_draw with the frame's table gg instead of MT19937, one per thread;
 // selection, round sizing and hand-over are the same code.  A guided candidate's stream position (endw) is the stream's
 // starting word: the pass consumes nothing of the MT19937 streams.
-template <int BAR_ID, int BAR_N, int NT, bool TW3 = (NT > 256), bool GUIDED = false>
+// RGBD (k1_slot_rgbd, k1_gslot_rgbd): a frame with SampleParams::skip_frame bits set samples nothing; the candidates go
+// to k1_kabsch instead of k1_filter / k1_solve, which changes nothing here.
+template <int BAR_ID, int BAR_N, int NT, bool TW3 = (NT > 256), bool GUIDED = false, bool RGBD = false>
 __device__ __forceinline__ void k1_slot_body(const K1SplitParams& q, K1GSmemT<NT / 32>& sm, const int tid, const int s, const int frame,
                                              const int slot_ov = -1, const GuidedGen gg = GuidedGen{}) {
     constexpr int NW = NT / 32, SEL_WORDS = K1S_MAX_CAP / 32 / NT;   // warps of the group; accept-bit words per thread in the selection
@@ -278,18 +280,21 @@ __device__ __forceinline__ void k1_slot_body(const K1SplitParams& q, K1GSmemT<NT
             }
             return;
         }
-        if constexpr (GUIDED) {
-            if (gg.bad[frame]) {   // DSAC_ST_BAD_WEIGHTS: nothing is sampled, the hypotheses of an exhausted stream
+        if constexpr (GUIDED || RGBD) {
+            // DSAC_ST_BAD_WEIGHTS / DSAC_ST_NO_DEPTH: nothing is sampled, the hypotheses of an exhausted stream
+            const uint32_t bits = RGBD ? p.skip_frame[frame] : (gg.bad[frame] ? 32u : 0u);
+            if (bits) {
                 k1_empty_hyps(p, frame, h0, quota, tid, NT);
                 if (tid == 0) {
                     S.done = 1; S.acc = 0; S.n_round = 0; S.target = 0; S.cand_base = 0; S.left_n = 0; S.any_reject = 0; S.overflow = 0; S.pos = 0; S.gen = 0;
                     p.stream_ncand[slot] = 0;
                     p.stream_endpos[slot] = (s == 0) ? p.skip : 0u;
-                    atomicOr(p.status + frame, 32u /* DSAC_ST_BAD_WEIGHTS */);
+                    atomicOr(p.status + frame, bits);
                 }
                 return;
             }
-        } else {
+        }
+        if constexpr (!GUIDED) {
             // stream s of global frame g: mt19937(seed + g*T + s)   (thread_rand.cpp:52 for g = 0)
             for (int k = tid; k < MT_N; k += NT) sm.st[k] = S.mt[k];   // seeded by k1_cells
         }
@@ -715,6 +720,15 @@ __global__ void __launch_bounds__(K1S_THREADS, K1S_MIN_BLOCKS) k1_slot(K1SplitPa
 __global__ void __launch_bounds__(K1S_THREADS, K1S_MIN_BLOCKS) k1_gslot(K1SplitParams q, GuidedGen gg) {
     __shared__ K1GSmem sm;
     k1_slot_body<0, 0, K1S_THREADS, false, true>(q, sm, threadIdx.x, blockIdx.x, blockIdx.y, -1, gg);
+}
+// the same two for RGB-D passes (frames without depth sample nothing)
+__global__ void __launch_bounds__(K1S_THREADS, K1S_MIN_BLOCKS) k1_slot_rgbd(K1SplitParams q) {
+    __shared__ K1GSmem sm;
+    k1_slot_body<0, 0, K1S_THREADS, false, false, true>(q, sm, threadIdx.x, blockIdx.x, blockIdx.y);
+}
+__global__ void __launch_bounds__(K1S_THREADS, K1S_MIN_BLOCKS) k1_gslot_rgbd(K1SplitParams q, GuidedGen gg) {
+    __shared__ K1GSmem sm;
+    k1_slot_body<0, 0, K1S_THREADS, false, true, true>(q, sm, threadIdx.x, blockIdx.x, blockIdx.y, -1, gg);
 }
 
 // ------------------------------------------------------------------ k1_spec / k1_stitch: one stream generated by many CTAs
@@ -1538,6 +1552,43 @@ __global__ void __launch_bounds__(K1V_THREADS, K1V_MIN_BLOCKS) k1_solve4(K1Split
 // the same with the per-frame camera table (SampleParams::cams)
 __global__ void __launch_bounds__(K1V_THREADS, K1V_MIN_BLOCKS) k1_solve_cam(K1SplitParams q) { k1_solve_body<K1V_GROUP, true>(q); }
 __global__ void __launch_bounds__(K1V_THREADS, K1V_MIN_BLOCKS) k1_solve4_cam(K1SplitParams q) { k1_solve_body<4, true>(q); }
+
+// ------------------------------------------------------------------ k1_kabsch
+// RGB-D passes: the rounds' acceptance test in place of k1_filter + k1_solve.  It consumes the launch set's work items and
+// writes the accept bits and pose_out that k1_slot's selection reads, one thread per candidate: rgbd_accept is a few
+// hundred fp64 operations, so there is no cheap screen worth a queue of its own.
+template <bool PER_FRAME>
+__global__ void __launch_bounds__(K1F_THREADS) k1_kabsch_t(K1SplitParams q) {
+    const SampleParams& p = q.sp;
+    const int n_items = q.wq_n[q.qidx];
+    const uint2* wq = q.wq + (size_t)q.qidx * q.wq_stride;
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+        const uint2 it2 = wq[item];
+        const int slot = (int)(it2.x >> 7), chunk = (int)(it2.x & 127u);
+        const int frame = slot / p.T, base = chunk * q.chunk, n_here = (int)it2.y;
+        const Cam cam = frame_cam<PER_FRAME>(p, frame);
+        const int16_t* coords = p.coords + (size_t)frame * DSAC_N_CONST * 3;
+        const int32_t* pix = p.pix + (size_t)frame * p.pix_stride;
+        const double* eye = p.eye + (size_t)frame * DSAC_N_CONST * 3;
+        for (int i = threadIdx.x; i < n_here; i += K1F_THREADS) {
+            const int ci = base + i;
+            const uint2 c = q.cells[(size_t)slot * q.cap + ci];
+            const int cells[4] = {(int)(c.x & 0xffffu), (int)(c.x >> 16), (int)(c.y & 0xffffu), (int)(c.y >> 16)};
+            double rvec[3], tvec[3];
+            bool fragile = false;
+            const bool ok = rgbd_accept_cells(coords, eye, pix, cells, cam.f, cam.cx, cam.cy, p.thr, rvec, tvec, &fragile);
+            if (fragile) atomicAdd(p.n_fragile, 1ull);
+            if (ok) {
+                double* po = q.pose_out + ((size_t)slot * q.cap + ci) * 6;
+                po[0] = rvec[0]; po[1] = rvec[1]; po[2] = rvec[2];
+                po[3] = tvec[0]; po[4] = tvec[1]; po[5] = tvec[2];
+                atomicOr(q.accbits + (size_t)slot * (q.cap >> 5) + (ci >> 5), 1u << (ci & 31));
+            }
+        }
+    }
+}
+constexpr auto k1_kabsch = k1_kabsch_t<false>;
+constexpr auto k1_kabsch_cam = k1_kabsch_t<true>;
 
 // The generator is camera-free: the selection of k1_slot writes the rows (fR0 ft0), (fR1 ft1) of hyp_P with the engine's
 // focal length.  With a per-frame camera table this kernel, launched after the sampler, writes them again from the

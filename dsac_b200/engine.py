@@ -16,6 +16,7 @@ N = GRID * GRID
 STAGE_SAMPLE, STAGE_SCORE, STAGE_REFINE, STAGE_EVAL, STAGE_ALL = 1, 2, 4, 8, 15
 ST_SAMPLER_EXHAUSTED, ST_REFINE_ABORTED = 1, 2
 ST_BAD_WEIGHTS = 32          # DSAC_ST_BAD_WEIGHTS
+ST_NO_DEPTH = 64             # DSAC_ST_NO_DEPTH
 
 # every symbol include/dsac_b200.h declares
 EXPORTS = [
@@ -29,7 +30,7 @@ EXPORTS = [
     "dsac_default_rgbd_camera", "dsac_set_dataset_cameras", "dsac_register_depth_device", "dsac_obj_coords_device", "dsac_obj_rng_init_device",
     "dsac_obj_draw_device", "dsac_gather_patches_at_device", "dsac_shuffle_permutation",
     "dsac_score_draw_device", "dsac_score_maps_device", "dsac_shuffle_permutations",
-    "dsac_set_sampling_logits_device", "dsac_sampling_table_device", "dsac_sampling_log_prob_device",
+    "dsac_set_sampling_logits_device", "dsac_set_cell_depth_device", "dsac_sampling_table_device", "dsac_sampling_log_prob_device",
     "dsac_sampling_log_prob_backward_device",
 ]
 
@@ -174,6 +175,7 @@ def load(build_if_missing=True):
     lib.dsac_set_cameras.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.dsac_set_stages.argtypes = [C.c_void_p, C.c_uint32]
     lib.dsac_set_sampling_logits_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.dsac_set_cell_depth_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.dsac_sampling_table_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
     lib.dsac_sampling_log_prob_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.dsac_sampling_log_prob_backward_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -397,6 +399,12 @@ class Engine:
         if cams.ndim != 2 or cams.shape[1] != 3:
             raise ValueError("cameras must be float64 [n][3] (focal, cx, cy), got %s" % (cams.shape,))
         self._check(self.lib.dsac_set_cameras(self.h, cams.shape[0], _p(cams), C.c_void_p(stream) if stream else None))
+
+    def set_cell_depth_device(self, n, d_depth, stream=None):
+        """dsac_set_cell_depth_device: float32 [n][1600] depth in mm per cell on the device (raw pointer as int) makes the
+        following passes RGB-D passes; d_depth None / 0 returns to RGB."""
+        self._check(self.lib.dsac_set_cell_depth_device(self.h, n if d_depth else 0, C.c_void_p(d_depth) if d_depth else None,
+                                                        C.c_void_p(stream) if stream else None))
 
     def set_sampling_logits_device(self, n, d_logits, stream=None):
         """dsac_set_sampling_logits_device: float32 [n][1600] logits on the device (raw pointer as int) guide the sampler of

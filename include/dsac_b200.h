@@ -48,6 +48,7 @@ extern "C" {
 #define DSAC_ST_OBJ_DRAW_EXHAUSTED 8u     /* dsac_obj_draw_device: a patch found no valid centre within max_attempts */
 #define DSAC_ST_DEPTH_DROPPED 16u         /* dsac_register_depth_device: registration targets outside the image were dropped */
 #define DSAC_ST_BAD_WEIGHTS 32u           /* guided sampling: a NaN or +inf logit, or fewer than 4 cells with weight > 0; nothing sampled */
+#define DSAC_ST_NO_DEPTH 64u              /* RGB-D pass: fewer than 4 cells with depth; nothing sampled */
 
 typedef struct dsac_engine dsac_engine;
 
@@ -182,6 +183,22 @@ int dsac_set_cameras(dsac_engine* e, int32_t n, const dsac_camera* cams, void* s
  * long time (INTEGRATION.md).  DSAC_ERR_ARG, with the engine left as it was:
  * n outside [1, max_frames], or a submitted pass that has not been awaited. */
 int dsac_set_sampling_logits_device(dsac_engine* e, int32_t n, const float* d_logits, void* stream);
+/* RGB-D localisation (Brachmann & Rother, TPAMI 2021): the hypotheses of the following passes are Kabsch fits of three
+ * cells' scene coordinates to their eye coordinates instead of P3P solves, and the refinement fits the selected inliers
+ * the same way instead of LM PnP.  d_depth: DEVICE float32 [n][1600], the depth in mm at each cell's grid pixel, cell
+ * y*40+x; a cell has depth iff its value is finite and > 0.  Copied on `stream` into an engine-owned buffer (sized once
+ * for max_frames); the buffer may be reused once `stream` has passed this call.  Cell c of frame g has the eye point
+ * ((u - cx) d / f, (v - cy) d / f, d) in fp64, (u, v) its pix and (f, cx, cy) the frame's camera.  The candidate streams
+ * (MT19937, or Philox when guided), quotas and max_candidates are unchanged; a candidate is accepted iff all four cells
+ * have depth, neither triangle of cells 0..2 (scene, eye) is degenerate (|(P1 - P0) x (P2 - P0)| >= 1 mm^2), all four
+ * points lie in front of the camera under the Kabsch fit of cells 0..2, and all four pass the reprojection check.  A
+ * frame with fewer than 4 cells with depth gets DSAC_ST_NO_DEPTH and no hypotheses (zero poses, img_idx -1).  Scoring is
+ * unchanged: every cell is scored, with or without depth.  Sticky like dsac_set_cameras: later passes must have n frames;
+ * d_depth == NULL (n ignored) returns to RGB.  Every backward entry point differentiates an RGB-D pass with the same jobs
+ * and central differences, the Kabsch fit in place of P3P and LM (depth is not differentiated); they,
+ * dsac_refined_jp6_device and dsac_sampling_log_prob*_device refuse a pass after which the setting changed.
+ * DSAC_ERR_ARG, with the engine left as it was: n outside [1, max_frames], or a submitted pass that has not been awaited. */
+int dsac_set_cell_depth_device(dsac_engine* e, int32_t n, const float* d_depth, void* stream);
 /* The integer weights q [n][1600] of the setting in force (DEVICE uint32), the distribution the sampler draws from.
  * Waits for the setting's table; n must equal its frame count. */
 int dsac_sampling_table_device(dsac_engine* e, int32_t n, uint32_t* d_q);
