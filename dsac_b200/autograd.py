@@ -38,6 +38,10 @@ from registered depth maps) makes the pass an RGB-D pass (INTEGRATION.md, "RGB-D
 refinement are Kabsch fits of scene to eye coordinates.  Like sampling_logits, the engine reads a detached copy applied on
 the current stream, and None leaves the setting alone.  The gradient goes to `prediction` only: depth is not differentiated.
 
+`derivatives` ("central" or "implicit") selects the scene-coordinate derivatives of the backward (INTEGRATION.md,
+"Implicit-function gradients"): it is applied to the engine right before the backward call and stays in force there;
+None leaves the engine's setting alone.
+
 Everything stays on the device, on torch.cuda.current_stream().  The engine holds one pass: a forward on the same engine
 between a loss and its backward() makes that backward() raise.
 """
@@ -133,7 +137,7 @@ def _grad_input(ctx, grad_loss):
 
 class _SoftamLoss(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, prediction, engine, pix, gt_jp, frame0, clamp):
+    def forward(ctx, prediction, engine, pix, gt_jp, frame0, clamp, derivatives):
         n, pix, gt_jp, shared = _check_inputs(engine, prediction, pix, gt_jp)
         stream = torch.cuda.current_stream(prediction.device).cuda_stream
         pred = prediction.detach().contiguous()
@@ -142,19 +146,21 @@ class _SoftamLoss(torch.autograd.Function):
         loss = torch.empty(n, dtype=torch.float64, device=prediction.device)
         engine.fetch_device(n, stream, loss=loss.data_ptr())
         ctx.engine, ctx.pass_id, ctx.n, ctx.clamp = engine, engine.passes, n, clamp
+        ctx.derivatives = derivatives
         ctx.keep = (coords, pix, gt_jp)   # the engine's backward reads the pass's inputs
         return loss
 
     @staticmethod
     def backward(ctx, grad_loss):
         g, grad = _grad_input(ctx, grad_loss)
+        _apply_deriv(ctx)
         ctx.engine.backward_device(ctx.n, g.data_ptr(), None, grad.data_ptr(), ctx.clamp, torch.cuda.current_stream(g.device).cuda_stream)
-        return grad, None, None, None, None, None
+        return grad, None, None, None, None, None, None
 
 
 class _DsacExpectedLoss(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, prediction, engine, pix, gt_jp, frame0, random_draw, clamp):
+    def forward(ctx, prediction, engine, pix, gt_jp, frame0, random_draw, clamp, derivatives):
         n, pix, gt_jp, shared = _check_inputs(engine, prediction, pix, gt_jp)
         stream = torch.cuda.current_stream(prediction.device).cuda_stream
         coords = _coords(engine, prediction.detach().contiguous(), stream)
@@ -162,19 +168,21 @@ class _DsacExpectedLoss(torch.autograd.Function):
         engine.forward_dsac_device(n, coords.data_ptr(), pix.data_ptr(), shared, gt_jp.data_ptr(), random_draw, frame0, stream,
                                    expected_loss=loss.data_ptr())
         ctx.engine, ctx.pass_id, ctx.n, ctx.clamp = engine, engine.passes, n, clamp
+        ctx.derivatives = derivatives
         ctx.keep = (coords, pix, gt_jp)
         return loss
 
     @staticmethod
     def backward(ctx, grad_loss):
         g, grad = _grad_input(ctx, grad_loss)
+        _apply_deriv(ctx)
         ctx.engine.backward_dsac_device(ctx.n, g.data_ptr(), grad.data_ptr(), ctx.clamp, torch.cuda.current_stream(g.device).cuda_stream)
-        return grad, None, None, None, None, None, None
+        return grad, None, None, None, None, None, None, None
 
 
 class _SoftamPose(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, prediction, engine, pix, frame0, clamp):
+    def forward(ctx, prediction, engine, pix, frame0, clamp, derivatives):
         n, pix, _, shared = _check_inputs(engine, prediction, pix, None, need_gt=False)
         stream = torch.cuda.current_stream(prediction.device).cuda_stream
         coords = _coords(engine, prediction.detach().contiguous(), stream)
@@ -182,20 +190,22 @@ class _SoftamPose(torch.autograd.Function):
         pose = torch.empty((n, 6), dtype=torch.float64, device=prediction.device)
         engine.refined_jp6_device(n, pose.data_ptr(), stream)
         ctx.engine, ctx.pass_id, ctx.n, ctx.clamp = engine, engine.passes, n, clamp
+        ctx.derivatives = derivatives
         ctx.keep = (coords, pix)
         return pose
 
     @staticmethod
     def backward(ctx, grad_pose):
         seed, grad = _grad_input(ctx, grad_pose)
+        _apply_deriv(ctx)
         ctx.engine.backward_pose_device(ctx.n, seed.data_ptr(), None, grad.data_ptr(), ctx.clamp,
                                         torch.cuda.current_stream(seed.device).cuda_stream)
-        return grad, None, None, None, None
+        return grad, None, None, None, None, None
 
 
 class _DsacHypotheses(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, prediction, engine, pix, frame0, random_draw, clamp):
+    def forward(ctx, prediction, engine, pix, frame0, random_draw, clamp, derivatives):
         n, pix, _, shared = _check_inputs(engine, prediction, pix, None, need_gt=False)
         stream = torch.cuda.current_stream(prediction.device).cuda_stream
         coords = _coords(engine, prediction.detach().contiguous(), stream)
@@ -206,6 +216,7 @@ class _DsacHypotheses(torch.autograd.Function):
         ref = torch.empty((n, H, 6), dtype=torch.float64, device=prediction.device)
         engine.refined_jp6_device(n, ref.data_ptr(), stream)
         ctx.engine, ctx.pass_id, ctx.n, ctx.clamp = engine, engine.passes, n, clamp
+        ctx.derivatives = derivatives
         ctx.keep = (coords, pix)
         ctx.set_materialize_grads(False)   # an unused output skips its path of the backward
         return sf, ref
@@ -214,52 +225,67 @@ class _DsacHypotheses(torch.autograd.Function):
     def backward(ctx, grad_sf, grad_ref):
         seeds = [g for g in (grad_sf, grad_ref) if g is not None]
         if not seeds:
-            return None, None, None, None, None, None
+            return None, None, None, None, None, None, None
         _, grad = _grad_input(ctx, seeds[0])
         ptr = [g.detach().to(torch.float64).contiguous() if g is not None else None for g in (grad_sf, grad_ref)]
+        _apply_deriv(ctx)
         ctx.engine.backward_dsac_pose_device(ctx.n, ptr[1].data_ptr() if ptr[1] is not None else None,
                                              ptr[0].data_ptr() if ptr[0] is not None else None, grad.data_ptr(), ctx.clamp,
                                              torch.cuda.current_stream(grad.device).cuda_stream)
-        return grad, None, None, None, None, None
+        return grad, None, None, None, None, None, None
 
 
-def softam_loss(engine, prediction, pix, gt_jp, frame0=0, clamp=0.1, cameras=None, sampling_logits=None, cell_depth=None):
+def _deriv(derivatives):
+    if derivatives not in (None, "central", "implicit"):
+        raise ValueError("derivatives must be None, 'central' or 'implicit', got %r" % (derivatives,))
+    return derivatives
+
+
+def _apply_deriv(ctx):
+    # the engine reads the setting when the backward starts; None leaves it as it is
+    if ctx.derivatives is not None:
+        ctx.engine.set_coord_derivatives(ctx.derivatives)
+
+
+def softam_loss(engine, prediction, pix, gt_jp, frame0=0, clamp=0.1, cameras=None, sampling_logits=None, cell_depth=None,
+                derivatives=None):
     """Per-frame loss of the soft-argmax pipeline (train_ransac_softam.cpp) on `prediction`, float64 [n]; differentiable
     with respect to `prediction`.  frame0: global index of the first frame (keys the sampler streams)."""
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
     _set_depth(engine, prediction, cell_depth)
-    return _SoftamLoss.apply(prediction, engine, pix, gt_jp, int(frame0), float(clamp))
+    return _SoftamLoss.apply(prediction, engine, pix, gt_jp, int(frame0), float(clamp), _deriv(derivatives))
 
 
 def dsac_expected_loss(engine, prediction, pix, gt_jp, frame0=0, random_draw=True, clamp=0.1, cameras=None,
-                       sampling_logits=None, cell_depth=None):
+                       sampling_logits=None, cell_depth=None, derivatives=None):
     """Per-frame expected loss of the DSAC / RANSAC variant (train_ransac.cpp) on `prediction`, float64 [n];
     differentiable with respect to `prediction`."""
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
     _set_depth(engine, prediction, cell_depth)
-    return _DsacExpectedLoss.apply(prediction, engine, pix, gt_jp, int(frame0), bool(random_draw), float(clamp))
+    return _DsacExpectedLoss.apply(prediction, engine, pix, gt_jp, int(frame0), bool(random_draw), float(clamp), _deriv(derivatives))
 
 
-def softam_pose(engine, prediction, pix, frame0=0, clamp=0.1, cameras=None, sampling_logits=None, cell_depth=None):
+def softam_pose(engine, prediction, pix, frame0=0, clamp=0.1, cameras=None, sampling_logits=None, cell_depth=None,
+                derivatives=None):
     """Refined pose of every frame of the soft-argmax pipeline as a jp 6-vector [rodrigues(R); t in mm], float64 [n][6];
     differentiable with respect to `prediction`.  Needs no ground truth."""
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
     _set_depth(engine, prediction, cell_depth)
-    return _SoftamPose.apply(prediction, engine, pix, int(frame0), float(clamp))
+    return _SoftamPose.apply(prediction, engine, pix, int(frame0), float(clamp), _deriv(derivatives))
 
 
 def dsac_hypotheses(engine, prediction, pix, frame0=0, random_draw=True, clamp=0.1, cameras=None, sampling_logits=None,
-                    cell_depth=None):
+                    cell_depth=None, derivatives=None):
     """(sf [n][H], refined jp 6-vectors [n][H][6]) of the DSAC / RANSAC variant, both float64 and differentiable with
     respect to `prediction`.  The gradient through the poses covers the hypotheses with sf > 1e-4 whose incoming
     gradient is nonzero; an output that receives no gradient costs nothing in the backward."""
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
     _set_depth(engine, prediction, cell_depth)
-    return _DsacHypotheses.apply(prediction, engine, pix, int(frame0), bool(random_draw), float(clamp))
+    return _DsacHypotheses.apply(prediction, engine, pix, int(frame0), bool(random_draw), float(clamp), _deriv(derivatives))
 
 
 class _SamplingLogProb(torch.autograd.Function):

@@ -13,6 +13,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include "ift.cuh"
 #include "pose_math.cuh"
 #include "refine.cuh"
 #include "rigid.cuh"
@@ -295,8 +296,12 @@ __global__ void __launch_bounds__(32) k_dsac_combine(DsacBwParams p) {
 }
 
 
-// ---- per frame: dLossMax (or the caller's seed) and the refine job list (one warp, lane 0 does the serial scan)
-__global__ void k_bw_prep(BwParams p, int n) {
+// ---- per frame: dLossMax (or the caller's seed) and the refine job list (one warp, lane 0 does the serial scan).
+// IMPLICIT (dsac_set_coord_derivatives): the 12 dRefineHyp jobs only, BW_JOBS_IMPLICIT per frame; dRefineObj is k_refine_ift's.
+constexpr int BW_JOBS_IMPLICIT = 12;
+template <bool IMPLICIT>
+__device__ __forceinline__ void bw_prep_body(const BwParams& p, int n) {
+    constexpr int BW_JOBS = IMPLICIT ? BW_JOBS_IMPLICIT : dsac::BW_JOBS;
     const int frame = blockIdx.x * blockDim.x + threadIdx.x;
     if (frame >= n) return;
     // dLoss/dRefinedPose
@@ -337,6 +342,7 @@ __global__ void k_bw_prep(BwParams p, int n) {
             jp[j * 2] = -1; jp[j * 2 + 1] = 0;
         }
     }
+    if constexpr (IMPLICIT) return;
     // jobs 12..: dRefineObj (cnn_softam.h:866-920): every skip-th ever-inlier pixel, x outer / y inner
     const int32_t* im = p.inlier_map + (size_t)frame * DSAC_N_CONST;
     int32_t* oc = p.s.obj_cells + (size_t)frame * BW_MAX_OBJ_PIX;
@@ -365,8 +371,14 @@ __global__ void k_bw_prep(BwParams p, int n) {
             }
 }
 
-// ---- per frame (one warp): dRefineHyp, dLossMax . dRefineObj into the row, scoreOutputGradients
-__global__ void k_bw_combine(BwParams p, int n) {
+__global__ void k_bw_prep(BwParams p, int n) { bw_prep_body<false>(p, n); }
+__global__ void k_bw_prep_implicit(BwParams p, int n) { bw_prep_body<true>(p, n); }
+
+// ---- per frame (one warp): dRefineHyp, dLossMax . dRefineObj into the row, scoreOutputGradients (IMPLICIT: no dRefineObj
+// columns, k_refine_ift adds them)
+template <bool IMPLICIT>
+__device__ __forceinline__ void bw_combine_body(const BwParams& p, int n) {
+    constexpr int BW_JOBS = IMPLICIT ? BW_JOBS_IMPLICIT : dsac::BW_JOBS;
     const int frame = blockIdx.x, lane = threadIdx.x;
     if (frame >= n) return;
     __shared__ double s_dref[36], s_dl[6], s_dldavg[6];
@@ -392,7 +404,7 @@ __global__ void k_bw_combine(BwParams p, int n) {
     // dRefineObj columns -> row (and the optional 6 x 4800 diagnostic matrix)
     double* row = p.s.row + (size_t)frame * DSAC_N_CONST * 3;
     const int32_t* oc = p.s.obj_cells + (size_t)frame * BW_MAX_OBJ_PIX;
-    for (int col = lane; col < BW_MAX_OBJ_PIX * 3; col += 32) {
+    for (int col = lane; !IMPLICIT && col < BW_MAX_OBJ_PIX * 3; col += 32) {
         const int px = col / 3, c = col % 3;
         if (oc[px] < 0) continue;
         const double* fS = jp6 + (12 + col * 2) * 6;
@@ -423,6 +435,8 @@ __global__ void k_bw_combine(BwParams p, int n) {
         p.s.sog[(size_t)frame * p.H + h] = sf[h] * hf - sf[h] * part;
     }
 }
+__global__ void k_bw_combine(BwParams p, int n) { bw_combine_body<false>(p, n); }
+__global__ void k_bw_combine_implicit(BwParams p, int n) { bw_combine_body<true>(p, n); }
 
 // ---- dPNP (cnn_softam.h:101-146): thread = (hypothesis, column 0..11); 2 full P3P solves each.
 // Also prepares the jp pose + Rodrigues Jacobian of every hypothesis for k_dscore.
@@ -743,6 +757,269 @@ __global__ void __launch_bounds__(K5_THREADS) k_dscore(BwParams p) {
         int x = pt % DSAC_GRID_CONST, y = pt / DSAC_GRID_CONST;
         int colb = p.fix_q4 ? pt * 3 : (x * DSAC_GRID_CONST + y) * 3;
         for (int k = 0; k < 3; k++) row[colb + k] += acc[j][k];
+    }
+}
+
+// ------------------------------------------------------------------ implicit-function derivatives (DSAC_DERIV_IMPLICIT)
+// dRefine / dObj of a refined pose: the IFT of the last accepted refinement step's fit over the cells it fitted (ift.cuh),
+// one CTA per refined pose (job).  The lanes own the recorded cells; the 21 Hessian entries are reduced with the transposed
+// butterfly of k_refine's normal_equations_pass, one lane factors and solves in fp64, then every lane writes its cells.
+struct IftParams {
+    const int16_t* coords;      // [n][N][3]
+    const int32_t* pix;
+    int pix_stride;
+    double f, cx, cy;
+    const Cam* cams;            // [n] or null
+    const double* eye;          // [n][N][3] (RGB-D) or null
+    const int32_t* job_frame;   // [jobs] frame, -1 unused; null: job j -> frame j
+    const double* pose;         // [jobs][6] cv pose the recording replay ended with
+    const uint16_t* sel;        // [jobs][K4_MAX_INLIERS] cells of its last accepted step
+    const int32_t* count;       // [jobs] their number, 0: no step accepted
+    const double* seed;         // [jobs][6] dOuter / d(refined jp6)
+    double* row;                // [n][N*3] += seed . dRefine/dObj (distinct cells per job), or null
+    double* drefobj;            // [n][6][N*3] dRefine/dObj, or null
+    double* contrib;            // [jobs][K4_MAX_INLIERS][3] seed . dRefine/dObj per recorded cell, or null
+};
+constexpr int IFT_THREADS = 64, IFT_WARPS = IFT_THREADS / 32;
+
+// the soft-argmax backward's recording replay (one job per frame), in dsac_engine::ift_buf
+struct IftScratch {
+    double* pose = nullptr;      // [n][6]
+    uint16_t* sel = nullptr;     // [n][K4_MAX_INLIERS]
+    int32_t* count = nullptr;    // [n]
+};
+
+template <bool PER_FRAME, bool RGBD>
+__device__ __forceinline__ void k_refine_ift_body(const IftParams& p) {
+    __shared__ double s_red[IFT_WARPS][32];
+    __shared__ double s_W[36], s_v[6];
+    __shared__ int s_ok;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int job = blockIdx.x;
+    const int frame = p.job_frame ? p.job_frame[job] : job;
+    if (frame < 0) return;
+    const Cam cam = frame_cam<PER_FRAME>(p, frame);
+    const int cnt = p.count[job];
+    const uint16_t* sel = p.sel + (size_t)job * K4_MAX_INLIERS;
+    const int16_t* coords = p.coords + (size_t)frame * DSAC_N_CONST * 3;
+    const int32_t* pix = p.pix + (size_t)frame * p.pix_stride;
+    double pose[6], R[9];
+    for (int k = 0; k < 6; k++) pose[k] = p.pose[(size_t)job * 6 + k];
+    rodrigues_v2m(pose, R);
+    auto point = [&](int i, IftPoint& P) {
+        const int c = sel[i];
+        const double Y[3] = {(double)coords[c * 3], (double)coords[c * 3 + 1], (double)coords[c * 3 + 2]};
+        double e[3];
+        if constexpr (RGBD) {
+            const double* ey = p.eye + ((size_t)frame * DSAC_N_CONST + c) * 3;
+            e[0] = ey[0]; e[1] = ey[1]; e[2] = ey[2];
+        } else {
+            e[0] = (double)pix[c * 2]; e[1] = (double)pix[c * 2 + 1]; e[2] = 0;
+        }
+        ift_point_setup(R, pose + 3, Y, e, cam.f, cam.cx, cam.cy, RGBD, P);
+    };
+    // Hessian: per-lane sums, then the transposed butterfly (lane L ends with entry L), then the warps in order
+    double v[32];
+#pragma unroll
+    for (int k = 0; k < 32; k++) v[k] = 0;
+    for (int i = tid; i < cnt; i += IFT_THREADS) {
+        IftPoint P;
+        point(i, P);
+        ift_point_hess(P, v);
+    }
+#pragma unroll
+    for (int half = 16, off = 16; half >= 1; half >>= 1, off >>= 1) {
+        const bool up = (lane & off) != 0;
+#pragma unroll
+        for (int i = 0; i < 16; i++) {
+            if (i < half) {
+                const double send = up ? v[i] : v[i + half];
+                const double keep = up ? v[i + half] : v[i];
+                v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
+            }
+        }
+    }
+    s_red[warp][lane] = v[0];
+    __syncthreads();
+    if (tid == 0) {
+        double U[21], M[36], Rm[9];
+        for (int k = 0; k < 21; k++) {
+            double t = 0;
+            for (int w = 0; w < IFT_WARPS; w++) t += s_red[w][k];
+            U[k] = t;
+        }
+        bool ok = cnt > 0 && ift_chol6(U);
+        if (ok) {
+            ift_jp_jacobian(pose, Rm, M);
+            ift_weights(U, M, s_W);
+            for (int a = 0; a < 6; a++) {
+                double t = 0;
+                for (int k = 0; k < 6; k++) t += s_W[a * 6 + k] * p.seed[(size_t)job * 6 + k];
+                s_v[a] = t;
+                ok = ok && t - t == 0.0;
+            }
+            for (int k = 0; k < 36; k++) ok = ok && s_W[k] - s_W[k] == 0.0;
+        }
+        s_ok = ok ? 1 : 0;
+    }
+    __syncthreads();
+    const bool ok = s_ok != 0;
+    double* row = p.row ? p.row + (size_t)frame * DSAC_N_CONST * 3 : nullptr;
+    for (int i = tid; i < cnt; i += IFT_THREADS) {
+        const int c = sel[i];
+        double o[3] = {0, 0, 0};
+        if (ok) {
+            IftPoint P;
+            double B[18];
+            point(i, P);
+            ift_point_cross(P, R, B);
+            for (int j = 0; j < 3; j++) {
+                double t = 0;
+                for (int a = 0; a < 6; a++) t += s_v[a] * B[a * 3 + j];
+                o[j] = -t;
+            }
+            if (p.drefobj) {
+                double D[18];
+                ift_point_deriv(s_W, B, D);
+                for (int k = 0; k < 6; k++)
+                    for (int j = 0; j < 3; j++) p.drefobj[((size_t)frame * 6 + k) * DSAC_N_CONST * 3 + c * 3 + j] = D[k * 3 + j];
+            }
+        }
+        for (int j = 0; j < 3; j++) {
+            if (row) row[c * 3 + j] += o[j];
+            if (p.contrib) p.contrib[((size_t)job * K4_MAX_INLIERS + i) * 3 + j] = o[j];
+        }
+    }
+}
+__global__ void __launch_bounds__(IFT_THREADS) k_refine_ift(IftParams p) { k_refine_ift_body<false, false>(p); }
+__global__ void __launch_bounds__(IFT_THREADS) k_refine_ift_cam(IftParams p) { k_refine_ift_body<true, false>(p); }
+__global__ void __launch_bounds__(IFT_THREADS) k_refine_ift_rgbd(IftParams p) { k_refine_ift_body<false, true>(p); }
+__global__ void __launch_bounds__(IFT_THREADS) k_refine_ift_rgbd_cam(IftParams p) { k_refine_ift_body<true, true>(p); }
+
+inline void launch_refine_ift(const IftParams& p, unsigned jobs, cudaStream_t stream) {
+    if (p.eye && p.cams) k_refine_ift_rgbd_cam<<<jobs, IFT_THREADS, 0, stream>>>(p);
+    else if (p.eye) k_refine_ift_rgbd<<<jobs, IFT_THREADS, 0, stream>>>(p);
+    else if (p.cams) k_refine_ift_cam<<<jobs, IFT_THREADS, 0, stream>>>(p);
+    else k_refine_ift<<<jobs, IFT_THREADS, 0, stream>>>(p);
+}
+
+// jp pose + Rodrigues Jacobian of hypothesis h for k_dscore, as k_dpnp / k_dkabsch write it
+__device__ __forceinline__ void write_hypjp(const BwParams& p, int frame, int h) {
+    double* hj = p.s.hypjp + ((size_t)frame * p.H + h) * 39;
+    double R[9], t[3], rod[3], Rt[9], J[27];
+    cv2our_dev(p.hyp_pose + ((size_t)frame * p.H + h) * 6, R, t);
+    rodrigues_m2v(R, rod);
+    rodrigues_jac(rod, Rt, J);
+    for (int k = 0; k < 9; k++) hj[k] = R[k];
+    for (int k = 0; k < 3; k++) hj[9 + k] = t[k];
+    for (int k = 0; k < 27; k++) hj[12 + k] = J[k];
+}
+
+// ---- dPNP by the IFT of the P3P equations at the hypothesis' pose (ift_dpnp_p3p): thread = (hypothesis, column 0..11) as
+// in k_dpnp, one 6x6 solve per column; a singular system or a non-finite column zeroes the hypothesis.
+__global__ void __launch_bounds__(192) k_dpnp_ift(BwParams p) {
+    const int frame = blockIdx.y;
+    const int h = blockIdx.x * 16 + threadIdx.x / 12, col = threadIdx.x % 12;
+    __shared__ int s_bad[16];
+    if (threadIdx.x < 16) s_bad[threadIdx.x] = 0;
+    __syncthreads();
+    const bool active = h < p.H;
+    double out[72];
+    bool ok = true;
+    if (active && col < 9) {
+        const int16_t* coords = p.coords + (size_t)frame * DSAC_N_CONST * 3;
+        const int32_t* pix = p.pix + (size_t)frame * p.pix_stride;
+        const int32_t* idx = p.img_idx + ((size_t)frame * p.H + h) * 4;
+        double X[9], uv[6];
+        for (int j = 0; j < 3; j++) {
+            int c = idx[j];
+            if (c < 0) { ok = false; c = 0; }
+            for (int k = 0; k < 3; k++) X[j * 3 + k] = (double)coords[c * 3 + k];
+            uv[j * 2] = (double)pix[c * 2]; uv[j * 2 + 1] = (double)pix[c * 2 + 1];
+        }
+        const Cam cam = frame_cam(p, frame);
+        ok = ok && ift_dpnp_p3p(p.hyp_pose + ((size_t)frame * p.H + h) * 6, X, uv, cam.f, cam.cx, cam.cy, out, col);
+        if (!ok) s_bad[threadIdx.x / 12] = 1;
+    }
+    __syncthreads();
+    if (active) {
+        const bool zero = s_bad[threadIdx.x / 12] != 0 || col >= 9;
+        double* o = p.s.dpnp + ((size_t)frame * p.H + h) * 72;
+        for (int k = 0; k < 6; k++) o[k * 12 + col] = zero ? 0.0 : out[k * 12 + col];
+        if (col == 0) write_hypjp(p, frame, h);
+    }
+}
+
+// ---- dPNP of an RGB-D pass by the IFT of the 3-point Kabsch fit (ift_dpnp_kabsch); grid and zero rule of k_dpnp_ift
+__global__ void __launch_bounds__(192) k_dkabsch_ift(BwParams p, const double* __restrict__ eye) {
+    const int frame = blockIdx.y;
+    const int h = blockIdx.x * 16 + threadIdx.x / 12, col = threadIdx.x % 12;
+    __shared__ int s_bad[16];
+    if (threadIdx.x < 16) s_bad[threadIdx.x] = 0;
+    __syncthreads();
+    const bool active = h < p.H;
+    double out[72];
+    bool ok = true;
+    if (active && col < 9) {
+        const int16_t* coords = p.coords + (size_t)frame * DSAC_N_CONST * 3;
+        const double* ey = eye + (size_t)frame * DSAC_N_CONST * 3;
+        const int32_t* idx = p.img_idx + ((size_t)frame * p.H + h) * 4;
+        double a[9], b[9];
+        for (int j = 0; j < 3; j++) {
+            int c = idx[j];
+            if (c < 0) { ok = false; c = 0; }
+            for (int k = 0; k < 3; k++) { a[j * 3 + k] = (double)coords[c * 3 + k]; b[j * 3 + k] = ey[c * 3 + k]; }
+        }
+        ok = ok && ift_dpnp_kabsch(a, b, out);
+        if (!ok) s_bad[threadIdx.x / 12] = 1;
+    }
+    __syncthreads();
+    if (active) {
+        const bool zero = s_bad[threadIdx.x / 12] != 0 || col >= 9;
+        double* o = p.s.dpnp + ((size_t)frame * p.H + h) * 72;
+        for (int k = 0; k < 6; k++) o[k * 12 + col] = zero ? 0.0 : out[k * 12 + col];
+        if (col == 0) write_hypjp(p, frame, h);
+    }
+}
+
+// ---- DSAC variant, implicit: the seed of selected hypothesis s, sf_h dLossMax(refined_h, gt) or the caller's seed_h, in
+// w [n H][6]; threads past the selection exit
+__global__ void k_dsac_ift_seed(DsacBwParams p, const int32_t* __restrict__ sel, const int32_t* __restrict__ sel_frame,
+                                const int32_t* __restrict__ totals, double* __restrict__ w) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= totals[0]) return;
+    const int g = sel[s];
+    if (p.seed) {
+        for (int k = 0; k < 6; k++) w[(size_t)s * 6 + k] = p.seed[(size_t)g * 6 + k];
+        return;
+    }
+    const double* gj = p.gt_jp + (size_t)sel_frame[s] * 12;
+    double gt6[6], ref6[6], dl[6];
+    rodrigues_m2v(gj, gt6);
+    gt6[3] = gj[9]; gt6[4] = gj[10]; gt6[5] = gj[11];
+    jp6_from_cv_dev(p.ref_pose + (size_t)g * 6, ref6);
+    dloss_max_dev(ref6, gt6, dl);
+    for (int k = 0; k < 6; k++) w[(size_t)s * 6 + k] = p.sf[g] * dl[k];
+}
+
+// ---- DSAC variant, implicit: path1 += the selected hypotheses' recorded-cell contributions (k_refine_ift's contrib), one
+// warp per frame, hypotheses in selection order (a hypothesis' cells are distinct, so its lanes add independently); the
+// support cells are skipped, as job_cell skips them in central mode.  No atomics: the same call gives the same bits.
+__global__ void __launch_bounds__(32) k_dsac_ift_combine(DsacBwParams p, const int32_t* __restrict__ sel, const int32_t* __restrict__ sel_begin,
+                                                         const uint16_t* __restrict__ rec_sel, const int32_t* __restrict__ rec_count,
+                                                         const double* __restrict__ contrib) {
+    const int frame = blockIdx.x, lane = threadIdx.x;
+    if (frame >= p.n_frames) return;
+    double* row = p.path1 + (size_t)frame * DSAC_N_CONST * 3;
+    for (int s = sel_begin[frame]; s < sel_begin[frame + 1]; s++) {
+        const int32_t* cells = p.img_idx + (size_t)sel[s] * 4;
+        const int cnt = rec_count[s];
+        for (int i = lane; i < cnt; i += 32) {
+            const int c = rec_sel[(size_t)s * K4_MAX_INLIERS + i];
+            if (c == cells[0] || c == cells[1] || c == cells[2] || c == cells[3]) continue;
+            for (int j = 0; j < 3; j++) row[c * 3 + j] += contrib[((size_t)s * K4_MAX_INLIERS + i) * 3 + j];
+        }
+        __syncwarp();
     }
 }
 

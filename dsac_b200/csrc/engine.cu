@@ -11,6 +11,7 @@
 #include <cstddef>
 #include <cstdio>
 #include <cstdlib>
+#include <climits>
 #include <cstring>
 #include <numeric>
 #include <random>
@@ -198,6 +199,9 @@ struct dsac_engine {
     int pending_n = 0, pending_chunks = 0;
     BackwardScratch bw;             // views into bw_buf
     DevMem<char> bw_buf;            // the soft-argmax backward's scratch block, grow-only
+    int coord_deriv = DSAC_DERIV_CENTRAL;   // dsac_set_coord_derivatives
+    IftScratch ift;                 // views into ift_buf (implicit mode's recording replay)
+    DevMem<char> ift_buf;
     std::vector<DevMem<char>> bw_pool;   // device buffers of dsac_backward_dsac, kept across calls
     Stream pipe[4];                 // chunked H2D / compute / D2H pipeline of dsac_forward
     // tail split (dsac_set_tail_split): the whole sampler waves of a batch run on a high-priority side stream, the
@@ -596,6 +600,15 @@ int dsac_set_tail_split(dsac_engine* e, int32_t mode) {
     if (!e) return DSAC_ERR_ARG;
     if (mode < 0 || mode > 2) return fail(e, DSAC_ERR_ARG, "tail split mode %d out of range [0,2]", mode);
     e->tail_split = mode;
+    return DSAC_OK;
+}
+
+int dsac_set_coord_derivatives(dsac_engine* e, int32_t mode) {
+    if (!e) return DSAC_ERR_ARG;
+    if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_set_coord_derivatives: a submitted pass has not been awaited (dsac_forward_wait)");
+    if (mode != DSAC_DERIV_CENTRAL && mode != DSAC_DERIV_IMPLICIT)
+        return fail(e, DSAC_ERR_ARG, "dsac_set_coord_derivatives: mode %d is neither DSAC_DERIV_CENTRAL (0) nor DSAC_DERIV_IMPLICIT (1)", mode);
+    e->coord_deriv = mode;
     return DSAC_OK;
 }
 

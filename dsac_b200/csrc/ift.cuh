@@ -1,0 +1,299 @@
+// ift.cuh -- implicit-function derivatives of a fitted pose with respect to its scene coordinates
+// (dsac_set_coord_derivatives(DSAC_DERIV_IMPLICIT)): the per-point and 6x6 arithmetic, shared by the kernels in
+// backward.cuh and the host build of the tests.
+//
+// A fitted pose theta* is a stationary point of E(theta) = sum_i |r_i(theta, Y_i)|^2 over the cells the fit used:
+//   RGB    r_i = pi(R Y_i + t) - p_i     (pi: pinhole projection with the frame's camera, p_i the cell's pixel)
+//   RGB-D  r_i = R Y_i + t - e_i         (e_i the cell's eye point)
+// so d theta* / d Y_i = -H^-1 B_i with the full Hessian H = d2E / d theta2 (Gauss-Newton terms plus the residual
+// curvature) and B_i = d2E / d theta dY_i (the common factor 2 cancels).  Both are evaluated in the chart
+// R = exp([w]x) R*, t = t* + tau at the solution (xi = (w, tau) = 0), where
+//   d/dw_a exp([w]x) q = e_a x q,   d2/dw_a dw_b exp([w]x) q = (e_a q_b + e_b q_a) / 2 - delta_ab q.
+// The derivative is reported in the jp 6-vector of jp6_from_cv_dev (rodrigues(D R), D t, D = diag(1, -1, -1)):
+// D exp([w]x) R* = exp([D w]x) D R*, so d jp6 / d xi = blockdiag(Jl^-1(r_jp) D, D) with Jl^-1 the inverse left Jacobian of
+// SO(3) -- the matrix->vector Rodrigues Jacobian contracted with the left perturbation, in a form that stays accurate
+// at the jp rotation of an ordinary pose, whose angle is near pi.
+#pragma once
+#include "pose_math.cuh"
+#include "rigid.cuh"
+
+namespace dsac {
+
+// Residual geometry of one point at the solution: q = R Y, X = q + t, the gradients g_m = dr_m/dX of the residual
+// components, Gs = sum_m r_m d2r_m/dX2 and gs = sum_m r_m g_m.
+struct IftPoint {
+    double q[3], g[3][3], Gs[6], gs[3];   // Gs: 00 01 02 11 12 22; RGB: g[2] = 0
+};
+
+// e: the pixel (u, v) for RGB, the eye point for RGB-D
+DSAC_HD void ift_point_setup(const double R[9], const double t[3], const double Y[3], const double e[3], double f, double cx,
+                             double cy, bool rgbd, IftPoint& P) {
+    double X[3];
+    for (int k = 0; k < 3; k++) {
+        P.q[k] = R[k * 3] * Y[0] + R[k * 3 + 1] * Y[1] + R[k * 3 + 2] * Y[2];
+        X[k] = P.q[k] + t[k];
+    }
+    if (rgbd) {
+        for (int m = 0; m < 3; m++) {
+            for (int k = 0; k < 3; k++) P.g[m][k] = m == k ? 1.0 : 0.0;
+            P.gs[m] = X[m] - e[m];
+        }
+        for (int k = 0; k < 6; k++) P.Gs[k] = 0;
+    } else {
+        const double iz = 1.0 / X[2];
+        const double r0 = f * X[0] * iz + cx - e[0], r1 = f * X[1] * iz + cy - e[1];
+        P.g[0][0] = f * iz; P.g[0][1] = 0; P.g[0][2] = -f * X[0] * iz * iz;
+        P.g[1][0] = 0; P.g[1][1] = f * iz; P.g[1][2] = -f * X[1] * iz * iz;
+        for (int k = 0; k < 3; k++) { P.g[2][k] = 0; P.gs[k] = r0 * P.g[0][k] + r1 * P.g[1][k]; }
+        P.Gs[0] = 0; P.Gs[1] = 0; P.Gs[2] = -r0 * f * iz * iz;
+        P.Gs[3] = 0; P.Gs[4] = -r1 * f * iz * iz;
+        P.Gs[5] = 2 * f * iz * iz * iz * (r0 * X[0] + r1 * X[1]);
+    }
+}
+
+// dX / dxi_a: e_a x q (rotation), e_a (translation)
+DSAC_HD void ift_dX(const double q[3], int a, double d[3]) {
+    d[0] = d[1] = d[2] = 0;
+    if (a >= 3) { d[a - 3] = 1; return; }
+    const int b = (a + 1) % 3, c = (a + 2) % 3;
+    d[c] = q[b];
+    d[b] = -q[c];
+}
+
+DSAC_HD double ift_quad(const double Gs[6], const double u[3], const double v[3]) {
+    const double w0 = Gs[0] * v[0] + Gs[1] * v[1] + Gs[2] * v[2];
+    const double w1 = Gs[1] * v[0] + Gs[3] * v[1] + Gs[4] * v[2];
+    const double w2 = Gs[2] * v[0] + Gs[4] * v[1] + Gs[5] * v[2];
+    return u[0] * w0 + u[1] * w1 + u[2] * w2;
+}
+
+// this point's term of the Hessian, added to H21 (upper triangle row by row: 00 01 .. 05 11 .. 55)
+DSAC_HD void ift_point_hess(const IftPoint& P, double H21[21]) {
+    double dX[6][3], J[3][6];
+    for (int a = 0; a < 6; a++) ift_dX(P.q, a, dX[a]);
+    for (int m = 0; m < 3; m++)
+        for (int a = 0; a < 6; a++) J[m][a] = P.g[m][0] * dX[a][0] + P.g[m][1] * dX[a][1] + P.g[m][2] * dX[a][2];
+    const double gq = P.gs[0] * P.q[0] + P.gs[1] * P.q[1] + P.gs[2] * P.q[2];
+    int k = 0;
+    for (int a = 0; a < 6; a++)
+        for (int b = a; b < 6; b++, k++) {
+            double h = 0;
+            for (int m = 0; m < 3; m++) h += J[m][a] * J[m][b];   // (RGB: row 2 of g is zero)
+            h += ift_quad(P.Gs, dX[a], dX[b]);
+            if (b < 3) h += 0.5 * (P.gs[a] * P.q[b] + P.gs[b] * P.q[a]) - (a == b ? gq : 0.0);
+            H21[k] += h;
+        }
+}
+
+// B = d2E / dxi dY of this point (6 x 3, row-major)
+DSAC_HD void ift_point_cross(const IftPoint& P, const double R[9], double B[18]) {
+    double dX[6][3], J[3][6];
+    for (int a = 0; a < 6; a++) ift_dX(P.q, a, dX[a]);
+    for (int m = 0; m < 3; m++)
+        for (int a = 0; a < 6; a++) J[m][a] = P.g[m][0] * dX[a][0] + P.g[m][1] * dX[a][1] + P.g[m][2] * dX[a][2];
+    for (int j = 0; j < 3; j++) {
+        const double c[3] = {R[j], R[3 + j], R[6 + j]};   // dX / dY_j
+        double JY[3];
+        for (int m = 0; m < 3; m++) JY[m] = P.g[m][0] * c[0] + P.g[m][1] * c[1] + P.g[m][2] * c[2];
+        const double cg[3] = {c[1] * P.gs[2] - c[2] * P.gs[1], c[2] * P.gs[0] - c[0] * P.gs[2], c[0] * P.gs[1] - c[1] * P.gs[0]};
+        for (int a = 0; a < 6; a++) {
+            double s = 0;
+            for (int m = 0; m < 3; m++) s += J[m][a] * JY[m];
+            s += ift_quad(P.Gs, dX[a], c);
+            if (a < 3) s += cg[a];   // gs . (e_a x c)
+            B[a * 3 + j] = s;
+        }
+    }
+}
+
+// In-place Cholesky of the packed upper triangle H21 (H = U^T U, U stored in place).  False when H is not positive
+// definite: a pivot below 1e-12 of its diagonal entry, or not finite.
+DSAC_HD bool ift_chol6(double U[21]) {
+    auto at = [](int i, int j) { return i * 6 - i * (i - 1) / 2 + (j - i); };
+    for (int i = 0; i < 6; i++) {
+        const double hii = U[at(i, i)];
+        double d = hii;
+        for (int k = 0; k < i; k++) d -= U[at(k, i)] * U[at(k, i)];
+        if (!(d > 1e-12 * hii) || !(d < 1e300)) return false;
+        d = sqrt(d);
+        U[at(i, i)] = d;
+        for (int j = i + 1; j < 6; j++) {
+            double s = U[at(i, j)];
+            for (int k = 0; k < i; k++) s -= U[at(k, i)] * U[at(k, j)];
+            U[at(i, j)] = s / d;
+        }
+    }
+    return true;
+}
+
+// x = H^-1 b with H = U^T U from ift_chol6
+DSAC_HD void ift_chol6_solve(const double U[21], const double b[6], double x[6]) {
+    auto at = [](int i, int j) { return i * 6 - i * (i - 1) / 2 + (j - i); };
+    double y[6];
+    for (int i = 0; i < 6; i++) {
+        double s = b[i];
+        for (int k = 0; k < i; k++) s -= U[at(k, i)] * y[k];
+        y[i] = s / U[at(i, i)];
+    }
+    for (int i = 5; i >= 0; i--) {
+        double s = y[i];
+        for (int k = i + 1; k < 6; k++) s -= U[at(i, k)] * x[k];
+        x[i] = s / U[at(i, i)];
+    }
+}
+
+// Inverse left Jacobian of SO(3) at rotation vector r: I - [r]x / 2 + c [r]x^2, c = 1/th^2 - cot(th/2) / (2 th)
+DSAC_HD void so3_jl_inv(const double r[3], double Ji[9]) {
+    const double th2 = r[0] * r[0] + r[1] * r[1] + r[2] * r[2], th = sqrt(th2);
+    const double c = th < 1e-4 ? 1.0 / 12 + th2 / 720 : 1.0 / th2 - cos(th / 2) / sin(th / 2) / (2 * th);
+    const double K[9] = {0, -r[2], r[1], r[2], 0, -r[0], -r[1], r[0], 0};
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) {
+            double k2 = 0;
+            for (int k = 0; k < 3; k++) k2 += K[i * 3 + k] * K[k * 3 + j];
+            Ji[i * 3 + j] = (i == j ? 1.0 : 0.0) - 0.5 * K[i * 3 + j] + c * k2;
+        }
+}
+
+// M = d jp6 / d xi (6 x 6, row-major) at the cv pose (rvec, tvec); R gets the cv rotation
+DSAC_HD void ift_jp_jacobian(const double pose[6], double R[9], double M[36]) {
+    rodrigues_v2m(pose, R);
+    double Rj[9], rj[3], Ji[9];
+    for (int k = 0; k < 9; k++) Rj[k] = k < 3 ? R[k] : -R[k];   // D R
+    rodrigues_m2v(Rj, rj);
+    so3_jl_inv(rj, Ji);
+    for (int k = 0; k < 36; k++) M[k] = 0;
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) M[i * 6 + j] = Ji[i * 3 + j] * (j == 0 ? 1.0 : -1.0);
+    M[3 * 6 + 3] = 1; M[4 * 6 + 4] = -1; M[5 * 6 + 5] = -1;
+}
+
+// W = H^-1 M^T (6 x 6, row-major: W[a * 6 + k]) from the Cholesky factor of H
+DSAC_HD void ift_weights(const double U[21], const double M[36], double W[36]) {
+    for (int k = 0; k < 6; k++) {
+        double b[6], x[6];
+        for (int a = 0; a < 6; a++) b[a] = M[k * 6 + a];
+        ift_chol6_solve(U, b, x);
+        for (int a = 0; a < 6; a++) W[a * 6 + k] = x[a];
+    }
+}
+
+// d jp6 / dY of one point, D[k * 3 + j] = -(W^T B)[k][j]
+DSAC_HD void ift_point_deriv(const double W[36], const double B[18], double D[18]) {
+    for (int k = 0; k < 6; k++)
+        for (int j = 0; j < 3; j++) {
+            double s = 0;
+            for (int a = 0; a < 6; a++) s += W[a * 6 + k] * B[a * 3 + j];
+            D[k * 3 + j] = -s;
+        }
+}
+
+// The refinement's IFT over m cells (host form of k_refine_ift): Y [m][3], e [m][3] (pixels (u, v, -) or eye points),
+// pose the cv pose.  D [m][6][3] = d jp6 / dY_i; false (D zero) when H is not positive definite or the result is not finite.
+DSAC_HD bool ift_fit_deriv(int m, const double* Y, const double* e, const double pose[6], double f, double cx, double cy, bool rgbd,
+                           double* D) {
+    double R[9], M[36], H[21] = {0}, W[36];
+    ift_jp_jacobian(pose, R, M);
+    IftPoint P;
+    for (int i = 0; i < m; i++) {
+        ift_point_setup(R, pose + 3, Y + i * 3, e + i * 3, f, cx, cy, rgbd, P);
+        ift_point_hess(P, H);
+    }
+    bool ok = m > 0 && ift_chol6(H);
+    if (ok) ift_weights(H, M, W);
+    for (int i = 0; i < m && ok; i++) {
+        double B[18];
+        ift_point_setup(R, pose + 3, Y + i * 3, e + i * 3, f, cx, cy, rgbd, P);
+        ift_point_cross(P, R, B);
+        ift_point_deriv(W, B, D + i * 18);
+        for (int k = 0; k < 18; k++) ok = ok && D[i * 18 + k] - D[i * 18 + k] == 0.0;
+    }
+    if (!ok)
+        for (int k = 0; k < m * 18; k++) D[k] = 0;
+    return ok;
+}
+
+// Gaussian elimination with partial pivoting of A x = b for `nb` right-hand sides (A 6 x 6, b 6 x nb, both row-major,
+// overwritten; x in b).  False when a pivot is below 1e-13 of the largest entry of A or not finite.
+DSAC_HD bool ift_lu6_solve(double A[36], double* b, int nb) {
+    double amax = 0;
+    for (int k = 0; k < 36; k++) amax = fmax(amax, fabs(A[k]));
+    for (int c = 0; c < 6; c++) {
+        int piv = c;
+        for (int r = c + 1; r < 6; r++)
+            if (fabs(A[r * 6 + c]) > fabs(A[piv * 6 + c])) piv = r;
+        if (!(fabs(A[piv * 6 + c]) > 1e-13 * amax) || !(amax < 1e300)) return false;
+        if (piv != c) {
+            for (int k = 0; k < 6; k++) { const double x = A[c * 6 + k]; A[c * 6 + k] = A[piv * 6 + k]; A[piv * 6 + k] = x; }
+            for (int k = 0; k < nb; k++) { const double x = b[c * nb + k]; b[c * nb + k] = b[piv * nb + k]; b[piv * nb + k] = x; }
+        }
+        for (int r = c + 1; r < 6; r++) {
+            const double l = A[r * 6 + c] / A[c * 6 + c];
+            for (int k = c; k < 6; k++) A[r * 6 + k] -= l * A[c * 6 + k];
+            for (int k = 0; k < nb; k++) b[r * nb + k] -= l * b[c * nb + k];
+        }
+    }
+    for (int c = 5; c >= 0; c--)
+        for (int k = 0; k < nb; k++) {
+            double s = b[c * nb + k];
+            for (int j = c + 1; j < 6; j++) s -= A[c * 6 + j] * b[j * nb + k];
+            b[c * nb + k] = s / A[c * 6 + c];
+        }
+    return true;
+}
+
+// dPNP of a P3P hypothesis by the IFT: the pose (cv) satisfies pi(R X_k + t) = p_k for k = 0..2, six equations in six
+// unknowns, so d xi / dX = -J_xi^-1 J_X.  X [3][3] scene points, uv [3][2] pixels.  out [6][12] = d jp6 / d(point, channel),
+// the 4th point's columns zero; false (out zero) for a singular system or a non-finite result.
+// col in 0..8: only that column is solved for and written (the others stay zero); -1: all nine.
+DSAC_HD bool ift_dpnp_p3p(const double pose[6], const double X[9], const double uv[6], double f, double cx, double cy, double out[72],
+                          int col = -1) {
+    double R[9], M[36], A[36], b[6 * 9];
+    ift_jp_jacobian(pose, R, M);
+    for (int k = 0; k < 6 * 9; k++) b[k] = 0;
+    for (int p = 0; p < 3; p++) {
+        const double e[3] = {uv[p * 2], uv[p * 2 + 1], 0};
+        IftPoint P;
+        ift_point_setup(R, pose + 3, X + p * 3, e, f, cx, cy, false, P);
+        for (int m = 0; m < 2; m++) {
+            double dX[3];
+            for (int a = 0; a < 6; a++) {
+                ift_dX(P.q, a, dX);
+                A[(p * 2 + m) * 6 + a] = P.g[m][0] * dX[0] + P.g[m][1] * dX[1] + P.g[m][2] * dX[2];
+            }
+            for (int j = 0; j < 3; j++)   // -dr / dY_j on the right-hand side
+                if (col < 0) b[(p * 2 + m) * 9 + p * 3 + j] = -(P.g[m][0] * R[j] + P.g[m][1] * R[3 + j] + P.g[m][2] * R[6 + j]);
+                else if (p * 3 + j == col) b[p * 2 + m] = -(P.g[m][0] * R[j] + P.g[m][1] * R[3 + j] + P.g[m][2] * R[6 + j]);
+        }
+    }
+    const int nb = col < 0 ? 9 : 1;
+    bool ok = ift_lu6_solve(A, b, nb);
+    for (int k = 0; k < 72; k++) out[k] = 0;
+    for (int i = 0; i < 6 && ok; i++)
+        for (int c = 0; c < nb; c++) {
+            double s = 0;
+            for (int a = 0; a < 6; a++) s += M[i * 6 + a] * b[a * nb + c];
+            out[i * 12 + (col < 0 ? c : col)] = s;
+            ok = ok && s - s == 0.0;
+        }
+    if (!ok)
+        for (int k = 0; k < 72; k++) out[k] = 0;
+    return ok;
+}
+
+// dPNP of an RGB-D hypothesis by the IFT of the 3-point Kabsch fit, scene a [3][3] to eye b [3][3] (the fit at which it is
+// evaluated is recomputed here); out [6][12] as ift_dpnp_p3p.
+DSAC_HD bool ift_dpnp_kabsch(const double a[9], const double b[9], double out[72]) {
+    double R[9], pose[6], D[3 * 18];
+    kabsch_fit(3, a, b, R, pose + 3);
+    rodrigues_m2v(R, pose);
+    const bool ok = ift_fit_deriv(3, a, b, pose, 0, 0, 0, true, D);
+    for (int i = 0; i < 6; i++) {
+        for (int p = 0; p < 3; p++)
+            for (int j = 0; j < 3; j++) out[i * 12 + p * 3 + j] = D[p * 18 + i * 3 + j];
+        for (int j = 9; j < 12; j++) out[i * 12 + j] = 0;
+    }
+    return ok;
+}
+
+}  // namespace dsac

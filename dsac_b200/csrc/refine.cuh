@@ -128,8 +128,11 @@ __device__ double max_loss_dev(const double R1[9], const double t1[3], const dou
 //            barriers per trial.
 // RGBD (k_refine_rgbd): the selection takes the first inlier_count flagged cells that have depth (eye [n_frames][N][3], NaN
 // without), and the pose update is the Kabsch fit of the selected cells, scene to eye (kabsch_fit), in place of LM.
-template <bool PER_FRAME, bool RGBD = false>
-__device__ __forceinline__ void k_refine_body(const RefineParams& p, const double* eye = nullptr) {
+// RECORD (the recording replay of dsac_set_coord_derivatives(DSAC_DERIV_IMPLICIT)): the cells the last accepted step fitted,
+// in selection order, go to rec_sel [n_jobs][K4_MAX_INLIERS] and their number to rec_count [n_jobs] (0: no step accepted).
+template <bool PER_FRAME, bool RGBD = false, bool RECORD = false>
+__device__ __forceinline__ void k_refine_body(const RefineParams& p, const double* eye = nullptr, uint16_t* rec_sel = nullptr,
+                                              int32_t* rec_count = nullptr) {
     // the frame's scene coordinates (int16 mm, this job's perturbation applied) and pixel positions, staged once per job:
     // every refinement step reads all of them for the inlier flags and the selected ones in each LM pass
     __shared__ short s_cX[DSAC_N_CONST], s_cY[DSAC_N_CONST], s_cZ[DSAC_N_CONST];
@@ -142,6 +145,8 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p, const doubl
     __shared__ double s_red[K4_WARPS][32];
     __shared__ double s_sum[2][32];
     __shared__ int s_count, s_ctl;
+    __shared__ int s_rec_count;                               // (RECORD only)
+    __shared__ unsigned short s_rec[RECORD ? K4_MAX_INLIERS : 1];
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int job = blockIdx.x;
@@ -262,6 +267,9 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p, const doubl
 
     inlier_flags();
 
+    if constexpr (RECORD) {
+        if (tid == 0) s_rec_count = 0;
+    }
     int steps_done = 0, n_perm = 0;
     for (int rStep = 0; rStep < step_limit; rStep++) {
         n_perm++;
@@ -357,6 +365,10 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p, const doubl
         if (nan) break;
         __syncthreads();
         if (tid < 6) s_pose[tid] = s_param[tid];
+        if constexpr (RECORD) {
+            for (int i = tid; i < count; i += K4_THREADS) s_rec[i] = s_sel[i];
+            if (tid == 0) s_rec_count = count;
+        }
         __syncthreads();
         steps_done++;
         inlier_flags();
@@ -364,6 +376,11 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p, const doubl
 
     // ---- outputs
     if (tid < 6) p.out_pose[(size_t)job * 6 + tid] = s_pose[tid];
+    if constexpr (RECORD) {
+        const int rc = s_rec_count;
+        for (int i = tid; i < rc; i += K4_THREADS) rec_sel[(size_t)job * K4_MAX_INLIERS + i] = s_rec[i];
+        if (tid == 0) rec_count[job] = rc;
+    }
     if (p.inlier_map)
         for (int i = tid; i < DSAC_N_CONST; i += K4_THREADS) p.inlier_map[(size_t)job * DSAC_N_CONST + i] = s_imap[i];
     if (tid == 0) {
@@ -399,12 +416,35 @@ __global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine_cam(Refine
 __global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine_rgbd(RefineParams p, const double* eye) { k_refine_body<false, true>(p, eye); }
 __global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine_rgbd_cam(RefineParams p, const double* eye) { k_refine_body<true, true>(p, eye); }
 
+// the recording replays (RECORD: rec_sel [n_jobs][K4_MAX_INLIERS], rec_count [n_jobs])
+__global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine_rec(RefineParams p, uint16_t* rec_sel, int32_t* rec_count) {
+    k_refine_body<false, false, true>(p, nullptr, rec_sel, rec_count);
+}
+__global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine_rec_cam(RefineParams p, uint16_t* rec_sel, int32_t* rec_count) {
+    k_refine_body<true, false, true>(p, nullptr, rec_sel, rec_count);
+}
+__global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine_rgbd_rec(RefineParams p, const double* eye, uint16_t* rec_sel,
+                                                                               int32_t* rec_count) {
+    k_refine_body<false, true, true>(p, eye, rec_sel, rec_count);
+}
+__global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine_rgbd_rec_cam(RefineParams p, const double* eye, uint16_t* rec_sel,
+                                                                                   int32_t* rec_count) {
+    k_refine_body<true, true, true>(p, eye, rec_sel, rec_count);
+}
+
 // one CTA per job, with the instantiation the parameters ask for; eye != null: an RGB-D pass
 inline void launch_refine(const RefineParams& p, unsigned jobs, cudaStream_t stream, const double* eye = nullptr) {
     if (eye && p.cams) k_refine_rgbd_cam<<<jobs, K4_THREADS, 0, stream>>>(p, eye);
     else if (eye) k_refine_rgbd<<<jobs, K4_THREADS, 0, stream>>>(p, eye);
     else if (p.cams) k_refine_cam<<<jobs, K4_THREADS, 0, stream>>>(p);
     else k_refine<<<jobs, K4_THREADS, 0, stream>>>(p);
+}
+inline void launch_refine_record(const RefineParams& p, unsigned jobs, cudaStream_t stream, const double* eye, uint16_t* rec_sel,
+                                 int32_t* rec_count) {
+    if (eye && p.cams) k_refine_rgbd_rec_cam<<<jobs, K4_THREADS, 0, stream>>>(p, eye, rec_sel, rec_count);
+    else if (eye) k_refine_rgbd_rec<<<jobs, K4_THREADS, 0, stream>>>(p, eye, rec_sel, rec_count);
+    else if (p.cams) k_refine_rec_cam<<<jobs, K4_THREADS, 0, stream>>>(p, rec_sel, rec_count);
+    else k_refine_rec<<<jobs, K4_THREADS, 0, stream>>>(p, rec_sel, rec_count);
 }
 
 }  // namespace dsac

@@ -5,7 +5,9 @@
 //   rgbd_accept  the acceptance test of an RGB-D minimal set (dsac_set_cell_depth_device): depth, non-degenerate triangles,
 //                Kabsch on points 0..2, all four points in front of the camera, then the reference's reprojection check
 #pragma once
+#ifdef __CUDACC__
 #include <cuda_runtime.h>
+#endif
 
 #include "pose_math.cuh"
 

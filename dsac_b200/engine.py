@@ -31,7 +31,7 @@ EXPORTS = [
     "dsac_obj_draw_device", "dsac_gather_patches_at_device", "dsac_shuffle_permutation",
     "dsac_score_draw_device", "dsac_score_maps_device", "dsac_shuffle_permutations",
     "dsac_set_sampling_logits_device", "dsac_set_cell_depth_device", "dsac_sampling_table_device", "dsac_sampling_log_prob_device",
-    "dsac_sampling_log_prob_backward_device",
+    "dsac_sampling_log_prob_backward_device", "dsac_set_coord_derivatives",
 ]
 
 ST_OBJ_DRAW_EXHAUSTED = 8    # DSAC_ST_OBJ_DRAW_EXHAUSTED
@@ -176,6 +176,7 @@ def load(build_if_missing=True):
     lib.dsac_set_stages.argtypes = [C.c_void_p, C.c_uint32]
     lib.dsac_set_sampling_logits_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.dsac_set_cell_depth_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.dsac_set_coord_derivatives.argtypes = [C.c_void_p, C.c_int32]
     lib.dsac_sampling_table_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
     lib.dsac_sampling_log_prob_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.dsac_sampling_log_prob_backward_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -405,6 +406,14 @@ class Engine:
         following passes RGB-D passes; d_depth None / 0 returns to RGB."""
         self._check(self.lib.dsac_set_cell_depth_device(self.h, n if d_depth else 0, C.c_void_p(d_depth) if d_depth else None,
                                                         C.c_void_p(stream) if stream else None))
+
+    def set_coord_derivatives(self, mode):
+        """dsac_set_coord_derivatives: "central" (the reference's central differences, the default) or "implicit" (the
+        implicit-function derivatives of the refinement and of the minimal solve; INTEGRATION.md)."""
+        modes = {"central": 0, "implicit": 1}
+        if mode not in modes:
+            raise ValueError("coordinate derivatives must be 'central' or 'implicit', got %r" % (mode,))
+        self._check(self.lib.dsac_set_coord_derivatives(self.h, modes[mode]))
 
     def set_sampling_logits_device(self, n, d_logits, stream=None):
         """dsac_set_sampling_logits_device: float32 [n][1600] logits on the device (raw pointer as int) guide the sampler of

@@ -199,6 +199,23 @@ int dsac_set_sampling_logits_device(dsac_engine* e, int32_t n, const float* d_lo
  * dsac_refined_jp6_device and dsac_sampling_log_prob*_device refuse a pass after which the setting changed.
  * DSAC_ERR_ARG, with the engine left as it was: n outside [1, max_frames], or a submitted pass that has not been awaited. */
 int dsac_set_cell_depth_device(dsac_engine* e, int32_t n, const float* d_depth, void* stream);
+/* Scene-coordinate derivatives of the backward passes (INTEGRATION.md, "Implicit-function gradients").
+ * DSAC_DERIV_CENTRAL (the default): the reference's central differences.  DSAC_DERIV_IMPLICIT: two quantities change.
+ *   dRefineObj  the implicit-function derivative of the refined pose with respect to the cells the last accepted refinement
+ *               step fitted (LM reprojection or, for RGB-D, Kabsch objective over that frozen set, full Hessian), dense
+ *               over those cells, zero elsewhere, with no sub-sampling: sub_sample neither limits nor affects the backward.
+ *               A pose with no accepted step, a Hessian that is not positive definite or a non-finite result gives zeros.
+ *               DSAC variant: per selected hypothesis, the support cells excluded; only the 9 minimal-set pairs remain jobs.
+ *   dPNP        the implicit-function derivative of the P3P equations of points 0..2 at the hypothesis (RGB-D: of the
+ *               3-point Kabsch fit); the 4th point's columns are zero; a singular or non-finite solve zeroes the hypothesis.
+ * Everything else (dRefineHyp, the minimal-set pairs, dScore, the score seam, fix_q4) is unchanged.  Sticky; read when a
+ * backward call starts (dsac_backward, _device, _pose_device, dsac_backward_dsac, _device, _pose_device), so it may change
+ * between a forward and its backward.  DSAC_ERR_ARG, with the engine left as it was: any other mode, or a submitted pass
+ * that has not been awaited. */
+#define DSAC_DERIV_CENTRAL 0
+#define DSAC_DERIV_IMPLICIT 1
+int dsac_set_coord_derivatives(dsac_engine* e, int32_t mode);
+
 /* The integer weights q [n][1600] of the setting in force (DEVICE uint32), the distribution the sampler draws from.
  * Waits for the setting's table; n must equal its frame count. */
 int dsac_sampling_table_device(dsac_engine* e, int32_t n, uint32_t* d_q);
@@ -267,9 +284,9 @@ typedef struct dsac_backward_out {
     double* dloss_dobj;       /* [n][N][3] */
     double* dloss_dref;       /* [n][6]   dLossMax              maxloss.h:87 */
     double* dref_dhyp;        /* [n][36]  dRefineHyp            cnn_softam.h:738 */
-    double* dref_dobj;        /* [n][6][N*3] dRefineObj         cnn_softam.h:853 */
+    double* dref_dobj;        /* [n][6][N*3] dRefineObj         cnn_softam.h:853 (DSAC_DERIV_IMPLICIT: the dense IFT matrix) */
     double* score_grads;      /* [n][H]   scoreOutputGradients  train_ransac_softam.cpp:361-376 */
-    double* dpnp;             /* [n][H][6][12] dPNP             cnn_softam.h:101 */
+    double* dpnp;             /* [n][H][6][12] dPNP             cnn_softam.h:101 (DSAC_DERIV_IMPLICIT: by the IFT) */
 } dsac_backward_out;
 int dsac_backward(dsac_engine* e, int32_t n_frames, const int16_t* coords, const int32_t* pix, int32_t pix_shared,
                   const double* gt_jp, dsac_backward_out* out);
@@ -329,7 +346,7 @@ typedef struct dsac_backward_dsac_out {
     double* path2;            /* [n][N][3]  nullable */
     double* score_grads;      /* [n][H]     scoreOutputGradients, nullable  cnn.h:733-741 */
     int32_t* n_selected;      /* [n]        hypotheses with sf > 1e-4, nullable */
-    int32_t* n_refine_jobs;   /* [n]        refine() evaluations of path I, nullable */
+    int32_t* n_refine_jobs;   /* [n]        refine() evaluations of path I, nullable (DSAC_DERIV_IMPLICIT: 18 per selected hypothesis) */
 } dsac_backward_dsac_out;
 int dsac_backward_dsac(dsac_engine* e, int32_t n_frames, dsac_backward_dsac_out* out);
 /* The same backward after a dsac_forward_dsac(_device), on the caller's `stream` (ordered after that forward by an event):
