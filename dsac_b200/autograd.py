@@ -7,6 +7,7 @@
     pose = softam_pose(engine, prediction, pix)                     # refined jp 6-vector per frame, [n][6]
     sf, ref = dsac_hypotheses(engine, prediction, pix)              # softmax [n][H], refined jp 6-vectors [n][H][6]
     my_loss(pose).backward()                                        # prediction.grad, no ground truth needed
+    unc = pose_uncertainty(engine, n)                               # covariances and support of the last pass's poses
 
 `prediction` is the coordinate CNN's output: float32 [n][1600][3] scene coordinates in metres on the engine's device,
 cell y*40+x.  It is the only input that receives a gradient.  The gradient is the one the reference hands to
@@ -286,6 +287,25 @@ def dsac_hypotheses(engine, prediction, pix, frame0=0, random_draw=True, clamp=0
     _set_sampling(engine, prediction, sampling_logits)
     _set_depth(engine, prediction, cell_depth)
     return _DsacHypotheses.apply(prediction, engine, pix, int(frame0), bool(random_draw), float(clamp), _deriv(derivatives))
+
+
+def pose_uncertainty(engine, n):
+    """Uncertainty of the refined poses of the engine's last pass over n frames (INTEGRATION.md, "Pose uncertainty"), a
+    dict of device tensors on torch.cuda.current_stream(): after softam_pose / softam_loss, one entry per frame
+    (cov_jp6 and cov_xi float64 [n][6][6], sigma2 float64 [n], n_fit, support and ok int32 [n]); after dsac_hypotheses /
+    dsac_expected_loss, one per hypothesis ([n][H][6][6], [n][H]).  cov_xi is the Gauss-Newton covariance of the last
+    refinement step's fit, in the chart R = exp([w]x) R*, t = t* + tau (w rad, tau mm); cov_jp6 the same in the jp
+    6-vector of the pose outputs.  These outputs are not differentiable: they carry no autograd history.  The shapes follow
+    the pass the engine holds (Engine.last_pass), which is the pass the engine reads: a forward it refused leaves both as
+    they were."""
+    dev = torch.device("cuda", engine.cfg.device)
+    lead = (n,) if engine.last_pass(n) == "softam" else (n, engine.cfg.n_hyps)
+    out = {k: torch.empty(lead + (6, 6), dtype=torch.float64, device=dev) for k in ("cov_jp6", "cov_xi")}
+    out["sigma2"] = torch.empty(lead, dtype=torch.float64, device=dev)
+    for k in ("n_fit", "support", "ok"):
+        out[k] = torch.empty(lead, dtype=torch.int32, device=dev)
+    engine.pose_uncertainty_device(n, torch.cuda.current_stream(dev).cuda_stream, **{k: v.data_ptr() for k, v in out.items()})
+    return out
 
 
 class _SamplingLogProb(torch.autograd.Function):

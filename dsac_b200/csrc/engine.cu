@@ -26,6 +26,7 @@
 #include "guided.cuh"
 #include "rgbd.cuh"
 #include "train.cuh"
+#include "uncertainty.cuh"
 #include "upstream.cuh"
 #include "objtrain.cuh"
 #include "scoretrain.cuh"
@@ -202,6 +203,11 @@ struct dsac_engine {
     int coord_deriv = DSAC_DERIV_CENTRAL;   // dsac_set_coord_derivatives
     IftScratch ift;                 // views into ift_buf (implicit mode's recording replay)
     DevMem<char> ift_buf;
+    // dsac_pose_uncertainty_device: its own recording replay (pose, cells, count per job), shared with no backward so
+    // that a call changes no later result; ev_unc is recorded after a call's last launch and the next call waits on it
+    IftScratch unc;
+    DevMem<char> unc_buf;
+    Event ev_unc;
     std::vector<DevMem<char>> bw_pool;   // device buffers of dsac_backward_dsac, kept across calls
     Stream pipe[4];                 // chunked H2D / compute / D2H pipeline of dsac_forward
     // tail split (dsac_set_tail_split): the whole sampler waves of a batch run on a high-priority side stream, the
@@ -583,6 +589,7 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
         CUC(cudaEventCreateWithFlags(e->ev_fwd.put(), cudaEventDisableTiming));
         CUC(cudaEventCreateWithFlags(e->ev_g.put(), cudaEventDisableTiming));
         CUC(cudaEventCreateWithFlags(e->ev_depth.put(), cudaEventDisableTiming));
+        CUC(cudaEventCreateWithFlags(e->ev_unc.put(), cudaEventDisableTiming));
         if (const char* ts = getenv("DSAC_TAIL_SPLIT")) e->tail_split = atoi(ts);
     }
 #undef CUC
@@ -1949,3 +1956,4 @@ int dsac_score_maps_device(dsac_engine* e, int32_t n_images, int32_t hyps_per_im
 
 #include "backward_host.inc"
 #include "backward_dsac_host.inc"
+#include "uncertainty_host.inc"

@@ -13,16 +13,18 @@
 // D exp([w]x) R* = exp([D w]x) D R*, so d jp6 / d xi = blockdiag(Jl^-1(r_jp) D, D) with Jl^-1 the inverse left Jacobian of
 // SO(3) -- the matrix->vector Rodrigues Jacobian contracted with the left perturbation, in a form that stays accurate
 // at the jp rotation of an ordinary pose, whose angle is near pi.
+// The same fit also gives the pose covariance of dsac_pose_uncertainty_device (ift_fit_covariance; uncertainty.cuh): the
+// Gauss-Newton information sum_i J_i^T J_i in the same chart, inverted and scaled by the residual variance.
 #pragma once
 #include "pose_math.cuh"
 #include "rigid.cuh"
 
 namespace dsac {
 
-// Residual geometry of one point at the solution: q = R Y, X = q + t, the gradients g_m = dr_m/dX of the residual
+// Residual geometry of one point at the solution: q = R Y, X = q + t, the residual r, the gradients g_m = dr_m/dX of its
 // components, Gs = sum_m r_m d2r_m/dX2 and gs = sum_m r_m g_m.
 struct IftPoint {
-    double q[3], g[3][3], Gs[6], gs[3];   // Gs: 00 01 02 11 12 22; RGB: g[2] = 0
+    double q[3], r[3], g[3][3], Gs[6], gs[3];   // Gs: 00 01 02 11 12 22; RGB: r[2] = 0, g[2] = 0
 };
 
 // e: the pixel (u, v) for RGB, the eye point for RGB-D
@@ -37,11 +39,13 @@ DSAC_HD void ift_point_setup(const double R[9], const double t[3], const double 
         for (int m = 0; m < 3; m++) {
             for (int k = 0; k < 3; k++) P.g[m][k] = m == k ? 1.0 : 0.0;
             P.gs[m] = X[m] - e[m];
+            P.r[m] = P.gs[m];
         }
         for (int k = 0; k < 6; k++) P.Gs[k] = 0;
     } else {
         const double iz = 1.0 / X[2];
         const double r0 = f * X[0] * iz + cx - e[0], r1 = f * X[1] * iz + cy - e[1];
+        P.r[0] = r0; P.r[1] = r1; P.r[2] = 0;
         P.g[0][0] = f * iz; P.g[0][1] = 0; P.g[0][2] = -f * X[0] * iz * iz;
         P.g[1][0] = 0; P.g[1][1] = f * iz; P.g[1][2] = -f * X[1] * iz * iz;
         for (int k = 0; k < 3; k++) { P.g[2][k] = 0; P.gs[k] = r0 * P.g[0][k] + r1 * P.g[1][k]; }
@@ -83,6 +87,19 @@ DSAC_HD void ift_point_hess(const IftPoint& P, double H21[21]) {
             if (b < 3) h += 0.5 * (P.gs[a] * P.q[b] + P.gs[b] * P.q[a]) - (a == b ? gq : 0.0);
             H21[k] += h;
         }
+}
+
+// this point's Gauss-Newton term J^T J alone (J = dr / dxi), added to acc[0..20] in ift_point_hess' order, and |r|^2 to
+// acc[21]: the information of a least-squares fit, whose residual-curvature terms vanish in expectation
+DSAC_HD void ift_point_gn(const IftPoint& P, double acc[22]) {
+    double dX[6][3], J[3][6];
+    for (int a = 0; a < 6; a++) ift_dX(P.q, a, dX[a]);
+    for (int m = 0; m < 3; m++)
+        for (int a = 0; a < 6; a++) J[m][a] = P.g[m][0] * dX[a][0] + P.g[m][1] * dX[a][1] + P.g[m][2] * dX[a][2];
+    int k = 0;
+    for (int a = 0; a < 6; a++)
+        for (int b = a; b < 6; b++, k++) acc[k] += J[0][a] * J[0][b] + J[1][a] * J[1][b] + J[2][a] * J[2][b];
+    acc[21] += P.r[0] * P.r[0] + P.r[1] * P.r[1] + P.r[2] * P.r[2];
 }
 
 // B = d2E / dxi dY of this point (6 x 3, row-major)
@@ -211,6 +228,62 @@ DSAC_HD bool ift_fit_deriv(int m, const double* Y, const double* e, const double
     if (!ok)
         for (int k = 0; k < m * 18; k++) D[k] = 0;
     return ok;
+}
+
+// Pose covariance of a least-squares fit over m cells from its Gauss-Newton information (the packed upper triangle
+// `info`, factored in place) and its residual sum of squares rss: sigma2 = rss / dof, dof = 2m - 6 (RGB) or 3m - 6 (RGB-D),
+// cov_xi = sigma2 info^-1 in the chart xi = (w, tau) of R = exp([w]x) R*, t = t* + tau, and cov_jp6 = M cov_xi M^T in the
+// jp 6-vector (M = ift_jp_jacobian at the cv pose).  Both outputs are exactly symmetric.  False, with every output zero,
+// when dof <= 0, ift_chol6 rejects the information or an output is not finite.
+DSAC_HD bool ift_cov_from_info(double info[21], double rss, int m, bool rgbd, const double pose[6], double cov_xi[36],
+                               double cov_jp6[36], double* sigma2) {
+    const int dof = (rgbd ? 3 : 2) * m - 6;
+    const double s2 = dof > 0 ? rss / dof : 0.0;
+    bool ok = dof > 0 && ift_chol6(info);
+    if (ok) {
+        for (int k = 0; k < 6; k++) {   // column k of info^-1
+            double b[6] = {0, 0, 0, 0, 0, 0}, x[6];
+            b[k] = 1;
+            ift_chol6_solve(info, b, x);
+            for (int a = 0; a < 6; a++) cov_xi[a * 6 + k] = s2 * x[a];
+        }
+        for (int a = 0; a < 6; a++)
+            for (int b = a + 1; b < 6; b++) cov_xi[a * 6 + b] = cov_xi[b * 6 + a] = 0.5 * (cov_xi[a * 6 + b] + cov_xi[b * 6 + a]);
+        double R[9], M[36], T[36];
+        ift_jp_jacobian(pose, R, M);
+        for (int i = 0; i < 6; i++)
+            for (int b = 0; b < 6; b++) {
+                double s = 0;
+                for (int a = 0; a < 6; a++) s += M[i * 6 + a] * cov_xi[a * 6 + b];
+                T[i * 6 + b] = s;
+            }
+        for (int i = 0; i < 6; i++)
+            for (int j = i; j < 6; j++) {
+                double s = 0;
+                for (int b = 0; b < 6; b++) s += T[i * 6 + b] * M[j * 6 + b];
+                cov_jp6[i * 6 + j] = cov_jp6[j * 6 + i] = s;
+            }
+        ok = s2 - s2 == 0.0;
+        for (int k = 0; k < 36; k++) ok = ok && cov_xi[k] - cov_xi[k] == 0.0 && cov_jp6[k] - cov_jp6[k] == 0.0;
+    }
+    if (!ok)
+        for (int k = 0; k < 36; k++) cov_xi[k] = cov_jp6[k] = 0;
+    *sigma2 = ok ? s2 : 0.0;
+    return ok;
+}
+
+// The covariance of the refined pose over the m cells its last accepted step fitted (host form of k_pose_uncertainty):
+// Y [m][3], e [m][3] (pixels (u, v, -) or eye points), pose the cv pose; outputs and false as ift_cov_from_info.
+DSAC_HD bool ift_fit_covariance(int m, const double* Y, const double* e, const double pose[6], double f, double cx, double cy,
+                                bool rgbd, double cov_xi[36], double cov_jp6[36], double* sigma2) {
+    double R[9], acc[22] = {0};
+    rodrigues_v2m(pose, R);
+    IftPoint P;
+    for (int i = 0; i < m; i++) {
+        ift_point_setup(R, pose + 3, Y + i * 3, e + i * 3, f, cx, cy, rgbd, P);
+        ift_point_gn(P, acc);
+    }
+    return ift_cov_from_info(acc, acc[21], m, rgbd, pose, cov_xi, cov_jp6, sigma2);
 }
 
 // Gaussian elimination with partial pivoting of A x = b for `nb` right-hand sides (A 6 x 6, b 6 x nb, both row-major,

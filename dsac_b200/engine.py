@@ -17,6 +17,7 @@ STAGE_SAMPLE, STAGE_SCORE, STAGE_REFINE, STAGE_EVAL, STAGE_ALL = 1, 2, 4, 8, 15
 ST_SAMPLER_EXHAUSTED, ST_REFINE_ABORTED = 1, 2
 ST_BAD_WEIGHTS = 32          # DSAC_ST_BAD_WEIGHTS
 ST_NO_DEPTH = 64             # DSAC_ST_NO_DEPTH
+PASS_SOFTAM, PASS_DSAC = 1, 2   # DSAC_PASS_SOFTAM, DSAC_PASS_DSAC (dsac_last_pass)
 
 # every symbol include/dsac_b200.h declares
 EXPORTS = [
@@ -31,7 +32,8 @@ EXPORTS = [
     "dsac_obj_draw_device", "dsac_gather_patches_at_device", "dsac_shuffle_permutation",
     "dsac_score_draw_device", "dsac_score_maps_device", "dsac_shuffle_permutations",
     "dsac_set_sampling_logits_device", "dsac_set_cell_depth_device", "dsac_sampling_table_device", "dsac_sampling_log_prob_device",
-    "dsac_sampling_log_prob_backward_device", "dsac_set_coord_derivatives",
+    "dsac_sampling_log_prob_backward_device", "dsac_set_coord_derivatives", "dsac_pose_uncertainty_device",
+    "dsac_last_pass",
 ]
 
 ST_OBJ_DRAW_EXHAUSTED = 8    # DSAC_ST_OBJ_DRAW_EXHAUSTED
@@ -129,6 +131,13 @@ class DsacOut(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in _DSAC_FIELDS]
 
 
+_UNC_FIELDS = ("cov_jp6", "cov_xi", "sigma2", "n_fit", "support", "ok")
+
+
+class PoseUncertaintyOut(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in _UNC_FIELDS]
+
+
 SCORE_HOOK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p)
 SCORE_BACKWARD_HOOK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p)
 
@@ -194,6 +203,8 @@ def load(build_if_missing=True):
     lib.dsac_backward_dsac_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(BackwardDsacOut), C.c_void_p, C.c_float,
                                               C.c_void_p]
     lib.dsac_refined_jp6_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.dsac_pose_uncertainty_device.argtypes = [C.c_void_p, C.c_int32, C.POINTER(PoseUncertaintyOut), C.c_void_p]
+    lib.dsac_last_pass.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
     lib.dsac_backward_pose_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]
     lib.dsac_backward_dsac_pose_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(BackwardDsacOut),
                                                    C.c_void_p, C.c_float, C.c_void_p]
@@ -586,6 +597,24 @@ class Engine:
         """dsac_refined_jp6_device (raw device pointers as ints): jp 6-vectors of the preceding pass's refined poses,
         [n][6] after a soft-argmax forward, [n][H][6] after a DSAC-variant forward."""
         self._check(self.lib.dsac_refined_jp6_device(self.h, n, C.c_void_p(d_jp6), C.c_void_p(stream) if stream else None))
+
+    def pose_uncertainty_device(self, n, stream=None, **ptrs):
+        """dsac_pose_uncertainty_device (raw device pointers as ints); ptrs: device destinations of the fields of
+        dsac_pose_uncertainty_out (cov_jp6, cov_xi, sigma2, n_fit, support, ok), one entry per refined pose of the preceding
+        pass: [n] after a soft-argmax forward, [n][H] after a DSAC-variant forward."""
+        raw = PoseUncertaintyOut()
+        for k, v in ptrs.items():
+            if k not in _UNC_FIELDS:
+                raise KeyError(k)
+            setattr(raw, k, v)
+        self._check(self.lib.dsac_pose_uncertainty_device(self.h, n, C.byref(raw), C.c_void_p(stream) if stream else None))
+
+    def last_pass(self, n):
+        """dsac_last_pass: "softam" or "dsac", the pipeline of the pass over n frames whose refined poses the engine holds
+        (what pose_uncertainty_device reads); raises if it holds none."""
+        kind = C.c_int32(0)
+        self._check(self.lib.dsac_last_pass(self.h, n, C.byref(kind)))
+        return {PASS_SOFTAM: "softam", PASS_DSAC: "dsac"}[kind.value]
 
     def backward_pose_device(self, n, d_grad_ref, d_dloss_dobj=None, d_dloss_dpred=None, clamp=0.0, stream=None):
         """dsac_backward_pose_device (raw device pointers as ints): soft-argmax backward seeded by dOuter/d(refined jp6)."""

@@ -367,6 +367,39 @@ int dsac_backward_dsac_device(dsac_engine* e, int32_t n_frames, const double* d_
  * [n][H][6] after dsac_forward_dsac(_device). */
 int dsac_refined_jp6_device(dsac_engine* e, int32_t n_frames, double* d_jp6, void* stream);
 
+/* Pose uncertainty of the refined poses of the preceding pass (INTEGRATION.md, "Pose uncertainty"): one job per frame after
+ * dsac_forward(_device/_submit), one per hypothesis ([n][H], h fastest) after dsac_forward_dsac(_device).  Stream ordering
+ * and input lifetime as in dsac_backward_device: ordered after the pass by an event, whose coords and pix must still be
+ * valid; no ground truth.  S is the set of cells the job's last accepted refinement step fitted, m = |S|, r_i the residual
+ * of that fit (RGB: reprojection with the frame's camera, px; RGB-D: R Y_i + t - e_i, mm) and J_i = dr_i/dxi at the refined
+ * pose in the chart xi = (w, tau) of R = exp([w]x) R*, t = t* + tau (w rad, tau mm):
+ *   cov_xi  = sigma2 (sum_S J_i^T J_i)^-1, the Gauss-Newton covariance of the fit over S held fixed,
+ *   sigma2  = sum_S |r_i|^2 / (2m - 6) (RGB, px^2) or / (3m - 6) (RGB-D, mm^2),
+ *   cov_jp6 = M cov_xi M^T in the jp 6-vector of dsac_refined_jp6_device, M = d jp6 / d xi.
+ * ok = 0, with the covariances and sigma2 zero, when no step was accepted (n_fit = 0: DSAC_ST_NO_DEPTH, DSAC_ST_BAD_WEIGHTS,
+ * empty hypotheses), the degrees of freedom are <= 0, the information is not positive definite, or a result is not
+ * finite.  support is filled whatever ok is: the cells of all 1600, with or without depth, whose reprojection error at the
+ * refined pose, in k_score's arithmetic with the frame's camera, is below thr2d.  The call changes no later result.
+ * DSAC_ERR_ARG, with the engine left as it was: not after a forward over the same n_frames, a submitted pass that has not
+ * been awaited, cameras or cell depth changed since the pass, or d_out NULL.  The outputs are not differentiated. */
+typedef struct dsac_pose_uncertainty_out {   /* DEVICE pointers, each nullable; jobs = n or n*H */
+    double* cov_jp6;          /* [jobs][6][6] covariance in the jp 6-vector */
+    double* cov_xi;           /* [jobs][6][6] covariance in the left-perturbation chart (w rad, tau mm) */
+    double* sigma2;           /* [jobs]       residual variance estimate (px^2 RGB, mm^2 RGB-D) */
+    int32_t* n_fit;           /* [jobs]       m: cells of the last accepted step, 0 if none */
+    int32_t* support;         /* [jobs]       cells with reprojection error < thr2d at the refined pose */
+    int32_t* ok;              /* [jobs]       1 if the covariance is defined */
+} dsac_pose_uncertainty_out;
+int dsac_pose_uncertainty_device(dsac_engine* e, int32_t n_frames, const dsac_pose_uncertainty_out* d_out, void* stream);
+/* The pipeline of the forward pass over n_frames whose refined poses the engine holds, i.e. whose poses
+ * dsac_pose_uncertainty_device reads: DSAC_PASS_SOFTAM (n_frames jobs) or DSAC_PASS_DSAC (n_frames * n_hyps jobs, h fastest).
+ * A caller that sizes the outputs of dsac_pose_uncertainty_device asks here rather than tracking its own forward calls,
+ * since a refused forward leaves the engine's pass as it was.  DSAC_ERR_ARG (*pipeline untouched) when the engine holds no
+ * pass over n_frames. */
+#define DSAC_PASS_SOFTAM 1
+#define DSAC_PASS_DSAC 2
+int dsac_last_pass(dsac_engine* e, int32_t n_frames, int32_t* pipeline);
+
 /* Soft-argmax backward seeded by d_grad_ref [n][6] = dOuter/d(refined jp6) instead of dLossMax.
  * No ground truth needed. dloss_dobj / dloss_dpred / clamp as in dsac_backward_device; clamp applies to the total. */
 int dsac_backward_pose_device(dsac_engine* e, int32_t n_frames, const double* d_grad_ref,
