@@ -39,6 +39,11 @@ from registered depth maps) makes the pass an RGB-D pass (INTEGRATION.md, "RGB-D
 refinement are Kabsch fits of scene to eye coordinates.  Like sampling_logits, the engine reads a detached copy applied on
 the current stream, and None leaves the setting alone.  The gradient goes to `prediction` only: depth is not differentiated.
 
+`pose_priors` = (poses, info, gate) puts k caller poses per frame into the hypothesis pool (INTEGRATION.md, "Pose
+priors"): poses float64 [n][k][6] cv poses, info float64 [n][k][6][6] information matrices or None (no gate), gate the
+chi^2 bound of the gate.  Like cell_depth, the engine reads a detached copy applied on the current stream, and None
+leaves the setting alone.  The priors are constants: no gradient flows to them.
+
 `derivatives` ("central" or "implicit") selects the scene-coordinate derivatives of the backward (INTEGRATION.md,
 "Implicit-function gradients"): it is applied to the engine right before the backward call and stays in force there;
 None leaves the engine's setting alone.
@@ -242,6 +247,28 @@ def _deriv(derivatives):
     return derivatives
 
 
+def _set_priors(engine, prediction, priors):
+    if priors is None:
+        return
+    poses, info, gate = priors
+    n = prediction.shape[0]
+    if poses.dtype != torch.float64 or poses.dim() != 3 or poses.shape[0] != n or poses.shape[2] != 6 \
+            or poses.device != prediction.device:
+        raise ValueError("pose_priors poses must be float64 [%d][k][6] on %s, got %s %s on %s"
+                         % (n, prediction.device, poses.dtype, tuple(poses.shape), poses.device))
+    k = poses.shape[1]
+    if info is not None and (info.dtype != torch.float64 or tuple(info.shape) != (n, k, 6, 6) or info.device != prediction.device):
+        raise ValueError("pose_priors info must be float64 [%d][%d][6][6] on %s, got %s %s on %s"
+                         % (n, k, prediction.device, info.dtype, tuple(info.shape), info.device))
+    pc = poses.detach().contiguous()
+    ic = info.detach().contiguous() if info is not None else None
+    stream = torch.cuda.current_stream(prediction.device)
+    engine.set_pose_priors_device(n, k, pc.data_ptr(), ic.data_ptr() if ic is not None else None, float(gate), stream.cuda_stream)
+    pc.record_stream(stream)
+    if ic is not None:
+        ic.record_stream(stream)
+
+
 def _apply_deriv(ctx):
     # the engine reads the setting when the backward starts; None leaves it as it is
     if ctx.derivatives is not None:
@@ -249,43 +276,47 @@ def _apply_deriv(ctx):
 
 
 def softam_loss(engine, prediction, pix, gt_jp, frame0=0, clamp=0.1, cameras=None, sampling_logits=None, cell_depth=None,
-                derivatives=None):
+                derivatives=None, pose_priors=None):
     """Per-frame loss of the soft-argmax pipeline (train_ransac_softam.cpp) on `prediction`, float64 [n]; differentiable
     with respect to `prediction`.  frame0: global index of the first frame (keys the sampler streams)."""
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
     _set_depth(engine, prediction, cell_depth)
+    _set_priors(engine, prediction, pose_priors)
     return _SoftamLoss.apply(prediction, engine, pix, gt_jp, int(frame0), float(clamp), _deriv(derivatives))
 
 
 def dsac_expected_loss(engine, prediction, pix, gt_jp, frame0=0, random_draw=True, clamp=0.1, cameras=None,
-                       sampling_logits=None, cell_depth=None, derivatives=None):
+                       sampling_logits=None, cell_depth=None, derivatives=None, pose_priors=None):
     """Per-frame expected loss of the DSAC / RANSAC variant (train_ransac.cpp) on `prediction`, float64 [n];
     differentiable with respect to `prediction`."""
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
     _set_depth(engine, prediction, cell_depth)
+    _set_priors(engine, prediction, pose_priors)
     return _DsacExpectedLoss.apply(prediction, engine, pix, gt_jp, int(frame0), bool(random_draw), float(clamp), _deriv(derivatives))
 
 
 def softam_pose(engine, prediction, pix, frame0=0, clamp=0.1, cameras=None, sampling_logits=None, cell_depth=None,
-                derivatives=None):
+                derivatives=None, pose_priors=None):
     """Refined pose of every frame of the soft-argmax pipeline as a jp 6-vector [rodrigues(R); t in mm], float64 [n][6];
     differentiable with respect to `prediction`.  Needs no ground truth."""
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
     _set_depth(engine, prediction, cell_depth)
+    _set_priors(engine, prediction, pose_priors)
     return _SoftamPose.apply(prediction, engine, pix, int(frame0), float(clamp), _deriv(derivatives))
 
 
 def dsac_hypotheses(engine, prediction, pix, frame0=0, random_draw=True, clamp=0.1, cameras=None, sampling_logits=None,
-                    cell_depth=None, derivatives=None):
+                    cell_depth=None, derivatives=None, pose_priors=None):
     """(sf [n][H], refined jp 6-vectors [n][H][6]) of the DSAC / RANSAC variant, both float64 and differentiable with
     respect to `prediction`.  The gradient through the poses covers the hypotheses with sf > 1e-4 whose incoming
     gradient is nonzero; an output that receives no gradient costs nothing in the backward."""
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
     _set_depth(engine, prediction, cell_depth)
+    _set_priors(engine, prediction, pose_priors)
     return _DsacHypotheses.apply(prediction, engine, pix, int(frame0), bool(random_draw), float(clamp), _deriv(derivatives))
 
 

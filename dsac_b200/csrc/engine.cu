@@ -34,6 +34,7 @@
 using namespace dsac;
 
 static_assert(sizeof(Cam) == sizeof(dsac_camera), "Cam mirrors dsac_camera");
+static_assert(PRIOR_MAX == DSAC_MAX_PRIORS && PRIOR_ST_BAD == DSAC_ST_BAD_PRIOR, "prior.cuh mirrors dsac_b200.h");
 static_assert(sizeof(ObjCam) == sizeof(dsac_rgbd_camera) && offsetof(ObjCam, sensor_trans) == offsetof(dsac_rgbd_camera, sensor_trans) &&
                   offsetof(ObjCam, raw_data) == offsetof(dsac_rgbd_camera, raw_data),
               "ObjCam mirrors dsac_rgbd_camera");
@@ -154,6 +155,18 @@ struct dsac_engine {
     int depth_n = 0;
     unsigned long long depth_gen = 0, fwd_depth_gen = 0;   // generation of the setting, and the one the last forward ran with
     bool fwd_rgbd = false;           // the last forward was an RGB-D pass
+    // pose priors (dsac_set_pose_priors_device): tables sized once for max_frames x DSAC_MAX_PRIORS on first use; prior_n == 0:
+    // none.  The prior of frame f, index j, takes hypothesis slot n_hyps - prior_k + j.
+    DevMem<double> d_prior_pose;     // [prior_n][prior_k][6] cv poses
+    DevMem<double> d_prior_info;     // [prior_n][prior_k][36] information matrices (a gate only)
+    DevMem<PriorGate> d_prior_tab;   // [prior_n][prior_k] what the gate reads (k_prior_prep)
+    DevMem<uint32_t> d_prior_bad;    // [prior_n] DSAC_ST_BAD_PRIOR or 0
+    Event ev_prior;                  // recorded after k_prior_prep: a pass starts only after it
+    int prior_n = 0, prior_k = 0;
+    bool prior_gate = false;
+    double prior_chi2 = 0;
+    unsigned long long prior_gen = 0, fwd_prior_gen = 0;   // generation of the setting, and the one the last forward ran with
+    int fwd_prior_k = 0;             // priors per frame of the last forward
     // per-dataset cameras of the pre-training data paths (dsac_set_dataset_cameras), indexed by dataset frame; grow-only.
     // ds_cams_n == 0: no table.  ds_cam0 is entry 0 on the host: the frame size and raw_data every entry shares.
     DevMem<ObjCam> d_ds_cams;
@@ -221,7 +234,8 @@ struct dsac_engine {
     int k1_rounds = 3, k1_cap = 0;   // rounds 0..2 finish every stream of the benchmark batches; a straggler continues in k_sample (resume). 5 rounds = 6 empty launches per pass
     bool k1_rounds_fixed = false;   // DSAC_K1_ROUNDS given
     int k1_filter_grid = 0, k1_solve_grid = 0;
-    unsigned long long k1_calls[2] = {0, 0};     // passes by sampler: [0] uniform, [1] guided (parity selects the statistics block)
+    unsigned long long k1_calls[4] = {0, 0, 0, 0};   // passes by sampler: [0] uniform, [1] guided, [2] gated uniform, [3] gated
+                                                     // guided (parity selects the statistics block)
     DevMem<K1SlotState> d_k1_state;
     DevMem<CellRec> d_k1_celltab;
     DevMem<uint2> d_k1_cells;
@@ -231,9 +245,10 @@ struct dsac_engine {
     DevMem<uint2> d_k1_wq;
     DevMem<uint32_t> d_k1_fq;
     DevMem<int> d_k1_counters;                    // wq_n[K1S_MAX_ROUNDS], fq_n[K1S_MAX_ROUNDS]
-    DevMem<unsigned long long> d_k1_stats;        // [2][2][2]: candidates / hypotheses of finished streams, by sampler (uniform,
-                                                  // guided) and call parity: the first round of a pass is sized from the last
-                                                  // pass of the same sampler, whose rate can differ from the other's many times over
+    DevMem<unsigned long long> d_k1_stats;        // [4][2][2]: candidates / hypotheses of finished streams, by sampler (uniform,
+                                                  // guided, and each of them gated by pose priors) and call parity: the first round
+                                                  // of a pass is sized from the last pass of the same sampler, whose rate can differ
+                                                  // from the others' many times over
     DevMem<unsigned long long> d_k1_dbg;          // [K1S_MAX_ROUNDS][4] (DSAC_K1_DEBUG=1 or dsac_sampler_profile), else null
     // dsac_sampler_profile: CUDA events between the sampler's launches of the last forward pass
     int k1_profile = 0;
@@ -253,7 +268,7 @@ struct dsac_engine {
         Event ev_filt[K1S_MAX_SETS], ev_solve[K1S_MAX_SETS], ev_gen[K1S_MAX_SETS], ev_round;
         DevMem<int> counters;
         DevMem<unsigned long long> stats;
-        unsigned long long calls[2] = {0, 0};
+        unsigned long long calls[4] = {0, 0, 0, 0};
     } lane1;
     int k1_lanes = 1;                             // DSAC_K1_LANES: 0 = never split a batch into two lanes
     int k1_overlap = 1;
@@ -466,6 +481,8 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
     CUC(cudaFuncSetAttribute(k_sample_cam, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1Smem)));
     CUC(cudaFuncSetAttribute(k_sample_rgbd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1Smem)));
     CUC(cudaFuncSetAttribute(k_sample_rgbd_cam, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1Smem)));
+    for (auto kern : {k_sample_gate, k_sample_cam_gate, k_sample_rgbd_gate, k_sample_rgbd_cam_gate})
+        CUC(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1Smem)));
     // k_refine wants 8 CTAs x 26 KB of shared memory per SM: ask for the carve-out explicitly (the default heuristic
     // need not pick the split the launch bounds were written for).  k_sample is left to the default: it spills to
     // local memory, so it wants the L1 that the largest carve-out would take away (DSAC_K1_CARVEOUT overrides).
@@ -555,8 +572,8 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
             }
             CUC(cudaEventCreateWithFlags(L.ev_round.put(), cudaEventDisableTiming));
             CUC(L.counters.reserve(2 * K1S_MAX_SETS * sizeof(int)));
-            CUC(L.stats.reserve(8 * sizeof(unsigned long long)));
-            CUC(cudaMemset(L.stats, 0, 8 * sizeof(unsigned long long)));
+            CUC(L.stats.reserve(16 * sizeof(unsigned long long)));
+            CUC(cudaMemset(L.stats, 0, 16 * sizeof(unsigned long long)));
             if (const char* ln = getenv("DSAC_K1_LANES")) e->k1_lanes = atoi(ln);
         }
         if (const char* ov = getenv("DSAC_K1_OVERLAP")) { e->k1_overlap = atoi(ov); e->k1_overlap_fixed = true; }
@@ -565,8 +582,8 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
         if (const char* s4 = getenv("DSAC_K1_SOLVE4")) e->k1_solve_group4 = atoi(s4);
         if (const char* sb = getenv("DSAC_K1_SOLVE_BATCH")) e->k1_solve_batch = atoi(sb);
         CUC(cudaFuncSetAttribute(k1_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1XSmem)));
-        CUC(e->d_k1_stats.reserve(8 * sizeof(unsigned long long)));
-        CUC(cudaMemset(e->d_k1_stats, 0, 8 * sizeof(unsigned long long)));
+        CUC(e->d_k1_stats.reserve(16 * sizeof(unsigned long long)));
+        CUC(cudaMemset(e->d_k1_stats, 0, 16 * sizeof(unsigned long long)));
         if (getenv("DSAC_K1_DEBUG")) CUC(e->d_k1_dbg.reserve(K1S_MAX_ROUNDS * 4 * sizeof(unsigned long long)));
         CUC(cudaFuncSetAttribute(k1_filter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1FSmem)));
         CUC(cudaFuncSetAttribute(k1_filter_cam, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1FSmem)));
@@ -660,6 +677,11 @@ static int cameras_begin_pass(dsac_engine* e, int32_t n, cudaStream_t stream) {
     if (e->depth_n && n != e->depth_n)
         return fail(e, DSAC_ERR_ARG, "n_frames %d differs from the %d frames of the cell depth (dsac_set_cell_depth_device)", n, e->depth_n);
     if (e->depth_n) CU(cudaStreamWaitEvent(stream, e->ev_depth, 0));
+    if (e->prior_n && n != e->prior_n)
+        return fail(e, DSAC_ERR_ARG, "n_frames %d differs from the %d frames of the pose priors (dsac_set_pose_priors_device)", n, e->prior_n);
+    if (e->prior_n) CU(cudaStreamWaitEvent(stream, e->ev_prior, 0));
+    e->fwd_prior_gen = e->prior_gen;
+    e->fwd_prior_k = e->prior_n ? e->prior_k : 0;
     e->fwd_cams_gen = e->cams_gen;
     e->fwd_depth_gen = e->depth_gen;
     e->fwd_rgbd = e->depth_n > 0;
@@ -717,6 +739,7 @@ static int sampling_log_prob_run(dsac_engine* e, const char* who, int32_t n, dou
     if (n != e->fwd_g_n) return fail(e, DSAC_ERR_ARG, "%s: n %d differs from the %d frames of the last pass", who, n, e->fwd_g_n);
     if (e->fwd_g_gen != e->g_gen) return fail(e, DSAC_ERR_ARG, "%s: the sampling logits were changed after the last pass", who);
     if (e->fwd_depth_gen != e->depth_gen) return fail(e, DSAC_ERR_ARG, "%s: the cell depth was changed after the last pass", who);
+    if (e->fwd_prior_gen != e->prior_gen) return fail(e, DSAC_ERR_ARG, "%s: the pose priors were changed after the last pass", who);
     if ((!d_logp && !d_grad_logp) || (d_grad_logp && !d_grad)) return fail(e, DSAC_ERR_ARG, "%s: null output", who);
     cudaStream_t stream = (cudaStream_t)stream_v;
     CU(cudaSetDevice(e->cfg.device));
@@ -766,12 +789,53 @@ int dsac_set_cell_depth_device(dsac_engine* e, int32_t n, const float* d_depth, 
     return DSAC_OK;
 }
 
+int dsac_set_pose_priors_device(dsac_engine* e, int32_t n, int32_t k, const double* d_poses, const double* d_info, double gate,
+                                void* stream_v) {
+    if (!e) return DSAC_ERR_ARG;
+    static const char* who = "dsac_set_pose_priors_device";
+    if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "%s: a submitted pass has not been awaited (dsac_forward_wait)", who);
+    if (!d_poses) {
+        if (e->prior_n) e->prior_gen++;
+        e->prior_n = 0;
+        return DSAC_OK;
+    }
+    if (n < 1 || n > e->cfg.max_frames) return fail(e, DSAC_ERR_ARG, "%s: n %d out of range [1,%d]", who, n, e->cfg.max_frames);
+    const int k_max = std::min(e->cfg.n_hyps, DSAC_MAX_PRIORS);
+    if (k < 1 || k > k_max) return fail(e, DSAC_ERR_ARG, "%s: k %d out of range [1,%d]", who, k, k_max);
+    if (d_info && !(std::isfinite(gate) && gate > 0)) return fail(e, DSAC_ERR_ARG, "%s: gate %g must be finite and > 0", who, gate);
+    cudaStream_t stream = (cudaStream_t)stream_v;
+    CU(cudaSetDevice(e->cfg.device));
+    const size_t slots = (size_t)e->cfg.max_frames * DSAC_MAX_PRIORS;
+    CU(e->d_prior_pose.reserve(slots * 6 * sizeof(double)));
+    CU(e->d_prior_info.reserve(slots * 36 * sizeof(double)));
+    CU(e->d_prior_tab.reserve(slots * sizeof(PriorGate)));
+    CU(e->d_prior_bad.reserve((size_t)e->cfg.max_frames * sizeof(uint32_t)));
+    if (!e->ev_prior) CU(cudaEventCreateWithFlags(e->ev_prior.put(), cudaEventDisableTiming));
+    CU(cudaStreamWaitEvent(stream, e->ev_fwd, 0));   // the last forward pass may still read the tables
+    e->prior_n = 0;                                   // (a failed copy leaves no priors in force)
+    e->prior_gen++;
+    const size_t nk = (size_t)n * k;
+    CU(cudaMemcpyAsync(e->d_prior_pose.get(), d_poses, nk * 6 * sizeof(double), cudaMemcpyDeviceToDevice, stream));
+    if (d_info) CU(cudaMemcpyAsync(e->d_prior_info.get(), d_info, nk * 36 * sizeof(double), cudaMemcpyDeviceToDevice, stream));
+    k_prior_prep<<<(unsigned)n, 32, 0, stream>>>(e->d_prior_pose, d_info ? e->d_prior_info.get() : nullptr, k, e->d_prior_tab, e->d_prior_bad);
+    e->launches++;
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(e->ev_prior, stream));
+    e->prior_n = n;
+    e->prior_k = k;
+    e->prior_gate = d_info != nullptr;
+    e->prior_chi2 = d_info ? gate : 0.0;
+    return DSAC_OK;
+}
+
 // A backward pass differentiates the forward before it, which ran with the cameras and the cell depth in force then.
 static int cameras_unchanged(dsac_engine* e, const char* who) {
     if (e->fwd_cams_gen != e->cams_gen)
         return fail(e, DSAC_ERR_ARG, "%s: the cameras were changed (dsac_set_cameras) after the forward pass", who);
     if (e->fwd_depth_gen != e->depth_gen)
         return fail(e, DSAC_ERR_ARG, "%s: the cell depth was changed (dsac_set_cell_depth_device) after the forward pass", who);
+    if (e->fwd_prior_gen != e->prior_gen)
+        return fail(e, DSAC_ERR_ARG, "%s: the pose priors were changed (dsac_set_pose_priors_device) after the forward pass", who);
     return DSAC_OK;
 }
 
@@ -877,6 +941,10 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
     const GuidedGen gg{guided ? e->d_g_cum + o * DSAC_N : nullptr, guided ? e->d_g_bad + o : nullptr};
     const bool rgbd = e->depth_n > 0;                         // RGB-D pass: this range's frames of the eye coordinates
     const double* eye = rgbd ? e->d_eye + o * Nn * 3 : nullptr;
+    // pose priors: the streams draw n_hyps - prior_k hypotheses into the first slots of each frame, k_prior_inject fills the rest
+    const int prior_k = e->prior_n ? e->prior_k : 0;
+    const bool gate = prior_k > 0 && e->prior_gate;
+    const int draw_h = c.n_hyps - prior_k;
 
     if (e->stages & DSAC_STAGE_SAMPLE) {
         CU(cudaMemsetAsync(e->d_status + o, 0, (size_t)n * sizeof(uint32_t), stream));
@@ -891,7 +959,7 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
         SampleParams sp;
         sp.coords = d_coords; sp.pix = d_pix; sp.pix_stride = pix_shared ? 0 : DSAC_N * 2;
         sp.f = c.focal; sp.cx = c.cx; sp.cy = c.cy; sp.cams = cams;
-        sp.H = c.n_hyps; sp.T = c.n_streams; sp.thr = c.thr2d;
+        sp.H = draw_h; sp.Hs = c.n_hyps; sp.T = c.n_streams; sp.thr = c.thr2d;
         sp.seed = c.seed; sp.skip = c.stream_skip; sp.max_candidates = c.max_candidates;
         sp.frame0 = frame0;
         sp.hyp_pose = e->d_hyp_pose + o * Hh * 6; sp.hyp_P = e->d_hyp_P + o * Hh * 12; sp.img_idx = e->d_img_idx + o * Hh * 4; sp.cand_idx = e->d_cand_idx + o * Hh;
@@ -900,11 +968,23 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
         { const char* g = getenv("DSAC_K1_A2_GENERIC"); sp.a2_generic = (g && g[0] == '1') ? 1 : 0; }
         sp.resume = nullptr;
         sp.eye = eye; sp.skip_frame = rgbd ? e->d_rgbd_skip + o : nullptr;
+        sp.prior_tab = gate ? e->d_prior_tab + o * prior_k : nullptr; sp.prior_bad = gate ? e->d_prior_bad + o : nullptr;
+        sp.prior_k = gate ? prior_k : 0; sp.prior_chi2 = gate ? e->prior_chi2 : 0.0;
+        // the monolithic sampler: the whole pass, or the resume tail of the split sampler's rounds
+        auto launch_sample = [&](const SampleParams& s) {
+            const dim3 g(c.n_streams, n);
+            const size_t sm = sizeof(K1Smem);
+            if (gate && rgbd && cams) k_sample_rgbd_cam_gate<<<g, K1_THREADS, sm, stream>>>(s);
+            else if (gate && rgbd) k_sample_rgbd_gate<<<g, K1_THREADS, sm, stream>>>(s);
+            else if (gate && cams) k_sample_cam_gate<<<g, K1_THREADS, sm, stream>>>(s);
+            else if (gate) k_sample_gate<<<g, K1_THREADS, sm, stream>>>(s);
+            else if (rgbd && cams) k_sample_rgbd_cam<<<g, K1_THREADS, sm, stream>>>(s);
+            else if (rgbd) k_sample_rgbd<<<g, K1_THREADS, sm, stream>>>(s);
+            else if (cams) k_sample_cam<<<g, K1_THREADS, sm, stream>>>(s);
+            else k_sample<<<g, K1_THREADS, sm, stream>>>(s);
+        };
         if (!e->k1_mode) {
-            if (rgbd && cams) k_sample_rgbd_cam<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
-            else if (rgbd) k_sample_rgbd<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
-            else if (cams) k_sample_cam<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
-            else k_sample<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
+            launch_sample(sp);
             e->launches++;
             CU(cudaGetLastError());
         } else {
@@ -917,8 +997,9 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             const Event* k_ev_gen = lane ? e->lane1.ev_gen : e->k1_ev_gen;
             cudaEvent_t k_ev_round = lane ? e->lane1.ev_round : e->k1_ev_round;
             int* k_counters = lane ? e->lane1.counters : e->d_k1_counters;
-            unsigned long long* k_stats = (lane ? e->lane1.stats : e->d_k1_stats) + (guided ? 4 : 0);
-            unsigned long long& k_calls = (lane ? e->lane1.calls : e->k1_calls)[guided ? 1 : 0];
+            const int sampler = (gate ? 2 : 0) + (guided ? 1 : 0);   // statistics block: uniform, guided, gated uniform, gated guided
+            unsigned long long* k_stats = (lane ? e->lane1.stats : e->d_k1_stats) + 4 * sampler;
+            unsigned long long& k_calls = (lane ? e->lane1.calls : e->k1_calls)[sampler];
             K1SplitParams q;
             q.sp = sp;
             q.state = e->d_k1_state + o * T; q.celltab = e->d_k1_celltab + o * Nn;
@@ -1011,7 +1092,7 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             if (few) q.first_frac = 1.15;
             // speculative first round (k1_spec / k1_stitch): one stream generated window by window on many SMs; pays when a
             // stream's first round is several windows long (>= 64 hypotheses per stream) and the GPU is otherwise idle
-            const int quota_max = (c.n_hyps + c.n_streams - 1) / c.n_streams;
+            const int quota_max = (draw_h + c.n_streams - 1) / c.n_streams;
             const bool use_spec = few && off == 0 && n_slots <= e->k1_spec_slots && quota_max >= 64 && c.max_candidates >= (1 << 16) && !fused_req && !guided && !rgbd;   // (the candidate bound cannot fall inside the speculative round)
             // chained generator (k1_pipe): K CTAs per stream, all of them resident at once
             const int pipe_K = (int)std::min<long long>(8, e->k1_slot_capacity / std::max<long long>(1, n_slots));
@@ -1045,7 +1126,8 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
                             k1_filter<<<fgrid, K1F_THREADS, sizeof(K1FSmem), stream>>>(qf);
                         }
                         mark(1);
-                        k1_solve<<<e->k1_solve_grid, K1V_THREADS, 0, stream>>>(qf);
+                        if (gate) k1_solve_gate<<<e->k1_solve_grid, K1V_THREADS, 0, stream>>>(qf);
+                        else k1_solve<<<e->k1_solve_grid, K1V_THREADS, 0, stream>>>(qf);
                         mark(2);
                         e->launches += 2;
                     }
@@ -1085,7 +1167,9 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
                         if (!batch && solve_side != side && set >= 2) CU(cudaStreamWaitEvent(side, k_ev_solve[set - 2], 0));   // the flag-queue region is free again
                     }
                     if (rgbd) {   // the acceptance test writes the accept bits itself: no flag queue, no solve
-                        if (cams) k1_kabsch_cam<<<fgrid, K1F_THREADS, 0, side>>>(q);
+                        if (gate && cams) k1_kabsch_cam_gate<<<fgrid, K1F_THREADS, 0, side>>>(q);
+                        else if (gate) k1_kabsch_gate<<<fgrid, K1F_THREADS, 0, side>>>(q);
+                        else if (cams) k1_kabsch_cam<<<fgrid, K1F_THREADS, 0, side>>>(q);
                         else k1_kabsch<<<fgrid, K1F_THREADS, 0, side>>>(q);
                         if (!overlap) mark(1);
                         e->launches += 2;
@@ -1101,7 +1185,11 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
                         CU(cudaStreamWaitEvent(solve_side, k_ev_filt[set], 0));
                     }
                     const bool group4 = few && e->k1_solve_group4;
-                    if (cams && group4) k1_solve4_cam<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
+                    if (gate && cams && group4) k1_solve4_cam_gate<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
+                    else if (gate && cams) k1_solve_cam_gate<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
+                    else if (gate && group4) k1_solve4_gate<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
+                    else if (gate) k1_solve_gate<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
+                    else if (cams && group4) k1_solve4_cam<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
                     else if (cams) k1_solve_cam<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
                     else if (group4) k1_solve4<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
                     else k1_solve<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
@@ -1116,20 +1204,32 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             launch_slot(q);
             mark(0);
             sp.resume = q.state;   // streams the rounds left unfinished (normally none) continue in the monolithic kernel
-            if (rgbd && guided && cams) k1_gtail_rgbd_cam<<<dim3(c.n_streams, n), KG_THREADS, 0, stream>>>(q, gg);
-            else if (rgbd && guided) k1_gtail_rgbd<<<dim3(c.n_streams, n), KG_THREADS, 0, stream>>>(q, gg);
-            else if (rgbd && cams) k_sample_rgbd_cam<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
-            else if (rgbd) k_sample_rgbd<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
-            else if (guided && cams) k1_gtail_cam<<<dim3(c.n_streams, n), KG_THREADS, 0, stream>>>(q, gg);   // ... or in guided steps
-            else if (guided) k1_gtail<<<dim3(c.n_streams, n), KG_THREADS, 0, stream>>>(q, gg);
-            else if (cams) k_sample_cam<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
-            else k_sample<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(sp);
+            const dim3 gt(c.n_streams, n);   // ... or in guided steps
+            if (gate && guided && rgbd && cams) k1_gtail_rgbd_cam_gate<<<gt, KG_THREADS, 0, stream>>>(q, gg);
+            else if (gate && guided && rgbd) k1_gtail_rgbd_gate<<<gt, KG_THREADS, 0, stream>>>(q, gg);
+            else if (gate && guided && cams) k1_gtail_cam_gate<<<gt, KG_THREADS, 0, stream>>>(q, gg);
+            else if (gate && guided) k1_gtail_gate<<<gt, KG_THREADS, 0, stream>>>(q, gg);
+            else if (rgbd && guided && cams) k1_gtail_rgbd_cam<<<gt, KG_THREADS, 0, stream>>>(q, gg);
+            else if (rgbd && guided) k1_gtail_rgbd<<<gt, KG_THREADS, 0, stream>>>(q, gg);
+            else if (guided && cams) k1_gtail_cam<<<gt, KG_THREADS, 0, stream>>>(q, gg);
+            else if (guided) k1_gtail<<<gt, KG_THREADS, 0, stream>>>(q, gg);
+            else launch_sample(sp);
             mark(3);
             e->launches += 2;
             if (cams) {   // the generator's selection wrote hyp_P with the config's focal length
                 k1_focal_rows_cam<<<(unsigned)(((size_t)n * c.n_hyps + 255) / 256), 256, 0, stream>>>(sp, n);
                 e->launches++;
             }
+            CU(cudaGetLastError());
+        }
+        if (prior_k) {   // the prior slots behind the sampled ones, or the empty frames of a bad setting
+            PriorInjectParams ip;
+            ip.poses = e->d_prior_pose + o * prior_k * 6; ip.bad = e->d_prior_bad + o;
+            ip.k = prior_k; ip.H = c.n_hyps; ip.T = c.n_streams; ip.skip = c.stream_skip; ip.f = c.focal; ip.cams = cams;
+            ip.hyp_pose = sp.hyp_pose; ip.hyp_P = sp.hyp_P; ip.img_idx = sp.img_idx; ip.cand_idx = sp.cand_idx;
+            ip.stream_ncand = sp.stream_ncand; ip.stream_endpos = sp.stream_endpos; ip.status = sp.status;
+            k_prior_inject<<<(unsigned)n, 128, 0, stream>>>(ip);
+            e->launches++;
             CU(cudaGetLastError());
         }
     }

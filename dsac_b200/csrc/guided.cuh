@@ -85,7 +85,8 @@ __global__ void __launch_bounds__(KG_THREADS) k_guided_table(const float* logits
 // quota or max_candidates candidates.  An exhausted stream gets the uniform path's empty hypotheses.  Normally no stream
 // is left: the kernel then returns after one look at the state.
 // RGBD: the candidates are accepted by rgbd_accept instead.
-template <bool PER_FRAME, bool RGBD = false>
+// GATE: behind the pose priors' covariance gate (prior_gate_ok), as the rounds' acceptance.
+template <bool PER_FRAME, bool RGBD = false, bool GATE = false>
 __global__ void __launch_bounds__(KG_THREADS) k1_gtail_t(K1SplitParams q, GuidedGen gg) {
     __shared__ uint32_t cum[DSAC_N_CONST];
     __shared__ int warp[2][KG_THREADS / 32];
@@ -142,11 +143,12 @@ __global__ void __launch_bounds__(KG_THREADS) k1_gtail_t(K1SplitParams q, Guided
                 if (fragile) atomicAdd(p.n_fragile, 1ull);
             }
         }
+        if constexpr (GATE) ok = ok && prior_gate_ok<GATE>(p, frame, rvec, tvec);
         int tot;
         const int rank = acc + block_excl_scan<KG_THREADS / 32>(ok ? 1 : 0, &tot, warp[par]);
         par ^= 1;
         if (ok && rank < quota) {
-            k1_write_hyp(p, (size_t)frame * p.H + h0 + rank, rvec, tvec, cells, ci);
+            k1_write_hyp(p, (size_t)frame * p.Hs + h0 + rank, rvec, tvec, cells, ci);
             if (rank == quota - 1) {
                 p.stream_ncand[slot] = ci + 1;
                 p.stream_endpos[slot] = pos0;
@@ -168,6 +170,10 @@ constexpr auto k1_gtail = k1_gtail_t<false>;
 constexpr auto k1_gtail_cam = k1_gtail_t<true>;
 constexpr auto k1_gtail_rgbd = k1_gtail_t<false, true>;
 constexpr auto k1_gtail_rgbd_cam = k1_gtail_t<true, true>;
+constexpr auto k1_gtail_gate = k1_gtail_t<false, false, true>;
+constexpr auto k1_gtail_cam_gate = k1_gtail_t<true, false, true>;
+constexpr auto k1_gtail_rgbd_gate = k1_gtail_t<false, true, true>;
+constexpr auto k1_gtail_rgbd_cam_gate = k1_gtail_t<true, true, true>;
 
 struct GuidedLogpParams {
     const double* w;                 // [n][N] softmax of the logits

@@ -13,6 +13,7 @@
 
 #include "camera.cuh"
 #include "pose_math.cuh"
+#include "prior.cuh"
 #include "rigid.cuh"
 #include "sampler.cuh"
 
@@ -118,7 +119,8 @@ struct SampleParams {
     int pix_stride;          // N*2 or 0 (shared grid)
     double f, cx, cy;
     const Cam* cams;         // [n] or null: the camera of every frame is f, cx, cy
-    int H, T, thr;
+    int H, T, thr;           // H: hypotheses the streams draw (quotas stream_chunk(H, T, s))
+    int Hs;                  // hypothesis slots per frame of the outputs: H, plus the pose priors' slots behind them
     uint32_t seed, skip;
     int max_candidates;
     long long frame0;
@@ -136,7 +138,20 @@ struct SampleParams {
     // RGB-D passes (dsac_set_cell_depth_device, rigid.cuh): minimal sets are accepted by rgbd_accept
     const double* eye;                 // [n][N][3] eye coordinates (mm), NaN without depth
     const uint32_t* skip_frame;        // [n] status bits of a frame that samples nothing (DSAC_ST_NO_DEPTH), else 0
+    // the covariance gate of the pose priors (prior.cuh), read by the GATE instantiations only
+    const PriorGate* prior_tab;        // [n][prior_k]
+    const uint32_t* prior_bad;         // [n] DSAC_ST_BAD_PRIOR: the frame's hypotheses are discarded, every candidate passes
+    int prior_k;
+    double prior_chi2;
 };
+
+// The gate at an acceptance site: an accepted candidate's pose must lie within chi2 of one of the frame's priors.
+template <bool GATE>
+__device__ __forceinline__ bool prior_gate_ok(const SampleParams& p, int frame, const double rvec[3], const double tvec[3]) {
+    if constexpr (!GATE) return true;
+    if (p.prior_bad[frame]) return true;
+    return prior_gate_pass(p.prior_tab + (size_t)frame * p.prior_k, p.prior_k, p.prior_chi2, rvec, tvec);
+}
 
 #ifndef K1_THREADS_DEF
 #define K1_THREADS_DEF 384
@@ -242,7 +257,8 @@ __device__ __forceinline__ int cand_parse_fast(const unsigned char* vals, int q,
 //   D  full solve + reprojection check on the queue, ordered compaction of the accepted
 // PER_FRAME: the camera of the CTA's frame comes from the per-frame table (SampleParams::cams) in place of p.f, p.cx, p.cy.
 // RGBD: every candidate goes to phase D, where one lane per candidate runs rgbd_accept in place of the four P3P lanes.
-template <bool PER_FRAME, bool RGBD = false>
+// GATE: an accepted candidate must also pass the pose priors' covariance gate (prior_gate_ok).
+template <bool PER_FRAME, bool RGBD = false, bool GATE = false>
 __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS) k_sample_t(SampleParams p) {
     if constexpr (PER_FRAME) {
         const Cam c = p.cams[blockIdx.y];
@@ -268,7 +284,7 @@ __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS) k_sample_t(SamplePa
     if constexpr (RGBD) {
         if (const uint32_t bits = p.skip_frame[frame]) {   // DSAC_ST_NO_DEPTH: nothing is sampled, the hypotheses of an exhausted stream
             for (int r = tid; r < quota; r += K1_THREADS) {
-                const size_t hi = (size_t)frame * p.H + h0 + r;
+                const size_t hi = (size_t)frame * p.Hs + h0 + r;
                 for (int k = 0; k < 6; k++) p.hyp_pose[hi * 6 + k] = 0.0;
                 float4* P = reinterpret_cast<float4*>(p.hyp_P + hi * 12);
                 P[0] = make_float4((float)p.f, 0.f, 0.f, 0.f);
@@ -635,11 +651,12 @@ __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS) k_sample_t(SamplePa
             if (nsol > 0 && bl == sub)
                 ok = minimal_set_accept(obj, img, p.f, p.cx, p.cy, p.thr, R, t, e2, rvec, tvec, &fragile);
             }
+            if constexpr (GATE) ok = ok && prior_gate_ok<GATE>(p, frame, rvec, tvec);
             if (fragile) atomicAdd(p.n_fragile, 1ull);
             int tot;
             int rank = acc + block_excl_scan<K1_WARPS>(ok ? 1 : 0, &tot, sm.warp[par]);
             if (ok && rank < quota) {
-                size_t hi = (size_t)frame * p.H + h0 + rank;
+                size_t hi = (size_t)frame * p.Hs + h0 + rank;
                 double* hp = p.hyp_pose + hi * 6;
                 hp[0] = rvec[0]; hp[1] = rvec[1]; hp[2] = rvec[2];
                 hp[3] = tvec[0]; hp[4] = tvec[1]; hp[5] = tvec[2];
@@ -706,7 +723,7 @@ __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS) k_sample_t(SamplePa
 
     if (acc < quota) {  // sampler exhausted: value-encode like a failed PnP (zero pose, cnn_softam.h:66-71)
         for (int r = acc + tid; r < quota; r += K1_THREADS) {
-            size_t hi = (size_t)frame * p.H + h0 + r;
+            size_t hi = (size_t)frame * p.Hs + h0 + r;
             for (int k = 0; k < 6; k++) p.hyp_pose[hi * 6 + k] = 0.0;
             float4* P = reinterpret_cast<float4*>(p.hyp_P + hi * 12);
             P[0] = make_float4((float)p.f, 0.f, 0.f, 0.f);
@@ -727,6 +744,10 @@ constexpr auto k_sample = k_sample_t<false>;
 constexpr auto k_sample_cam = k_sample_t<true>;
 constexpr auto k_sample_rgbd = k_sample_t<false, true>;
 constexpr auto k_sample_rgbd_cam = k_sample_t<true, true>;
+constexpr auto k_sample_gate = k_sample_t<false, false, true>;
+constexpr auto k_sample_cam_gate = k_sample_t<true, false, true>;
+constexpr auto k_sample_rgbd_gate = k_sample_t<false, true, true>;
+constexpr auto k_sample_rgbd_cam_gate = k_sample_t<true, true, true>;
 
 // ------------------------------------------------------------------ K2: fused scoring
 struct ScoreParams {

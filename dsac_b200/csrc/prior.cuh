@@ -1,0 +1,186 @@
+// prior.cuh -- pose priors (dsac_set_pose_priors_device): caller poses that take the last k hypothesis slots of a frame, and
+// the optional covariance gate on the sampled hypotheses.
+//
+//   PriorGate        one prior as the gate reads it: its rotation, translation and the Cholesky factor of its information
+//   prior_cholesky   the factor from the lower triangle of a 6x6 information matrix, with the refusal of DSAC_ST_BAD_PRIOR
+//   so3_log          the principal log of a rotation, accurate up to and at pi
+//   prior_d2         xi^T Lambda xi of a pose against one prior, xi = (log(R_h R_j^T), t_h - t_j)
+//   k_prior_prep     once per setting: validates every prior of a frame, writes the gate table and the frame's bad flag
+//   k_prior_inject   once per pass, after the sampler: the prior slots, or the empty frame of a bad setting
+//
+// The math compiles for the host as well (DSAC_HOST_ONLY): tests/host_shim/prior_shim.cpp checks it against scipy.
+#pragma once
+#include <math.h>
+#include <stdint.h>
+
+#include "pose_math.cuh"
+
+namespace dsac {
+
+constexpr int PRIOR_MAX = 16;                 // DSAC_MAX_PRIORS
+constexpr uint32_t PRIOR_ST_BAD = 128u;       // DSAC_ST_BAD_PRIOR
+constexpr double PRIOR_PIVOT_REL = 1e-12;     // a Cholesky pivot below this fraction of its diagonal entry is refused
+
+struct PriorGate {
+    double R[9];    // rotation of the prior (row-major, from its rvec)
+    double t[3];    // translation (mm)
+    double L[21];   // lower Cholesky factor of the information, by rows: L(i, j) = L[i (i + 1) / 2 + j], j <= i
+};
+
+// Lambda = L L^T from the lower triangle of info (row-major 6x6; entries above the diagonal are not read).  False when an
+// entry is not finite, a diagonal entry is not > 0, or a pivot falls below PRIOR_PIVOT_REL of its diagonal entry
+// (singular or indefinite).
+DSAC_HD bool prior_cholesky(const double* info, double L[21]) {
+    for (int i = 0; i < 6; i++) {
+        for (int j = 0; j <= i; j++) {
+            double s = info[i * 6 + j];
+            if (!isfinite(s)) return false;
+            for (int k = 0; k < j; k++) s -= L[i * (i + 1) / 2 + k] * L[j * (j + 1) / 2 + k];
+            if (i == j) {
+                const double a = info[i * 6 + i];
+                if (!(a > 0) || !(s > PRIOR_PIVOT_REL * a)) return false;
+                L[i * (i + 1) / 2 + i] = sqrt(s);
+            } else {
+                L[i * (i + 1) / 2 + j] = s / L[j * (j + 1) / 2 + j];
+            }
+        }
+    }
+    return true;
+}
+
+// w = log(M), |w| <= pi, for a rotation M (row-major).  The angle comes from atan2(|skew|, (tr - 1) / 2), accurate everywhere;
+// the axis from the skew part below pi / 2 and from the symmetric part M + M^T = 2 c I + 2 (1 - c) n n^T above, where the
+// skew part vanishes (its sign picks n against -n; at exactly pi both are the principal log).
+DSAC_HD void so3_log(const double M[9], double w[3]) {
+    const double v[3] = {0.5 * (M[7] - M[5]), 0.5 * (M[2] - M[6]), 0.5 * (M[3] - M[1])};   // sin(th) n
+    const double s = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+    const double c = 0.5 * (M[0] + M[4] + M[8] - 1.0);
+    const double th = atan2(s, c);
+    if (c > 0) {
+        const double k = s > 0 ? th / s : 1.0;
+        for (int i = 0; i < 3; i++) w[i] = k * v[i];
+        return;
+    }
+    int i = 0;
+    for (int j = 1; j < 3; j++)
+        if (M[j * 4] > M[i * 4]) i = j;
+    const double bii = M[i * 4] - c;   // (1 - c) n_i^2, the largest of the three
+    const double sc = 1.0 / sqrt(bii * (1.0 - c));
+    double n[3];
+    for (int j = 0; j < 3; j++) n[j] = (j == i ? bii : 0.5 * (M[i * 3 + j] + M[j * 3 + i])) * sc;
+    const double sg = (n[0] * v[0] + n[1] * v[1] + n[2] * v[2]) < 0 ? -th : th;
+    for (int j = 0; j < 3; j++) w[j] = sg * n[j];
+}
+
+// d^2 = xi^T Lambda xi = |L^T xi|^2 of the pose (Rh, th) against prior g, xi = (log(Rh Rj^T) rad, th - tj mm), fp64.
+DSAC_HD double prior_d2(const double Rh[9], const double th[3], const PriorGate& g) {
+    double M[9];
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) M[i * 3 + j] = Rh[i * 3] * g.R[j * 3] + Rh[i * 3 + 1] * g.R[j * 3 + 1] + Rh[i * 3 + 2] * g.R[j * 3 + 2];
+    double xi[6];
+    so3_log(M, xi);
+    for (int i = 0; i < 3; i++) xi[3 + i] = th[i] - g.t[i];
+    double d2 = 0;
+    for (int j = 0; j < 6; j++) {
+        double y = 0;
+        for (int i = j; i < 6; i++) y += g.L[i * (i + 1) / 2 + j] * xi[i];
+        d2 += y * y;
+    }
+    return d2;
+}
+
+// The gate: the cv pose (rvec, tvec) passes iff min_j d^2_j <= chi2 over the frame's k priors.
+DSAC_HD bool prior_gate_pass(const PriorGate* tab, int k, double chi2, const double rvec[3], const double tvec[3]) {
+    double R[9];
+    rodrigues_v2m(rvec, R);
+    for (int j = 0; j < k; j++)
+        if (prior_d2(R, tvec, tab[j]) <= chi2) return true;
+    return false;
+}
+
+// One prior's gate entry from its cv pose and (nullable) information; false: DSAC_ST_BAD_PRIOR.
+DSAC_HD bool prior_entry(const double pose[6], const double* info, PriorGate& g) {
+    bool ok = true;
+    for (int m = 0; m < 6; m++) ok = ok && isfinite(pose[m]);
+    const double zero[6] = {0, 0, 0, 0, 0, 0};
+    const double* po = ok ? pose : zero;
+    rodrigues_v2m(po, g.R);
+    for (int m = 0; m < 3; m++) g.t[m] = po[3 + m];
+    for (int m = 0; m < 21; m++) g.L[m] = 0;
+    if (info) ok = prior_cholesky(info, g.L) && ok;
+    return ok;
+}
+
+#if defined(__CUDACC__) && !defined(DSAC_HOST_ONLY)
+}  // namespace dsac
+#include "camera.cuh"
+namespace dsac {
+
+// One warp per frame, lane j < k for prior j: the gate table [n][k] and bad [n] (0 or DSAC_ST_BAD_PRIOR).
+__global__ void __launch_bounds__(32) k_prior_prep(const double* __restrict__ poses, const double* __restrict__ info, int k,
+                                                   PriorGate* __restrict__ tab, uint32_t* __restrict__ bad) {
+    const int f = blockIdx.x, j = threadIdx.x;
+    bool ok = true;
+    if (j < k) {
+        const size_t i = (size_t)f * k + j;
+        PriorGate g;
+        ok = prior_entry(poses + i * 6, info ? info + i * 36 : nullptr, g);
+        tab[i] = g;
+    }
+    const unsigned any_bad = __ballot_sync(0xffffffffu, !ok);
+    if (j == 0) bad[f] = any_bad ? PRIOR_ST_BAD : 0u;
+}
+
+struct PriorInjectParams {
+    const double* poses;       // [n][k][6]
+    const uint32_t* bad;       // [n]
+    int k, H, T;               // priors per frame, hypothesis slots per frame, sampler streams
+    uint32_t skip;             // stream_skip: where stream 0 stands after a frame that sampled nothing
+    double f;                  // the config's focal length
+    const Cam* cams;           // [n] or null
+    double* hyp_pose;          // [n][H][6]
+    float* hyp_P;              // [n][H][12]
+    int32_t* img_idx;          // [n][H][4]
+    int32_t* cand_idx;         // [n][H]
+    long long* stream_ncand;   // [n][T]
+    unsigned long long* stream_endpos;   // [n][T]
+    uint32_t* status;          // [n]
+};
+
+// One CTA per frame, after the sampler.  Prior j goes to slot H - k + j: its pose bits, hyp_P as the sampler writes it
+// (k1_write_hyp, with the frame's focal length), img_idx and cand_idx -1.  A bad frame instead gets the empty hypotheses
+// of an exhausted stream in all H slots, no candidates, stream 0 right after stream_skip, and DSAC_ST_BAD_PRIOR in place
+// of DSAC_ST_SAMPLER_EXHAUSTED, as if it had sampled nothing.  With k == H nothing was sampled either: stream 0 stands right
+// after stream_skip, where the DSAC variant's draw continues it.
+__global__ void __launch_bounds__(128) k_prior_inject(PriorInjectParams p) {
+    const int f = blockIdx.x, tid = threadIdx.x;
+    const double fc = p.cams ? p.cams[f].f : p.f;
+    const bool bad = p.bad[f] != 0;
+    const int h0 = bad ? 0 : p.H - p.k;
+    for (int h = h0 + tid; h < p.H; h += blockDim.x) {
+        const size_t hi = (size_t)f * p.H + h;
+        double po[6] = {0, 0, 0, 0, 0, 0};
+        if (!bad)
+            for (int m = 0; m < 6; m++) po[m] = p.poses[((size_t)f * p.k + (h - h0)) * 6 + m];
+        for (int m = 0; m < 6; m++) p.hyp_pose[hi * 6 + m] = po[m];
+        double Rm[9];
+        rodrigues_v2m(po, Rm);
+        float4* P = reinterpret_cast<float4*>(p.hyp_P + hi * 12);
+        P[0] = make_float4((float)(fc * Rm[0]), (float)(fc * Rm[1]), (float)(fc * Rm[2]), (float)(fc * po[3]));
+        P[1] = make_float4((float)(fc * Rm[3]), (float)(fc * Rm[4]), (float)(fc * Rm[5]), (float)(fc * po[4]));
+        P[2] = make_float4((float)Rm[6], (float)Rm[7], (float)Rm[8], (float)po[5]);
+        *reinterpret_cast<int4*>(p.img_idx + hi * 4) = make_int4(-1, -1, -1, -1);
+        p.cand_idx[hi] = -1;
+    }
+    if (!bad && p.k < p.H) return;
+    // nothing sampled (a bad frame, or k == H: every stream had a quota of 0)
+    for (int s = tid; s < p.T; s += blockDim.x) {
+        p.stream_ncand[(size_t)f * p.T + s] = 0;
+        p.stream_endpos[(size_t)f * p.T + s] = (s == 0) ? p.skip : 0u;
+    }
+    if (tid == 0 && bad) p.status[f] = (p.status[f] & ~1u) | PRIOR_ST_BAD;
+}
+
+#endif
+
+}  // namespace dsac

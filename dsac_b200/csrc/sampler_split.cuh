@@ -53,7 +53,7 @@ __device__ __forceinline__ void k1_write_hyp(const SampleParams& p, size_t hi, c
 // Hypotheses [h, h + count) of `frame` as an exhausted stream leaves them (zero pose, k_sample's value encoding).
 __device__ __forceinline__ void k1_empty_hyps(const SampleParams& p, int frame, int h, int count, int tid, int nt) {
     for (int r = tid; r < count; r += nt) {
-        const size_t hi = (size_t)frame * p.H + h + r;
+        const size_t hi = (size_t)frame * p.Hs + h + r;
         for (int k = 0; k < 6; k++) p.hyp_pose[hi * 6 + k] = 0.0;
         float4* P = reinterpret_cast<float4*>(p.hyp_P + hi * 12);
         P[0] = make_float4((float)p.f, 0.f, 0.f, 0.f);
@@ -338,7 +338,7 @@ __device__ __forceinline__ void k1_slot_body(const K1SplitParams& q, K1GSmemT<NT
         const int n_emit = min(tot, room);
         for (int k = tid; k < n_emit; k += NT) {
             const int i = sm.acc_list[k];
-            const size_t hi = (size_t)frame * p.H + h0 + acc + k;
+            const size_t hi = (size_t)frame * p.Hs + h0 + acc + k;
             const double* po = q.pose_out + (cbase + i) * 6;
             const double rvec[3] = {po[0], po[1], po[2]}, tvec[3] = {po[3], po[4], po[5]};
             const uint2 cc = q.cells[cbase + i];
@@ -1482,7 +1482,7 @@ __global__ void __launch_bounds__(K1X_THREADS, 1) k1_fused(K1SplitParams qf, K1S
 #ifndef K1V_MIN_BLOCKS
 #define K1V_MIN_BLOCKS 4
 #endif
-template <int GROUP, bool PER_FRAME = false>
+template <int GROUP, bool PER_FRAME = false, bool GATE = false>
 __device__ __forceinline__ void k1_solve_body(const K1SplitParams& q) {
     const SampleParams& p = q.sp;
     const int tid = threadIdx.x;
@@ -1534,6 +1534,7 @@ __device__ __forceinline__ void k1_solve_body(const K1SplitParams& q) {
         }
         if (nsol > 0 && bl == sub)
             ok = minimal_set_accept(obj, img, cam.f, cam.cx, cam.cy, p.thr, R, t, e2, rvec, tvec, &fragile);
+        if constexpr (GATE) ok = ok && prior_gate_ok<GATE>(p, slot / p.T, rvec, tvec);
         if (fragile) atomicAdd(p.n_fragile, 1ull);
         if (ok) {
             double* po = q.pose_out + ((size_t)slot * q.cap + ci) * 6;
@@ -1552,12 +1553,17 @@ __global__ void __launch_bounds__(K1V_THREADS, K1V_MIN_BLOCKS) k1_solve4(K1Split
 // the same with the per-frame camera table (SampleParams::cams)
 __global__ void __launch_bounds__(K1V_THREADS, K1V_MIN_BLOCKS) k1_solve_cam(K1SplitParams q) { k1_solve_body<K1V_GROUP, true>(q); }
 __global__ void __launch_bounds__(K1V_THREADS, K1V_MIN_BLOCKS) k1_solve4_cam(K1SplitParams q) { k1_solve_body<4, true>(q); }
+// the same behind the pose priors' covariance gate
+__global__ void __launch_bounds__(K1V_THREADS, K1V_MIN_BLOCKS) k1_solve_gate(K1SplitParams q) { k1_solve_body<K1V_GROUP, false, true>(q); }
+__global__ void __launch_bounds__(K1V_THREADS, K1V_MIN_BLOCKS) k1_solve4_gate(K1SplitParams q) { k1_solve_body<4, false, true>(q); }
+__global__ void __launch_bounds__(K1V_THREADS, K1V_MIN_BLOCKS) k1_solve_cam_gate(K1SplitParams q) { k1_solve_body<K1V_GROUP, true, true>(q); }
+__global__ void __launch_bounds__(K1V_THREADS, K1V_MIN_BLOCKS) k1_solve4_cam_gate(K1SplitParams q) { k1_solve_body<4, true, true>(q); }
 
 // ------------------------------------------------------------------ k1_kabsch
 // RGB-D passes: the rounds' acceptance test in place of k1_filter + k1_solve.  It consumes the launch set's work items and
 // writes the accept bits and pose_out that k1_slot's selection reads, one thread per candidate: rgbd_accept is a few
 // hundred fp64 operations, so there is no cheap screen worth a queue of its own.
-template <bool PER_FRAME>
+template <bool PER_FRAME, bool GATE = false>
 __global__ void __launch_bounds__(K1F_THREADS) k1_kabsch_t(K1SplitParams q) {
     const SampleParams& p = q.sp;
     const int n_items = q.wq_n[q.qidx];
@@ -1576,7 +1582,8 @@ __global__ void __launch_bounds__(K1F_THREADS) k1_kabsch_t(K1SplitParams q) {
             const int cells[4] = {(int)(c.x & 0xffffu), (int)(c.x >> 16), (int)(c.y & 0xffffu), (int)(c.y >> 16)};
             double rvec[3], tvec[3];
             bool fragile = false;
-            const bool ok = rgbd_accept_cells(coords, eye, pix, cells, cam.f, cam.cx, cam.cy, p.thr, rvec, tvec, &fragile);
+            bool ok = rgbd_accept_cells(coords, eye, pix, cells, cam.f, cam.cx, cam.cy, p.thr, rvec, tvec, &fragile);
+            if constexpr (GATE) ok = ok && prior_gate_ok<GATE>(p, frame, rvec, tvec);
             if (fragile) atomicAdd(p.n_fragile, 1ull);
             if (ok) {
                 double* po = q.pose_out + ((size_t)slot * q.cap + ci) * 6;
@@ -1589,14 +1596,16 @@ __global__ void __launch_bounds__(K1F_THREADS) k1_kabsch_t(K1SplitParams q) {
 }
 constexpr auto k1_kabsch = k1_kabsch_t<false>;
 constexpr auto k1_kabsch_cam = k1_kabsch_t<true>;
+constexpr auto k1_kabsch_gate = k1_kabsch_t<false, true>;
+constexpr auto k1_kabsch_cam_gate = k1_kabsch_t<true, true>;
 
 // The generator is camera-free: the selection of k1_slot writes the rows (fR0 ft0), (fR1 ft1) of hyp_P with the engine's
 // focal length.  With a per-frame camera table this kernel, launched after the sampler, writes them again from the
 // hypothesis pose with the frame's own focal length, in the selection's arithmetic.  One thread per (frame, hypothesis).
 __global__ void __launch_bounds__(256) k1_focal_rows_cam(SampleParams p, int n_frames) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_frames * p.H) return;
-    const double f = p.cams[i / p.H].f;
+    if (i >= n_frames * p.Hs) return;
+    const double f = p.cams[i / p.Hs].f;
     const double* hp = p.hyp_pose + (size_t)i * 6;
     const double rvec[3] = {hp[0], hp[1], hp[2]}, tvec[2] = {hp[3], hp[4]};
     double Rm[9];

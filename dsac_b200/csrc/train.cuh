@@ -5,6 +5,7 @@
 // reference's order, so the kernels downstream (k_refine, k_dsac_combine, k_dscore) see the same jobs in the same order.
 #pragma once
 #include "pose_math.cuh"
+#include "prior.cuh"
 #include "sampler.cuh"
 
 namespace dsac {
@@ -142,6 +143,8 @@ __device__ __forceinline__ int block_exclusive_sum(int v, int* s_warp, int* tota
 
 struct SelectParams {
     int n, H, skip;
+    int prior_k;                 // pose priors of the pass: slots H - prior_k .. H - 1 of a frame without DSAC_ST_BAD_PRIOR
+    const uint32_t* status;      // [n] (read with prior_k > 0)
     const double* sf;            // [n][H]
     const int32_t* img_idx;      // [n][H][4]
     const double* hyp_pose;      // [n][H][6]
@@ -171,8 +174,8 @@ struct SelectParams {
     int32_t* pair_scale;         // [pairs]
 };
 
-// The hypotheses with sf > 1e-4 and a minimal set (train_ransac.cpp:320), and in a seeded backward a nonzero seed (a zero
-// seed contributes nothing to path I), stably compacted; one CTA walks the frames.
+// The hypotheses with sf > 1e-4 and a minimal set (train_ransac.cpp:320) or a pose prior in their slot, and in a seeded
+// backward a nonzero seed (a zero seed contributes nothing to path I), stably compacted; one CTA walks the frames.
 constexpr int SELECT_THREADS = 1024;   // = DSAC_MAX_HYPS: one pass per frame
 __global__ void __launch_bounds__(SELECT_THREADS) k_dsac_select(SelectParams p) {
     __shared__ int s_warp[33];
@@ -180,7 +183,8 @@ __global__ void __launch_bounds__(SELECT_THREADS) k_dsac_select(SelectParams p) 
     int base = 0;
     for (int f = 0; f < p.n; f++) {
         const size_t g = (size_t)f * p.H + tid;
-        bool take = tid < p.H && p.sf[g] > SELECT_MIN_SF && p.img_idx[g * 4] >= 0;
+        const bool prior = p.prior_k > 0 && tid >= p.H - p.prior_k && !(p.status[f] & PRIOR_ST_BAD);
+        bool take = tid < p.H && p.sf[g] > SELECT_MIN_SF && (p.img_idx[g * 4] >= 0 || prior);
         if (take && p.seeded) {
             bool nz = false;
             if (p.seed)
@@ -207,7 +211,8 @@ __device__ __forceinline__ bool job_cell(const int32_t* im, const int32_t* cells
     return im[c] != 0 && c != cells[0] && c != cells[1] && c != cells[2] && c != cells[3];
 }
 
-// Pairs of hypothesis s: 9 on the minimal set, 3 per skip-th job cell.  Grid: n H CTAs, those past the selection exit.
+// Pairs of hypothesis s: 9 on the minimal set (none for a pose prior, which has no minimal set: img_idx -1), 3 per skip-th
+// job cell.  Grid: n H CTAs, those past the selection exit.
 constexpr int JOBS_THREADS = 256;
 constexpr int JOBS_CELLS = (DSAC_N_CONST + JOBS_THREADS - 1) / JOBS_THREADS;   // 7 cells of the x-outer order per thread
 __global__ void __launch_bounds__(JOBS_THREADS) k_dsac_jobs_count(SelectParams p) {
@@ -220,7 +225,7 @@ __global__ void __launch_bounds__(JOBS_THREADS) k_dsac_jobs_count(SelectParams p
     for (int c = threadIdx.x; c < DSAC_N_CONST; c += JOBS_THREADS) nz += job_cell(im, cells, c) ? 1 : 0;
     int total;
     block_exclusive_sum(nz, s_warp, &total);
-    if (threadIdx.x == 0) p.pair_count[s] = 9 + 3 * (total / p.skip);
+    if (threadIdx.x == 0) p.pair_count[s] = (cells[0] >= 0 ? 9 : 0) + 3 * (total / p.skip);
 }
 
 // Exclusive scan of the pair counts; per-frame pair ranges and job counts; totals[1] = refinement jobs.  One CTA.
@@ -267,7 +272,8 @@ __global__ void __launch_bounds__(JOBS_THREADS) k_dsac_jobs(SelectParams p) {
     const int g = p.sel[s], f = p.sel_frame[s], q0 = p.pair_begin[s], nper = p.n_perm[s];
     const int32_t* im = p.imaps + (size_t)s * DSAC_N_CONST;
     const int32_t* cells = p.img_idx + (size_t)g * 4;
-    if (tid < 9) write_pair(p, q0 + tid, g, f, cells[tid / 3], tid % 3, true, tid / 3, nper);
+    const int n_min = cells[0] >= 0 ? 9 : 0;   // a pose prior: no minimal-set pairs
+    if (tid < n_min) write_pair(p, q0 + tid, g, f, cells[tid / 3], tid % 3, true, tid / 3, nper);
     const int o0 = tid * JOBS_CELLS;
     int nz = 0;
     for (int o = o0; o < min(o0 + JOBS_CELLS, DSAC_N_CONST); o++) nz += job_cell(im, cells, (o % DSAC_GRID_CONST) * DSAC_GRID_CONST + o / DSAC_GRID_CONST) ? 1 : 0;
@@ -277,7 +283,7 @@ __global__ void __launch_bounds__(JOBS_THREADS) k_dsac_jobs(SelectParams p) {
         const int cell = (o % DSAC_GRID_CONST) * DSAC_GRID_CONST + o / DSAC_GRID_CONST;   // o = x * 40 + y
         if (!job_cell(im, cells, cell)) continue;
         if (++k % p.skip != 0) continue;
-        const int q = q0 + 9 + (k / p.skip - 1) * 3;
+        const int q = q0 + n_min + (k / p.skip - 1) * 3;
         for (int ch = 0; ch < 3; ch++) write_pair(p, q + ch, g, f, cell, ch, false, 0, nper);
     }
 }

@@ -33,11 +33,13 @@ EXPORTS = [
     "dsac_score_draw_device", "dsac_score_maps_device", "dsac_shuffle_permutations",
     "dsac_set_sampling_logits_device", "dsac_set_cell_depth_device", "dsac_sampling_table_device", "dsac_sampling_log_prob_device",
     "dsac_sampling_log_prob_backward_device", "dsac_set_coord_derivatives", "dsac_pose_uncertainty_device",
-    "dsac_last_pass",
+    "dsac_last_pass", "dsac_set_pose_priors_device",
 ]
 
 ST_OBJ_DRAW_EXHAUSTED = 8    # DSAC_ST_OBJ_DRAW_EXHAUSTED
 ST_DEPTH_DROPPED = 16        # DSAC_ST_DEPTH_DROPPED
+ST_BAD_PRIOR = 128           # DSAC_ST_BAD_PRIOR
+MAX_PRIORS = 16              # DSAC_MAX_PRIORS
 OBJ_STATE_WORDS = 625        # one ThreadRand stream: std::mt19937's 624 words and its position
 
 
@@ -185,6 +187,7 @@ def load(build_if_missing=True):
     lib.dsac_set_stages.argtypes = [C.c_void_p, C.c_uint32]
     lib.dsac_set_sampling_logits_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.dsac_set_cell_depth_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.dsac_set_pose_priors_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p]
     lib.dsac_set_coord_derivatives.argtypes = [C.c_void_p, C.c_int32]
     lib.dsac_sampling_table_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
     lib.dsac_sampling_log_prob_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
@@ -417,6 +420,15 @@ class Engine:
         following passes RGB-D passes; d_depth None / 0 returns to RGB."""
         self._check(self.lib.dsac_set_cell_depth_device(self.h, n if d_depth else 0, C.c_void_p(d_depth) if d_depth else None,
                                                         C.c_void_p(stream) if stream else None))
+
+    def set_pose_priors_device(self, n, k, d_poses, d_info=None, gate=0.0, stream=None):
+        """dsac_set_pose_priors_device: k cv poses per frame, float64 [n][k][6] on the device (raw pointer as int), take the
+        last k hypothesis slots of the following passes; d_info (float64 [n][k][6][6] information matrices, or None) gates
+        the sampled hypotheses at the chi^2 bound `gate` (INTEGRATION.md, "Pose priors").  d_poses None / 0 clears them."""
+        self._check(self.lib.dsac_set_pose_priors_device(self.h, n if d_poses else 0, k if d_poses else 0,
+                                                         C.c_void_p(d_poses) if d_poses else None,
+                                                         C.c_void_p(d_info) if d_info else None, float(gate),
+                                                         C.c_void_p(stream) if stream else None))
 
     def set_coord_derivatives(self, mode):
         """dsac_set_coord_derivatives: "central" (the reference's central differences, the default) or "implicit" (the

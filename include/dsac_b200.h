@@ -34,6 +34,7 @@ extern "C" {
 #define DSAC_MAXINPUT 100.0f              /* CNN_OBJ_MAXINPUT, lua_calls.h:36 */
 #define DSAC_MAX_HYPS 1024
 #define DSAC_MAX_REF_STEPS 16
+#define DSAC_MAX_PRIORS 16
 
 #define DSAC_OK 0
 #define DSAC_ERR_ARG (-1)
@@ -49,6 +50,7 @@ extern "C" {
 #define DSAC_ST_DEPTH_DROPPED 16u         /* dsac_register_depth_device: registration targets outside the image were dropped */
 #define DSAC_ST_BAD_WEIGHTS 32u           /* guided sampling: a NaN or +inf logit, or fewer than 4 cells with weight > 0; nothing sampled */
 #define DSAC_ST_NO_DEPTH 64u              /* RGB-D pass: fewer than 4 cells with depth; nothing sampled */
+#define DSAC_ST_BAD_PRIOR 128u            /* a non-finite prior or an information matrix that is not positive definite; nothing sampled */
 
 typedef struct dsac_engine dsac_engine;
 
@@ -199,6 +201,31 @@ int dsac_set_sampling_logits_device(dsac_engine* e, int32_t n, const float* d_lo
  * dsac_refined_jp6_device and dsac_sampling_log_prob*_device refuse a pass after which the setting changed.
  * DSAC_ERR_ARG, with the engine left as it was: n outside [1, max_frames], or a submitted pass that has not been awaited. */
 int dsac_set_cell_depth_device(dsac_engine* e, int32_t n, const float* d_depth, void* stream);
+/* Pose priors (INTEGRATION.md, "Pose priors"): k caller poses per frame join the hypothesis pool of the following passes, for
+ * a tracker's prediction or the last frame's refined pose.  d_poses: DEVICE float64 [n][k][6] cv poses (rvec, tvec mm,
+ * scene->camera, the representation of hyp_pose and ref_pose).  Prior j of frame f takes hypothesis slot n_hyps - k + j:
+ * hyp_pose its bits, img_idx (all four) and cand_idx -1; slots 0 .. n_hyps - k - 1 are drawn exactly as an engine with
+ * n_hyps - k draws them (quotas stream_chunk(n_hyps - k, n_streams, s)); k == n_hyps samples nothing.  Everything after
+ * sampling (scoring, the score seam, softmax, refinement, the DSAC draw, refine-all, every backward and the pose queries)
+ * sees n_hyps hypotheses.  d_info: DEVICE float64 [n][k][6][6] or NULL.  If set, an information matrix Lambda_j (an inverse
+ * covariance) per prior in the chart R = exp([w]x) R_j, t = t_j + tau (w rad, tau mm; inv(cov_xi + Q) of
+ * dsac_pose_uncertainty_device is one), lower triangle read; a candidate the sampler would accept (the P3P pose after the
+ * 4-point check, or the RGB-D Kabsch fit after its tests) is accepted only if min_j xi^T Lambda_j xi <= gate, xi =
+ * (log(R_h R_j^T) principal, t_h - t_j) in fp64; a gated-out candidate is an ordinary rejection (counts, quotas,
+ * max_candidates, DSAC_ST_SAMPLER_EXHAUSTED, the used candidates of dsac_sampling_log_prob_device).  gate: a chi^2 bound,
+ * finite and > 0 with d_info, else ignored.  A frame with a non-finite prior entry, or a Lambda_j whose Cholesky has a pivot
+ * below 1e-12 of its diagonal entry, gets DSAC_ST_BAD_PRIOR, samples nothing and has all n_hyps slots empty (zero pose,
+ * img_idx -1); decided on the device, other frames unaffected.  Priors are constants of the backward passes: a prior's
+ * dPNP is zero, its score is differentiated directly, and in the DSAC variant a selected prior has its inlier-cell
+ * refinement jobs and no minimal-set jobs.  Copied on `stream` into engine-owned buffers (sized once for max_frames x
+ * DSAC_MAX_PRIORS); the caller's buffers may be reused once `stream` has passed this call.  Sticky like dsac_set_cell_depth_device:
+ * later passes must have n frames; d_poses == NULL (n, k ignored) clears the setting.  Every backward entry point,
+ * dsac_refined_jp6_device, dsac_pose_uncertainty_device and dsac_sampling_log_prob*_device refuse a pass after which the
+ * setting changed.  DSAC_ERR_ARG, with the engine left as it was: n outside [1, max_frames], k outside
+ * [1, min(n_hyps, DSAC_MAX_PRIORS)], a bad gate, or a submitted pass that has not been awaited. */
+int dsac_set_pose_priors_device(dsac_engine* e, int32_t n, int32_t k, const double* d_poses, const double* d_info, double gate,
+                                void* stream);
+
 /* Scene-coordinate derivatives of the backward passes (INTEGRATION.md, "Implicit-function gradients").
  * DSAC_DERIV_CENTRAL (the default): the reference's central differences.  DSAC_DERIV_IMPLICIT: two quantities change.
  *   dRefineObj  the implicit-function derivative of the refined pose with respect to the cells the last accepted refinement
@@ -346,7 +373,8 @@ typedef struct dsac_backward_dsac_out {
     double* path2;            /* [n][N][3]  nullable */
     double* score_grads;      /* [n][H]     scoreOutputGradients, nullable  cnn.h:733-741 */
     int32_t* n_selected;      /* [n]        hypotheses with sf > 1e-4, nullable */
-    int32_t* n_refine_jobs;   /* [n]        refine() evaluations of path I, nullable (DSAC_DERIV_IMPLICIT: 18 per selected hypothesis) */
+    int32_t* n_refine_jobs;   /* [n]        refine() evaluations of path I, nullable (DSAC_DERIV_IMPLICIT: 18 per selected hypothesis,
+                                 0 per selected pose prior) */
 } dsac_backward_dsac_out;
 int dsac_backward_dsac(dsac_engine* e, int32_t n_frames, dsac_backward_dsac_out* out);
 /* The same backward after a dsac_forward_dsac(_device), on the caller's `stream` (ordered after that forward by an event):
