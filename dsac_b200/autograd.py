@@ -8,6 +8,7 @@
     sf, ref = dsac_hypotheses(engine, prediction, pix)              # softmax [n][H], refined jp 6-vectors [n][H][6]
     my_loss(pose).backward()                                        # prediction.grad, no ground truth needed
     unc = pose_uncertainty(engine, n)                               # covariances and support of the last pass's poses
+    modes = pose_modes(engine, n, 4, 0.17, 100.0)                   # up to 4 distinct refined poses per frame
 
 `prediction` is the coordinate CNN's output: float32 [n][1600][3] scene coordinates in metres on the engine's device,
 cell y*40+x.  It is the only input that receives a gradient.  The gradient is the one the reference hands to
@@ -336,6 +337,28 @@ def pose_uncertainty(engine, n):
     for k in ("n_fit", "support", "ok"):
         out[k] = torch.empty(lead, dtype=torch.int32, device=dev)
     engine.pose_uncertainty_device(n, torch.cuda.current_stream(dev).cuda_stream, **{k: v.data_ptr() for k, v in out.items()})
+    return out
+
+
+def pose_modes(engine, n, max_modes, rot_rad, trans_mm):
+    """The distinct refined poses of each frame's hypothesis pool after the engine's last pass over n frames, of either
+    pipeline (INTEGRATION.md, "Pose modes"), a dict of device tensors on torch.cuda.current_stream(): n_modes int32 [n];
+    hyp, members, steps_done, n_fit, support and ok int32 [n][M]; score, mass and sigma2 float64 [n][M]; pose float64
+    [n][M][6] (cv poses, as the priors of pose_priors= take them); cov_xi float64 [n][M][6][6], M = max_modes.  Modes
+    0 .. n_modes - 1 are in seed order (the best-scored first); later entries have hyp -1 and zeros.  Two poses are near
+    iff their rotations differ by at most rot_rad and their translations by at most trans_mm.  These outputs carry no
+    autograd history."""
+    dev = torch.device("cuda", engine.cfg.device)
+    M = int(max_modes)
+    out = {"n_modes": torch.empty((n,), dtype=torch.int32, device=dev),
+           "pose": torch.empty((n, M, 6), dtype=torch.float64, device=dev),
+           "cov_xi": torch.empty((n, M, 6, 6), dtype=torch.float64, device=dev)}
+    for k in ("score", "mass", "sigma2"):
+        out[k] = torch.empty((n, M), dtype=torch.float64, device=dev)
+    for k in ("hyp", "members", "steps_done", "n_fit", "support", "ok"):
+        out[k] = torch.empty((n, M), dtype=torch.int32, device=dev)
+    engine.pose_modes_device(n, M, rot_rad, trans_mm, torch.cuda.current_stream(dev).cuda_stream,
+                             **{k: v.data_ptr() for k, v in out.items()})
     return out
 
 

@@ -27,6 +27,7 @@
 #include "rgbd.cuh"
 #include "train.cuh"
 #include "uncertainty.cuh"
+#include "modes.cuh"
 #include "upstream.cuh"
 #include "objtrain.cuh"
 #include "scoretrain.cuh"
@@ -35,6 +36,7 @@ using namespace dsac;
 
 static_assert(sizeof(Cam) == sizeof(dsac_camera), "Cam mirrors dsac_camera");
 static_assert(PRIOR_MAX == DSAC_MAX_PRIORS && PRIOR_ST_BAD == DSAC_ST_BAD_PRIOR, "prior.cuh mirrors dsac_b200.h");
+static_assert(MODE_MAX == DSAC_MAX_MODES && DSAC_MAX_HYPS <= 1024, "modes.cuh mirrors dsac_b200.h");
 static_assert(sizeof(ObjCam) == sizeof(dsac_rgbd_camera) && offsetof(ObjCam, sensor_trans) == offsetof(dsac_rgbd_camera, sensor_trans) &&
                   offsetof(ObjCam, raw_data) == offsetof(dsac_rgbd_camera, raw_data),
               "ObjCam mirrors dsac_rgbd_camera");
@@ -128,6 +130,7 @@ struct dsac_engine {
     int cur_pix_shared = 0;
     const double* cur_gt = nullptr;
     int cur_n = 0;
+    uint32_t fwd_stages = DSAC_STAGE_ALL;   // the stages the last soft-argmax pass ran (dsac_set_stages)
     int k1_slots = 296;             // resident k_sample CTAs on this GPU (SMs x CTAs/SM), set at creation
     int dsac_n = 0;                 // frames of the last dsac_forward_dsac (0: none), for dsac_backward_dsac
     long long cur_frame0 = 0;
@@ -221,6 +224,10 @@ struct dsac_engine {
     IftScratch unc;
     DevMem<char> unc_buf;
     Event ev_unc;
+    // dsac_pose_modes_device: its seeds, recording replay and covariances in one grow-only block of its own, ordered by
+    // ev_modes as the uncertainty scratch is by ev_unc
+    DevMem<char> modes_buf;
+    Event ev_modes;
     std::vector<DevMem<char>> bw_pool;   // device buffers of dsac_backward_dsac, kept across calls
     Stream pipe[4];                 // chunked H2D / compute / D2H pipeline of dsac_forward
     // tail split (dsac_set_tail_split): the whole sampler waves of a batch run on a high-priority side stream, the
@@ -607,6 +614,7 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
         CUC(cudaEventCreateWithFlags(e->ev_g.put(), cudaEventDisableTiming));
         CUC(cudaEventCreateWithFlags(e->ev_depth.put(), cudaEventDisableTiming));
         CUC(cudaEventCreateWithFlags(e->ev_unc.put(), cudaEventDisableTiming));
+        CUC(cudaEventCreateWithFlags(e->ev_modes.put(), cudaEventDisableTiming));
         if (const char* ts = getenv("DSAC_TAIL_SPLIT")) e->tail_split = atoi(ts);
     }
 #undef CUC
@@ -1349,6 +1357,7 @@ int dsac_forward_device(dsac_engine* e, int32_t n, int64_t frame0, const int16_t
     e->cur_pix_shared = pix_shared;
     e->cur_gt = d_gt_jp;
     e->cur_n = n;
+    e->fwd_stages = e->stages;
     e->dsac_n = 0;
     e->cur_frame0 = frame0;
     if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_forward_device: a submitted pass has not been awaited (dsac_forward_wait)");
@@ -1444,6 +1453,7 @@ static int forward_submit_impl(dsac_engine* e, int32_t n, int64_t frame0, const 
     e->cur_pix_shared = pix_shared;
     e->cur_gt = gt_jp ? e->d_gt.get() : nullptr;
     e->cur_n = n;
+    e->fwd_stages = e->stages;
     e->dsac_n = 0;
     e->cur_frame0 = frame0;
     // Frames are independent, so the batch is cut into up to 4 chunks, each on its own stream:
@@ -2057,3 +2067,4 @@ int dsac_score_maps_device(dsac_engine* e, int32_t n_images, int32_t hyps_per_im
 #include "backward_host.inc"
 #include "backward_dsac_host.inc"
 #include "uncertainty_host.inc"
+#include "modes_host.inc"

@@ -3,6 +3,7 @@
 //
 //   PriorGate        one prior as the gate reads it: its rotation, translation and the Cholesky factor of its information
 //   prior_cholesky   the factor from the lower triangle of a 6x6 information matrix, with the refusal of DSAC_ST_BAD_PRIOR
+//   so3_angle        the angle of a rotation, atan2(|skew part|, (tr - 1) / 2)
 //   so3_log          the principal log of a rotation, accurate up to and at pi
 //   prior_d2         xi^T Lambda xi of a pose against one prior, xi = (log(R_h R_j^T), t_h - t_j)
 //   k_prior_prep     once per setting: validates every prior of a frame, writes the gate table and the frame's bad flag
@@ -48,14 +49,28 @@ DSAC_HD bool prior_cholesky(const double* info, double L[21]) {
     return true;
 }
 
-// w = log(M), |w| <= pi, for a rotation M (row-major).  The angle comes from atan2(|skew|, (tr - 1) / 2), accurate everywhere;
-// the axis from the skew part below pi / 2 and from the symmetric part M + M^T = 2 c I + 2 (1 - c) n n^T above, where the
-// skew part vanishes (its sign picks n against -n; at exactly pi both are the principal log).
+// M = A B^T of two row-major 3x3 matrices.
+DSAC_HD void rot_mul_bt(const double A[9], const double B[9], double M[9]) {
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) M[i * 3 + j] = A[i * 3] * B[j * 3] + A[i * 3 + 1] * B[j * 3 + 1] + A[i * 3 + 2] * B[j * 3 + 2];
+}
+
+// The rotation angle th in [0, pi] of a rotation M (row-major): atan2(|v|, c), accurate everywhere, from the skew part
+// v = sin(th) n and c = cos(th) = (tr - 1) / 2; also returns v, s = |v| and c.  so3_log and the pose modes' nearness test
+// (modes.cuh) share it.
+DSAC_HD double so3_angle(const double M[9], double v[3], double* s, double* c) {
+    v[0] = 0.5 * (M[7] - M[5]); v[1] = 0.5 * (M[2] - M[6]); v[2] = 0.5 * (M[3] - M[1]);
+    *s = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+    *c = 0.5 * (M[0] + M[4] + M[8] - 1.0);
+    return atan2(*s, *c);
+}
+
+// w = log(M), |w| <= pi, for a rotation M (row-major).  The angle is so3_angle's; the axis comes from the skew part below
+// pi / 2 and from the symmetric part M + M^T = 2 c I + 2 (1 - c) n n^T above, where the skew part vanishes (its sign picks n
+// against -n; at exactly pi both are the principal log).
 DSAC_HD void so3_log(const double M[9], double w[3]) {
-    const double v[3] = {0.5 * (M[7] - M[5]), 0.5 * (M[2] - M[6]), 0.5 * (M[3] - M[1])};   // sin(th) n
-    const double s = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
-    const double c = 0.5 * (M[0] + M[4] + M[8] - 1.0);
-    const double th = atan2(s, c);
+    double v[3], s, c;
+    const double th = so3_angle(M, v, &s, &c);
     if (c > 0) {
         const double k = s > 0 ? th / s : 1.0;
         for (int i = 0; i < 3; i++) w[i] = k * v[i];
@@ -75,8 +90,7 @@ DSAC_HD void so3_log(const double M[9], double w[3]) {
 // d^2 = xi^T Lambda xi = |L^T xi|^2 of the pose (Rh, th) against prior g, xi = (log(Rh Rj^T) rad, th - tj mm), fp64.
 DSAC_HD double prior_d2(const double Rh[9], const double th[3], const PriorGate& g) {
     double M[9];
-    for (int i = 0; i < 3; i++)
-        for (int j = 0; j < 3; j++) M[i * 3 + j] = Rh[i * 3] * g.R[j * 3] + Rh[i * 3 + 1] * g.R[j * 3 + 1] + Rh[i * 3 + 2] * g.R[j * 3 + 2];
+    rot_mul_bt(Rh, g.R, M);
     double xi[6];
     so3_log(M, xi);
     for (int i = 0; i < 3; i++) xi[3 + i] = th[i] - g.t[i];

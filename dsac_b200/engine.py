@@ -33,13 +33,14 @@ EXPORTS = [
     "dsac_score_draw_device", "dsac_score_maps_device", "dsac_shuffle_permutations",
     "dsac_set_sampling_logits_device", "dsac_set_cell_depth_device", "dsac_sampling_table_device", "dsac_sampling_log_prob_device",
     "dsac_sampling_log_prob_backward_device", "dsac_set_coord_derivatives", "dsac_pose_uncertainty_device",
-    "dsac_last_pass", "dsac_set_pose_priors_device",
+    "dsac_last_pass", "dsac_set_pose_priors_device", "dsac_pose_modes_device",
 ]
 
 ST_OBJ_DRAW_EXHAUSTED = 8    # DSAC_ST_OBJ_DRAW_EXHAUSTED
 ST_DEPTH_DROPPED = 16        # DSAC_ST_DEPTH_DROPPED
 ST_BAD_PRIOR = 128           # DSAC_ST_BAD_PRIOR
 MAX_PRIORS = 16              # DSAC_MAX_PRIORS
+MAX_MODES = 16               # DSAC_MAX_MODES
 OBJ_STATE_WORDS = 625        # one ThreadRand stream: std::mt19937's 624 words and its position
 
 
@@ -140,6 +141,13 @@ class PoseUncertaintyOut(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in _UNC_FIELDS]
 
 
+_MODES_FIELDS = ("n_modes", "hyp", "pose", "score", "mass", "members", "steps_done", "cov_xi", "sigma2", "n_fit", "support", "ok")
+
+
+class PoseModesOut(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in _MODES_FIELDS]
+
+
 SCORE_HOOK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p)
 SCORE_BACKWARD_HOOK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p)
 
@@ -208,6 +216,8 @@ def load(build_if_missing=True):
     lib.dsac_refined_jp6_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.dsac_pose_uncertainty_device.argtypes = [C.c_void_p, C.c_int32, C.POINTER(PoseUncertaintyOut), C.c_void_p]
     lib.dsac_last_pass.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
+    lib.dsac_pose_modes_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_double, C.c_double, C.POINTER(PoseModesOut),
+                                           C.c_void_p]
     lib.dsac_backward_pose_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]
     lib.dsac_backward_dsac_pose_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(BackwardDsacOut),
                                                    C.c_void_p, C.c_float, C.c_void_p]
@@ -620,6 +630,19 @@ class Engine:
                 raise KeyError(k)
             setattr(raw, k, v)
         self._check(self.lib.dsac_pose_uncertainty_device(self.h, n, C.byref(raw), C.c_void_p(stream) if stream else None))
+
+    def pose_modes_device(self, n, max_modes, rot_rad, trans_mm, stream=None, **ptrs):
+        """dsac_pose_modes_device (raw device pointers as ints): the distinct refined poses of each frame's hypothesis pool
+        after the preceding pass over n frames (INTEGRATION.md, "Pose modes"); ptrs: device destinations of the fields of
+        dsac_pose_modes_out (n_modes [n]; hyp, pose, score, mass, members, steps_done, cov_xi, sigma2, n_fit, support, ok
+        [n][max_modes](...))."""
+        raw = PoseModesOut()
+        for k, v in ptrs.items():
+            if k not in _MODES_FIELDS:
+                raise KeyError(k)
+            setattr(raw, k, v)
+        self._check(self.lib.dsac_pose_modes_device(self.h, n, max_modes, float(rot_rad), float(trans_mm), C.byref(raw),
+                                                    C.c_void_p(stream) if stream else None))
 
     def last_pass(self, n):
         """dsac_last_pass: "softam" or "dsac", the pipeline of the pass over n frames whose refined poses the engine holds

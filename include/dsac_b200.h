@@ -428,6 +428,43 @@ int dsac_pose_uncertainty_device(dsac_engine* e, int32_t n_frames, const dsac_po
 #define DSAC_PASS_DSAC 2
 int dsac_last_pass(dsac_engine* e, int32_t n_frames, int32_t* pipeline);
 
+/* Pose modes of the preceding pass (INTEGRATION.md, "Pose modes"): per frame up to M = max_modes distinct refined poses of
+ * its hypothesis pool, each with the pool's probability behind it, its covariance and its support; a frame's modes fit one
+ * dsac_set_pose_priors_device setting.  After either pipeline's forward over n_frames (the pass dsac_last_pass names):
+ *   1. occupied slots: img_idx[f][h][0] >= 0, or a prior slot of a pass with priors whose frame lacks DSAC_ST_BAD_PRIOR;
+ *   2. they are ranked by scores (the hook's, with a score hook) descending, ties to the lower slot, NaN after every score;
+ *   3. walking the ranking, a slot near a seed joins the first such seed in seed order, else becomes a new seed while fewer
+ *      than M exist, else joins nothing.  Two poses are near iff theta <= rot_rad and |t_a - t_b| <= trans_mm, theta the
+ *      angle of R_a R_b^T (atan2 of its skew part's norm and (tr - 1) / 2, fp64).  A seed's mass is the sum of its
+ *      members' sf in rank order, members their number;
+ *   4. each seed is refined from its own hypothesis pose as dsac_forward_dsac refines that slot (pose, steps_done), and has
+ *      the covariance of dsac_pose_uncertainty_device's entry for that DSAC-variant job (cov_xi .. ok);
+ *   5. in seed order, a seed whose refined pose is near the refined pose of an earlier surviving seed adds its mass and
+ *      members to the first such one and is dropped.  The survivors are entries 0 .. n_modes - 1 in seed order; every
+ *      later entry has hyp -1 and zeros.
+ * Stream ordering, input lifetime and "changes no later result" as in dsac_pose_uncertainty_device; the pass's outputs are
+ * untouched.  DSAC_ERR_ARG, with the engine left as it was: not after a forward over the same n_frames, a submitted pass
+ * that has not been awaited, cameras, cell depth or priors changed since the pass, a pass that skipped the sample or
+ * score stage (dsac_set_stages), max_modes outside [1, min(n_hyps, DSAC_MAX_MODES)], rot_rad or trans_mm not finite or
+ * negative, or d_out NULL.  The outputs are not differentiated. */
+#define DSAC_MAX_MODES 16          /* = DSAC_MAX_PRIORS: a frame's modes fit one priors setting */
+typedef struct dsac_pose_modes_out {   /* DEVICE pointers, each nullable; M = max_modes */
+    int32_t* n_modes;     /* [n]           modes found, 0 .. M */
+    int32_t* hyp;         /* [n][M]        hypothesis slot of the mode's seed, -1 unused */
+    double*  pose;        /* [n][M][6]     refined cv pose (rvec, tvec mm), as hyp_pose / ref_pose */
+    double*  score;       /* [n][M]        the seed's score (before softmax) */
+    double*  mass;        /* [n][M]        sum of sf over the mode's members */
+    int32_t* members;     /* [n][M]        hypotheses in the mode */
+    int32_t* steps_done;  /* [n][M] */
+    double*  cov_xi;      /* [n][M][6][6]  as dsac_pose_uncertainty_out.cov_xi */
+    double*  sigma2;      /* [n][M] */
+    int32_t* n_fit;       /* [n][M] */
+    int32_t* support;     /* [n][M] */
+    int32_t* ok;          /* [n][M] */
+} dsac_pose_modes_out;
+int dsac_pose_modes_device(dsac_engine* e, int32_t n_frames, int32_t max_modes, double rot_rad, double trans_mm,
+                           const dsac_pose_modes_out* d_out, void* stream);
+
 /* Soft-argmax backward seeded by d_grad_ref [n][6] = dOuter/d(refined jp6) instead of dLossMax.
  * No ground truth needed. dloss_dobj / dloss_dpred / clamp as in dsac_backward_device; clamp applies to the total. */
 int dsac_backward_pose_device(dsac_engine* e, int32_t n_frames, const double* d_grad_ref,
