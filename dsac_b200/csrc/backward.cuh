@@ -897,10 +897,9 @@ __global__ void __launch_bounds__(IFT_THREADS) k_refine_ift_rgbd(IftParams p) { 
 __global__ void __launch_bounds__(IFT_THREADS) k_refine_ift_rgbd_cam(IftParams p) { k_refine_ift_body<true, true>(p); }
 
 inline void launch_refine_ift(const IftParams& p, unsigned jobs, cudaStream_t stream) {
-    if (p.eye && p.cams) k_refine_ift_rgbd_cam<<<jobs, IFT_THREADS, 0, stream>>>(p);
-    else if (p.eye) k_refine_ift_rgbd<<<jobs, IFT_THREADS, 0, stream>>>(p);
-    else if (p.cams) k_refine_ift_cam<<<jobs, IFT_THREADS, 0, stream>>>(p);
-    else k_refine_ift<<<jobs, IFT_THREADS, 0, stream>>>(p);
+    // [per-frame camera][RGB-D]
+    constexpr void (*tab[2][2])(IftParams) = {{k_refine_ift, k_refine_ift_rgbd}, {k_refine_ift_cam, k_refine_ift_rgbd_cam}};
+    tab[p.cams != nullptr][p.eye != nullptr]<<<jobs, IFT_THREADS, 0, stream>>>(p);
 }
 
 // jp pose + Rodrigues Jacobian of hypothesis h for k_dscore, as k_dpnp / k_dkabsch write it

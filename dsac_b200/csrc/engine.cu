@@ -43,6 +43,25 @@ static_assert(sizeof(ObjCam) == sizeof(dsac_rgbd_camera) && offsetof(ObjCam, sen
 
 static std::string g_create_error;
 
+// The instantiations of the forward pass's kernel families, indexed by the pass's variant flags in one order:
+// [per-frame camera][RGB-D][prior gate], then a family's own flag (k1_solve: four lanes per candidate, k_score: write the
+// diffmaps).  dsac_engine_create sets their attributes through the same tables.
+static constexpr void (*k_sample_tab[2][2][2])(SampleParams) = {
+    {{k_sample_t<false, false, false>, k_sample_t<false, false, true>}, {k_sample_t<false, true, false>, k_sample_t<false, true, true>}},
+    {{k_sample_t<true, false, false>, k_sample_t<true, false, true>}, {k_sample_t<true, true, false>, k_sample_t<true, true, true>}}};
+static constexpr void (*k1_gtail_tab[2][2][2])(K1SplitParams, GuidedGen) = {
+    {{k1_gtail_t<false, false, false>, k1_gtail_t<false, false, true>}, {k1_gtail_t<false, true, false>, k1_gtail_t<false, true, true>}},
+    {{k1_gtail_t<true, false, false>, k1_gtail_t<true, false, true>}, {k1_gtail_t<true, true, false>, k1_gtail_t<true, true, true>}}};
+static constexpr void (*k1_solve_tab[2][2][2])(K1SplitParams) = {{{k1_solve, k1_solve4}, {k1_solve_gate, k1_solve4_gate}},
+                                                                 {{k1_solve_cam, k1_solve4_cam}, {k1_solve_cam_gate, k1_solve4_cam_gate}}};
+static constexpr void (*k1_kabsch_tab[2][2])(K1SplitParams) = {{k1_kabsch_t<false, false>, k1_kabsch_t<false, true>},
+                                                               {k1_kabsch_t<true, false>, k1_kabsch_t<true, true>}};
+static constexpr void (*k1_filter_tab[2])(K1SplitParams) = {k1_filter, k1_filter_cam};
+static constexpr void (*k1_cells_tab[2])(K1SplitParams, int, int) = {k1_cells, k1_cells_cam};
+static constexpr void (*k_rgbd_eye_tab[2])(const float*, const int32_t*, int, Cam, const Cam*, const uint32_t*, double*, uint32_t*) = {
+    k_rgbd_eye_t<false>, k_rgbd_eye_t<true>};
+static constexpr void (*k_score_tab[2][2])(ScoreParams) = {{k_score<false>, k_score<true>}, {k_score_cam<false>, k_score_cam<true>}};
+
 // Owners of the engine's CUDA resources, the only code here that frees any.  Each releases what it holds in its
 // destructor, is move-only, and converts to the raw pointer or handle for use at call sites.
 template <typename T, cudaError_t (*Alloc)(void**, size_t), cudaError_t (*Free)(void*)>
@@ -106,6 +125,35 @@ class Handle {
 using Stream = Handle<cudaStream_t, cudaStreamDestroy>;
 using Event = Handle<cudaEvent_t, cudaEventDestroy>;
 
+// The per-frame settings of the following passes, indices into dsac_engine::set.
+enum { SET_CAMS, SET_LOGITS, SET_DEPTH, SET_PRIORS, SET_COUNT };
+
+// One per-frame setting: the frames it covers (0: off), a generation that changes with every update, and the event
+// recorded after an update's copy or kernel, which a pass waits for before it reads the setting's buffers.
+struct Setting {
+    int n = 0;
+    unsigned long long gen = 0;
+    Event ev;
+};
+
+// The forward pass the engine holds, which the backward passes and the pose queries read: its inputs and the snapshot
+// of the settings it ran with.
+struct Pass {
+    int32_t kind = 0;               // DSAC_PASS_SOFTAM, DSAC_PASS_DSAC, or 0: none
+    int n = 0;
+    const int16_t* coords = nullptr;
+    const int32_t* pix = nullptr;
+    int pix_shared = 0;
+    const double* gt = nullptr;
+    long long frame0 = 0;
+    uint32_t stages = DSAC_STAGE_ALL;   // the stages the pass ran (dsac_set_stages)
+    uint32_t seed = 0;
+    unsigned long long gen[SET_COUNT] = {};
+    int set_n[SET_COUNT] = {};
+    int prior_k = 0;                // priors per frame
+    bool rgbd() const { return set_n[SET_DEPTH] > 0; }
+};
+
 struct dsac_engine {
     dsac_config cfg;
     std::string err;
@@ -124,52 +172,31 @@ struct dsac_engine {
     DevMem<int16_t> d_coords;
     DevMem<int32_t> d_pix;
     DevMem<double> d_gt;
-    // last-call input views (device), used by fetch / backward
-    const int16_t* cur_coords = nullptr;
-    const int32_t* cur_pix = nullptr;
-    int cur_pix_shared = 0;
-    const double* cur_gt = nullptr;
-    int cur_n = 0;
-    uint32_t fwd_stages = DSAC_STAGE_ALL;   // the stages the last soft-argmax pass ran (dsac_set_stages)
+    Pass pass;                      // the last forward pass
     int k1_slots = 296;             // resident k_sample CTAs on this GPU (SMs x CTAs/SM), set at creation
-    int dsac_n = 0;                 // frames of the last dsac_forward_dsac (0: none), for dsac_backward_dsac
-    long long cur_frame0 = 0;
-    // per-frame cameras (dsac_set_cameras): sized once for max_frames; cams_n == 0: the config's camera
+    Setting set[SET_COUNT];
+    // per-frame cameras (dsac_set_cameras): sized once for max_frames; set[SET_CAMS].n == 0: the config's camera.  Its event
+    // also guards the staging: it is rewritten only after the copy
     DevMem<Cam> d_cams;
     PinnedMem<dsac_camera> h_cams;  // staging of the copy to d_cams
-    Event ev_cams;                  // recorded after that copy: the staging is rewritten, and a pass starts, only after it
-    int cams_n = 0;
-    unsigned long long cams_gen = 0, fwd_cams_gen = 0;   // generation of the setting, and the one the last forward ran with
-    // guided sampling (dsac_set_sampling_logits_device): per-frame tables sized once for max_frames on first use; g_n == 0:
-    // the reference's uniform sampler
+    // guided sampling (dsac_set_sampling_logits_device): per-frame tables sized once for max_frames on first use; off: the
+    // reference's uniform sampler
     DevMem<double> d_g_w;            // [max_frames][N] softmax of the logits
     DevMem<uint32_t> d_g_q, d_g_cum; // [max_frames][N] integer weights and their inclusive prefix sums
     DevMem<uint32_t> d_g_bad;        // [max_frames] DSAC_ST_BAD_WEIGHTS
-    Event ev_g;                      // recorded after the table kernel: a pass starts only after it
-    Event ev_depth;                  // recorded after the copy of the cell depth: a pass starts only after it
-    int g_n = 0;
-    unsigned long long g_gen = 0, fwd_g_gen = 0;   // generation of the setting, and the one the last forward ran with
-    int fwd_g_n = 0;                 // frames of the last forward if it was guided, else 0
-    uint32_t fwd_seed = 0;
-    // RGB-D localisation (dsac_set_cell_depth_device): buffers sized once for max_frames on first use; depth_n == 0: RGB
+    // RGB-D localisation (dsac_set_cell_depth_device): buffers sized once for max_frames on first use; off: RGB
     DevMem<float> d_depth;           // [max_frames][N] the setting's per-cell depth (mm)
     DevMem<double> d_eye;            // [max_frames][N][3] eye coordinates of the pass's cells, NaN without depth
     DevMem<uint32_t> d_rgbd_skip;    // [max_frames] status bits of frames that sample nothing (DSAC_ST_NO_DEPTH, ...)
-    int depth_n = 0;
-    unsigned long long depth_gen = 0, fwd_depth_gen = 0;   // generation of the setting, and the one the last forward ran with
-    bool fwd_rgbd = false;           // the last forward was an RGB-D pass
-    // pose priors (dsac_set_pose_priors_device): tables sized once for max_frames x DSAC_MAX_PRIORS on first use; prior_n == 0:
-    // none.  The prior of frame f, index j, takes hypothesis slot n_hyps - prior_k + j.
-    DevMem<double> d_prior_pose;     // [prior_n][prior_k][6] cv poses
-    DevMem<double> d_prior_info;     // [prior_n][prior_k][36] information matrices (a gate only)
-    DevMem<PriorGate> d_prior_tab;   // [prior_n][prior_k] what the gate reads (k_prior_prep)
-    DevMem<uint32_t> d_prior_bad;    // [prior_n] DSAC_ST_BAD_PRIOR or 0
-    Event ev_prior;                  // recorded after k_prior_prep: a pass starts only after it
-    int prior_n = 0, prior_k = 0;
+    // pose priors (dsac_set_pose_priors_device): tables sized once for max_frames x DSAC_MAX_PRIORS on first use; off: none.
+    // The prior of frame f, index j, takes hypothesis slot n_hyps - prior_k + j.
+    DevMem<double> d_prior_pose;     // [n][prior_k][6] cv poses
+    DevMem<double> d_prior_info;     // [n][prior_k][36] information matrices (a gate only)
+    DevMem<PriorGate> d_prior_tab;   // [n][prior_k] what the gate reads (k_prior_prep)
+    DevMem<uint32_t> d_prior_bad;    // [n] DSAC_ST_BAD_PRIOR or 0
+    int prior_k = 0;
     bool prior_gate = false;
     double prior_chi2 = 0;
-    unsigned long long prior_gen = 0, fwd_prior_gen = 0;   // generation of the setting, and the one the last forward ran with
-    int fwd_prior_k = 0;             // priors per frame of the last forward
     // per-dataset cameras of the pre-training data paths (dsac_set_dataset_cameras), indexed by dataset frame; grow-only.
     // ds_cams_n == 0: no table.  ds_cam0 is entry 0 on the host: the frame size and raw_data every entry shares.
     DevMem<ObjCam> d_ds_cams;
@@ -452,7 +479,7 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
     CUC(e->h_totals.reserve(2 * sizeof(int32_t)));
     CUC(e->d_cams.reserve(n * sizeof(Cam)));
     CUC(e->h_cams.reserve(n * sizeof(dsac_camera)));
-    CUC(cudaEventCreateWithFlags(e->ev_cams.put(), cudaEventDisableTiming));
+    for (Setting& s : e->set) CUC(cudaEventCreateWithFlags(s.ev.put(), cudaEventDisableTiming));
     CUC(cudaEventCreateWithFlags(e->ev_ds_cams.put(), cudaEventDisableTiming));
     CUC(cudaEventCreateWithFlags(e->ev_ds_use.put(), cudaEventDisableTiming));
     CUC(cudaMemset(e->d_frame_counter, 0, n * sizeof(unsigned int)));
@@ -484,26 +511,21 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
         }
         CUC(cudaMemcpy(e->d_perm, perm.data(), perm.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
     }
-    CUC(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1Smem)));
-    CUC(cudaFuncSetAttribute(k_sample_cam, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1Smem)));
-    CUC(cudaFuncSetAttribute(k_sample_rgbd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1Smem)));
-    CUC(cudaFuncSetAttribute(k_sample_rgbd_cam, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1Smem)));
-    for (auto kern : {k_sample_gate, k_sample_cam_gate, k_sample_rgbd_gate, k_sample_rgbd_cam_gate})
-        CUC(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1Smem)));
+    for (const auto& by_rgbd : k_sample_tab)
+        for (const auto& by_gate : by_rgbd)
+            for (auto kern : by_gate) CUC(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1Smem)));
     // k_refine wants 8 CTAs x 26 KB of shared memory per SM: ask for the carve-out explicitly (the default heuristic
     // need not pick the split the launch bounds were written for).  k_sample is left to the default: it spills to
     // local memory, so it wants the L1 that the largest carve-out would take away (DSAC_K1_CARVEOUT overrides).
-    CUC(cudaFuncSetAttribute(k_refine, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    CUC(cudaFuncSetAttribute(k_refine_cam, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    CUC(cudaFuncSetAttribute(k_refine_rgbd, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    CUC(cudaFuncSetAttribute(k_refine_rgbd_cam, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-    if (const char* co = getenv("DSAC_K1_CARVEOUT")) {
-        CUC(cudaFuncSetAttribute(k_sample, cudaFuncAttributePreferredSharedMemoryCarveout, atoi(co)));
-        CUC(cudaFuncSetAttribute(k_sample_cam, cudaFuncAttributePreferredSharedMemoryCarveout, atoi(co)));
+    for (int cam = 0; cam < 2; cam++) {
+        CUC(cudaFuncSetAttribute(k_refine_tab[cam], cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+        CUC(cudaFuncSetAttribute(k_refine_rgbd_tab[cam], cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+        if (const char* co = getenv("DSAC_K1_CARVEOUT"))
+            CUC(cudaFuncSetAttribute(k_sample_tab[cam][0][0], cudaFuncAttributePreferredSharedMemoryCarveout, atoi(co)));
     }
     {
         int per_sm = 0, sms = 0;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_sample, K1_THREADS, sizeof(K1Smem));
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_sample_tab[0][0][0], K1_THREADS, sizeof(K1Smem));
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cfg->device);
         if (per_sm > 0 && sms > 0) e->k1_slots = per_sm * sms;
     }
@@ -592,8 +614,7 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
         CUC(e->d_k1_stats.reserve(16 * sizeof(unsigned long long)));
         CUC(cudaMemset(e->d_k1_stats, 0, 16 * sizeof(unsigned long long)));
         if (getenv("DSAC_K1_DEBUG")) CUC(e->d_k1_dbg.reserve(K1S_MAX_ROUNDS * 4 * sizeof(unsigned long long)));
-        CUC(cudaFuncSetAttribute(k1_filter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1FSmem)));
-        CUC(cudaFuncSetAttribute(k1_filter_cam, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1FSmem)));
+        for (auto kern : k1_filter_tab) CUC(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(K1FSmem)));
         int per_sm = 0;
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k1_filter, K1F_THREADS, sizeof(K1FSmem));
         e->k1_filter_grid = std::max(1, per_sm) * e->sm_count;
@@ -611,8 +632,6 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
         CUC(cudaEventCreateWithFlags(e->ev_fork.put(), cudaEventDisableTiming));
         CUC(cudaEventCreateWithFlags(e->ev_join.put(), cudaEventDisableTiming));
         CUC(cudaEventCreateWithFlags(e->ev_fwd.put(), cudaEventDisableTiming));
-        CUC(cudaEventCreateWithFlags(e->ev_g.put(), cudaEventDisableTiming));
-        CUC(cudaEventCreateWithFlags(e->ev_depth.put(), cudaEventDisableTiming));
         CUC(cudaEventCreateWithFlags(e->ev_unc.put(), cudaEventDisableTiming));
         CUC(cudaEventCreateWithFlags(e->ev_modes.put(), cudaEventDisableTiming));
         if (const char* ts = getenv("DSAC_TAIL_SPLIT")) e->tail_split = atoi(ts);
@@ -644,12 +663,31 @@ int dsac_set_coord_derivatives(dsac_engine* e, int32_t mode) {
     return DSAC_OK;
 }
 
+// The steps every setter of a per-frame setting shares.  A clear changes the generation only if the setting was on.
+static void setting_clear(Setting& s) {
+    if (s.n) s.gen++;
+    s.n = 0;
+}
+// An update turns the setting off until setting_commit, so that a failed copy or launch leaves it off, and `stream` waits
+// for the last forward pass, which may still read the setting's buffers.
+static int setting_begin(dsac_engine* e, Setting& s, cudaStream_t stream) {
+    s.n = 0;
+    s.gen++;
+    CU(cudaStreamWaitEvent(stream, e->ev_fwd, 0));
+    return DSAC_OK;
+}
+static int setting_commit(dsac_engine* e, Setting& s, int32_t n, cudaStream_t stream) {
+    CU(cudaEventRecord(s.ev, stream));
+    s.n = n;
+    return DSAC_OK;
+}
+
 int dsac_set_cameras(dsac_engine* e, int32_t n, const dsac_camera* cams, void* stream_v) {
     if (!e) return DSAC_ERR_ARG;
     if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_set_cameras: a submitted pass has not been awaited (dsac_forward_wait)");
+    Setting& s = e->set[SET_CAMS];
     if (!cams) {
-        if (e->cams_n) e->cams_gen++;
-        e->cams_n = 0;
+        setting_clear(s);
         return DSAC_OK;
     }
     if (n < 1 || n > e->cfg.max_frames) return fail(e, DSAC_ERR_ARG, "dsac_set_cameras: n %d out of range [1,%d]", n, e->cfg.max_frames);
@@ -661,50 +699,120 @@ int dsac_set_cameras(dsac_engine* e, int32_t n, const dsac_camera* cams, void* s
     }
     cudaStream_t stream = (cudaStream_t)stream_v;
     CU(cudaSetDevice(e->cfg.device));
-    CU(cudaEventSynchronize(e->ev_cams));             // the previous copy has left the staging buffer
+    CU(cudaEventSynchronize(s.ev));                   // the previous copy has left the staging buffer
     memcpy(e->h_cams.get(), cams, (size_t)n * sizeof(dsac_camera));
-    CU(cudaStreamWaitEvent(stream, e->ev_fwd, 0));   // the last forward pass may still read the table
-    e->cams_n = 0;                                    // (a failed copy leaves the config's camera in force)
-    e->cams_gen++;
+    if (int rc = setting_begin(e, s, stream)) return rc;
     CU(cudaMemcpyAsync(e->d_cams.get(), e->h_cams.get(), (size_t)n * sizeof(dsac_camera), cudaMemcpyHostToDevice, stream));
-    CU(cudaEventRecord(e->ev_cams, stream));
-    e->cams_n = n;
+    return setting_commit(e, s, n, stream);
+}
+
+// What the pass start reports for a batch that does not match a setting: "n_frames %d differs from the %d <frames>",
+// and what a consumer of the pass reports when the setting changed after it: "the <changed> changed".
+static const struct {
+    const char* setter;
+    const char* frames;
+    const char* changed;
+} k_setting[SET_COUNT] = {
+    {"dsac_set_cameras", "cameras set by dsac_set_cameras", "cameras were"},
+    {"dsac_set_sampling_logits_device", "frames of the sampling logits (dsac_set_sampling_logits_device)", "sampling logits were"},
+    {"dsac_set_cell_depth_device", "frames of the cell depth (dsac_set_cell_depth_device)", "cell depth was"},
+    {"dsac_set_pose_priors_device", "frames of the pose priors (dsac_set_pose_priors_device)", "pose priors were"},
+};
+
+// The start every forward entry point shares: the batch matches each setting in force, each of `streams` waits for the
+// settings' updates, and the record of the pass takes its inputs and the settings' snapshot.  A pipeline's entry point
+// sets the record's kind once the engine holds a pass of it.
+static int pass_begin(dsac_engine* e, int32_t kind, int32_t n, int64_t frame0, const int16_t* coords, const int32_t* pix,
+                      int32_t pix_shared, const double* gt, std::initializer_list<cudaStream_t> streams) {
+    Pass p;
+    for (int i = 0; i < SET_COUNT; i++) {
+        const Setting& s = e->set[i];
+        if (s.n && n != s.n) return fail(e, DSAC_ERR_ARG, "n_frames %d differs from the %d %s", n, s.n, k_setting[i].frames);
+        if (s.n)
+            for (cudaStream_t st : streams) CU(cudaStreamWaitEvent(st, s.ev, 0));
+        p.gen[i] = s.gen;
+        p.set_n[i] = s.n;
+    }
+    p.prior_k = e->set[SET_PRIORS].n ? e->prior_k : 0;
+    p.kind = kind;
+    p.n = n;
+    p.coords = coords; p.pix = pix; p.pix_shared = pix_shared; p.gt = gt;
+    p.frame0 = frame0;
+    p.stages = e->stages;
+    p.seed = e->cfg.seed;
+    e->pass = p;
     return DSAC_OK;
 }
 
-// The checks and the bookkeeping every forward entry point shares: the batch matches the camera table, the pass is
-// stamped with the table's generation and `stream` waits for the table's copy.
-static int cameras_begin_pass(dsac_engine* e, int32_t n, cudaStream_t stream) {
-    if (e->cams_n && n != e->cams_n)
-        return fail(e, DSAC_ERR_ARG, "n_frames %d differs from the %d cameras set by dsac_set_cameras", n, e->cams_n);
-    if (e->cams_n) CU(cudaStreamWaitEvent(stream, e->ev_cams, 0));
-    if (e->g_n && n != e->g_n)
-        return fail(e, DSAC_ERR_ARG, "n_frames %d differs from the %d frames of the sampling logits (dsac_set_sampling_logits_device)", n, e->g_n);
-    if (e->g_n && !e->k1_mode) return fail(e, DSAC_ERR_ARG, "guided sampling needs the split sampler (DSAC_K1_MODE unset)");
-    if (e->g_n) CU(cudaStreamWaitEvent(stream, e->ev_g, 0));
-    if (e->depth_n && n != e->depth_n)
-        return fail(e, DSAC_ERR_ARG, "n_frames %d differs from the %d frames of the cell depth (dsac_set_cell_depth_device)", n, e->depth_n);
-    if (e->depth_n) CU(cudaStreamWaitEvent(stream, e->ev_depth, 0));
-    if (e->prior_n && n != e->prior_n)
-        return fail(e, DSAC_ERR_ARG, "n_frames %d differs from the %d frames of the pose priors (dsac_set_pose_priors_device)", n, e->prior_n);
-    if (e->prior_n) CU(cudaStreamWaitEvent(stream, e->ev_prior, 0));
-    e->fwd_prior_gen = e->prior_gen;
-    e->fwd_prior_k = e->prior_n ? e->prior_k : 0;
-    e->fwd_cams_gen = e->cams_gen;
-    e->fwd_depth_gen = e->depth_gen;
-    e->fwd_rgbd = e->depth_n > 0;
-    e->fwd_g_gen = e->g_gen;
-    e->fwd_g_n = e->g_n;
-    e->fwd_seed = e->cfg.seed;
-    return DSAC_OK;
+// What a consumer of the held pass needs.  kinds: a pass of the soft-argmax pipeline, the DSAC one, or either, over the
+// same n frames; or PASS_GUIDED, a guided pass over n frames.  settings (1 << SET_*): those whose change since the pass
+// makes it stale for the consumer.
+enum { PASS_SOFTAM = 1, PASS_DSAC = 2, PASS_EITHER = 3, PASS_GUIDED = 4 };
+constexpr unsigned SETTINGS_GEOMETRY = 1u << SET_CAMS | 1u << SET_DEPTH | 1u << SET_PRIORS;
+constexpr unsigned SETTINGS_SAMPLING = 1u << SET_LOGITS | 1u << SET_DEPTH | 1u << SET_PRIORS;
+
+static int pass_check(dsac_engine* e, const char* who, int32_t n, unsigned kinds, unsigned settings) {
+    const Pass& p = e->pass;
+    auto unchanged = [&]() {
+        for (int i = 0; i < SET_COUNT; i++) {
+            if (!(settings >> i & 1u) || p.gen[i] == e->set[i].gen) continue;
+            if (kinds == PASS_GUIDED) return fail(e, DSAC_ERR_ARG, "%s: the %s changed after the last pass", who, k_setting[i].changed);
+            return fail(e, DSAC_ERR_ARG, "%s: the %s changed (%s) after the forward pass", who, k_setting[i].changed, k_setting[i].setter);
+        }
+        return (int)DSAC_OK;
+    };
+    if (kinds == PASS_GUIDED) {
+        const int g_n = p.set_n[SET_LOGITS];
+        if (!g_n) return fail(e, DSAC_ERR_ARG, "%s: the last forward pass was not guided", who);
+        if (n != g_n) return fail(e, DSAC_ERR_ARG, "%s: n %d differs from the %d frames of the last pass", who, n, g_n);
+        return unchanged();
+    }
+    // the consumers of either pipeline's poses report a stale setting before a missing pass, the backward passes after it
+    if (kinds == PASS_EITHER)
+        if (int rc = unchanged()) return rc;
+    const unsigned held = p.kind == DSAC_PASS_SOFTAM ? PASS_SOFTAM : p.kind == DSAC_PASS_DSAC ? PASS_DSAC : 0;
+    if (n < 1 || p.n != n || !(held & kinds))
+        return fail(e, DSAC_ERR_ARG, "%s must follow %s over the same %d frames", who,
+                    kinds == PASS_SOFTAM ? "a dsac_forward" : kinds == PASS_DSAC ? "a dsac_forward_dsac" : "a forward pass", n);
+    return kinds == PASS_EITHER ? DSAC_OK : unchanged();
+}
+
+// The per-frame camera table and the eye coordinates of the held pass (null: the config's camera, an RGB pass).
+static const Cam* pass_cams(const dsac_engine* e) { return e->pass.set_n[SET_CAMS] ? e->d_cams.get() : nullptr; }
+static const double* pass_eye(const dsac_engine* e) { return e->pass.rgbd() ? e->d_eye.get() : nullptr; }
+
+// The part of RefineParams every refinement shares: the inputs, the permutations, the camera and the thresholds.
+static RefineParams refine_params(const dsac_engine* e, const int16_t* coords, const int32_t* pix, int32_t pix_shared, const Cam* cams) {
+    const dsac_config& c = e->cfg;
+    RefineParams rp;
+    memset(&rp, 0, sizeof(rp));
+    rp.coords = coords; rp.pix = pix; rp.pix_stride = pix_shared ? 0 : DSAC_N * 2;
+    rp.perm = e->d_perm;
+    rp.f = c.focal; rp.cx = c.cx; rp.cy = c.cy; rp.cams = cams;
+    rp.thr = c.thr2d; rp.inlier_count = c.inlier_count; rp.ref_steps = c.ref_steps;
+    return rp;
+}
+// ... over the inputs of the held pass
+static RefineParams pass_refine_params(const dsac_engine* e) {
+    return refine_params(e, e->pass.coords, e->pass.pix, e->pass.pix_shared, pass_cams(e));
+}
+// The part of UncParams the pose queries share, over the inputs of the held pass.
+static UncParams pass_unc_params(const dsac_engine* e) {
+    const dsac_config& c = e->cfg;
+    UncParams up;
+    memset(&up, 0, sizeof(up));
+    up.coords = e->pass.coords; up.pix = e->pass.pix; up.pix_stride = e->pass.pix_shared ? 0 : DSAC_N * 2;
+    up.f = c.focal; up.cx = c.cx; up.cy = c.cy; up.cams = pass_cams(e); up.eye = pass_eye(e);
+    up.thr = (float)c.thr2d;
+    return up;
 }
 
 int dsac_set_sampling_logits_device(dsac_engine* e, int32_t n, const float* d_logits, void* stream_v) {
     if (!e) return DSAC_ERR_ARG;
     if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_set_sampling_logits_device: a submitted pass has not been awaited (dsac_forward_wait)");
+    Setting& s = e->set[SET_LOGITS];
     if (!d_logits) {
-        if (e->g_n) e->g_gen++;
-        e->g_n = 0;
+        setting_clear(s);
         return DSAC_OK;
     }
     if (n < 1 || n > e->cfg.max_frames)
@@ -717,23 +825,20 @@ int dsac_set_sampling_logits_device(dsac_engine* e, int32_t n, const float* d_lo
     CU(e->d_g_q.reserve(cells * sizeof(uint32_t)));
     CU(e->d_g_cum.reserve(cells * sizeof(uint32_t)));
     CU(e->d_g_bad.reserve((size_t)e->cfg.max_frames * sizeof(uint32_t)));
-    CU(cudaStreamWaitEvent(stream, e->ev_fwd, 0));   // the last forward pass may still read the tables
-    e->g_n = 0;                                       // (a failed launch leaves the uniform sampler in force)
-    e->g_gen++;
+    if (int rc = setting_begin(e, s, stream)) return rc;
     k_guided_table<<<(unsigned)n, KG_THREADS, 0, stream>>>(d_logits, e->d_g_w, e->d_g_q, e->d_g_cum, e->d_g_bad);
     e->launches++;
     CU(cudaGetLastError());
-    CU(cudaEventRecord(e->ev_g, stream));
-    e->g_n = n;
-    return DSAC_OK;
+    return setting_commit(e, s, n, stream);
 }
 
 int dsac_sampling_table_device(dsac_engine* e, int32_t n, uint32_t* d_q) {
     if (!e || !d_q) return DSAC_ERR_ARG;
-    if (!e->g_n) return fail(e, DSAC_ERR_ARG, "dsac_sampling_table_device: no sampling logits are set");
-    if (n != e->g_n) return fail(e, DSAC_ERR_ARG, "dsac_sampling_table_device: n %d differs from the %d frames of the setting", n, e->g_n);
+    const Setting& s = e->set[SET_LOGITS];
+    if (!s.n) return fail(e, DSAC_ERR_ARG, "dsac_sampling_table_device: no sampling logits are set");
+    if (n != s.n) return fail(e, DSAC_ERR_ARG, "dsac_sampling_table_device: n %d differs from the %d frames of the setting", n, s.n);
     CU(cudaSetDevice(e->cfg.device));
-    CU(cudaEventSynchronize(e->ev_g));
+    CU(cudaEventSynchronize(s.ev));
     CU(cudaMemcpy(d_q, e->d_g_q, (size_t)n * DSAC_N * sizeof(uint32_t), cudaMemcpyDeviceToDevice));
     return DSAC_OK;
 }
@@ -743,18 +848,14 @@ static int sampling_log_prob_run(dsac_engine* e, const char* who, int32_t n, dou
                                  void* stream_v) {
     if (!e) return DSAC_ERR_ARG;
     if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "%s: a submitted pass has not been awaited (dsac_forward_wait)", who);
-    if (!e->fwd_g_n) return fail(e, DSAC_ERR_ARG, "%s: the last forward pass was not guided", who);
-    if (n != e->fwd_g_n) return fail(e, DSAC_ERR_ARG, "%s: n %d differs from the %d frames of the last pass", who, n, e->fwd_g_n);
-    if (e->fwd_g_gen != e->g_gen) return fail(e, DSAC_ERR_ARG, "%s: the sampling logits were changed after the last pass", who);
-    if (e->fwd_depth_gen != e->depth_gen) return fail(e, DSAC_ERR_ARG, "%s: the cell depth was changed after the last pass", who);
-    if (e->fwd_prior_gen != e->prior_gen) return fail(e, DSAC_ERR_ARG, "%s: the pose priors were changed after the last pass", who);
+    if (int rc = pass_check(e, who, n, PASS_GUIDED, SETTINGS_SAMPLING)) return rc;
     if ((!d_logp && !d_grad_logp) || (d_grad_logp && !d_grad)) return fail(e, DSAC_ERR_ARG, "%s: null output", who);
     cudaStream_t stream = (cudaStream_t)stream_v;
     CU(cudaSetDevice(e->cfg.device));
     CU(cudaStreamWaitEvent(stream, e->ev_fwd, 0));
     GuidedLogpParams g;
     g.w = e->d_g_w; g.cum = e->d_g_cum; g.bad = e->d_g_bad; g.stream_ncand = e->d_stream_ncand;
-    g.T = e->cfg.n_streams; g.seed = e->fwd_seed; g.frame0 = e->cur_frame0;
+    g.T = e->cfg.n_streams; g.seed = e->pass.seed; g.frame0 = e->pass.frame0;
     g.logp = d_logp; g.grad_logp = d_grad_logp; g.grad_logits = d_grad;
     k_guided_logp<<<(unsigned)n, KG_THREADS, 0, stream>>>(g);
     e->launches++;
@@ -775,9 +876,9 @@ int dsac_sampling_log_prob_backward_device(dsac_engine* e, int32_t n, const doub
 int dsac_set_cell_depth_device(dsac_engine* e, int32_t n, const float* d_depth, void* stream_v) {
     if (!e) return DSAC_ERR_ARG;
     if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_set_cell_depth_device: a submitted pass has not been awaited (dsac_forward_wait)");
+    Setting& s = e->set[SET_DEPTH];
     if (!d_depth) {
-        if (e->depth_n) e->depth_gen++;
-        e->depth_n = 0;
+        setting_clear(s);
         return DSAC_OK;
     }
     if (n < 1 || n > e->cfg.max_frames)
@@ -788,13 +889,9 @@ int dsac_set_cell_depth_device(dsac_engine* e, int32_t n, const float* d_depth, 
     CU(e->d_depth.reserve(cells * sizeof(float)));
     CU(e->d_eye.reserve(cells * 3 * sizeof(double)));
     CU(e->d_rgbd_skip.reserve((size_t)e->cfg.max_frames * sizeof(uint32_t)));
-    CU(cudaStreamWaitEvent(stream, e->ev_fwd, 0));   // the last forward pass may still read the buffer
-    e->depth_n = 0;                                   // (a failed copy leaves RGB in force)
-    e->depth_gen++;
+    if (int rc = setting_begin(e, s, stream)) return rc;
     CU(cudaMemcpyAsync(e->d_depth.get(), d_depth, (size_t)n * DSAC_N * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-    CU(cudaEventRecord(e->ev_depth, stream));
-    e->depth_n = n;
-    return DSAC_OK;
+    return setting_commit(e, s, n, stream);
 }
 
 int dsac_set_pose_priors_device(dsac_engine* e, int32_t n, int32_t k, const double* d_poses, const double* d_info, double gate,
@@ -802,9 +899,9 @@ int dsac_set_pose_priors_device(dsac_engine* e, int32_t n, int32_t k, const doub
     if (!e) return DSAC_ERR_ARG;
     static const char* who = "dsac_set_pose_priors_device";
     if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "%s: a submitted pass has not been awaited (dsac_forward_wait)", who);
+    Setting& s = e->set[SET_PRIORS];
     if (!d_poses) {
-        if (e->prior_n) e->prior_gen++;
-        e->prior_n = 0;
+        setting_clear(s);
         return DSAC_OK;
     }
     if (n < 1 || n > e->cfg.max_frames) return fail(e, DSAC_ERR_ARG, "%s: n %d out of range [1,%d]", who, n, e->cfg.max_frames);
@@ -818,32 +915,17 @@ int dsac_set_pose_priors_device(dsac_engine* e, int32_t n, int32_t k, const doub
     CU(e->d_prior_info.reserve(slots * 36 * sizeof(double)));
     CU(e->d_prior_tab.reserve(slots * sizeof(PriorGate)));
     CU(e->d_prior_bad.reserve((size_t)e->cfg.max_frames * sizeof(uint32_t)));
-    if (!e->ev_prior) CU(cudaEventCreateWithFlags(e->ev_prior.put(), cudaEventDisableTiming));
-    CU(cudaStreamWaitEvent(stream, e->ev_fwd, 0));   // the last forward pass may still read the tables
-    e->prior_n = 0;                                   // (a failed copy leaves no priors in force)
-    e->prior_gen++;
+    if (int rc = setting_begin(e, s, stream)) return rc;
     const size_t nk = (size_t)n * k;
     CU(cudaMemcpyAsync(e->d_prior_pose.get(), d_poses, nk * 6 * sizeof(double), cudaMemcpyDeviceToDevice, stream));
     if (d_info) CU(cudaMemcpyAsync(e->d_prior_info.get(), d_info, nk * 36 * sizeof(double), cudaMemcpyDeviceToDevice, stream));
     k_prior_prep<<<(unsigned)n, 32, 0, stream>>>(e->d_prior_pose, d_info ? e->d_prior_info.get() : nullptr, k, e->d_prior_tab, e->d_prior_bad);
     e->launches++;
     CU(cudaGetLastError());
-    CU(cudaEventRecord(e->ev_prior, stream));
-    e->prior_n = n;
+    if (int rc = setting_commit(e, s, n, stream)) return rc;
     e->prior_k = k;
     e->prior_gate = d_info != nullptr;
     e->prior_chi2 = d_info ? gate : 0.0;
-    return DSAC_OK;
-}
-
-// A backward pass differentiates the forward before it, which ran with the cameras and the cell depth in force then.
-static int cameras_unchanged(dsac_engine* e, const char* who) {
-    if (e->fwd_cams_gen != e->cams_gen)
-        return fail(e, DSAC_ERR_ARG, "%s: the cameras were changed (dsac_set_cameras) after the forward pass", who);
-    if (e->fwd_depth_gen != e->depth_gen)
-        return fail(e, DSAC_ERR_ARG, "%s: the cell depth was changed (dsac_set_cell_depth_device) after the forward pass", who);
-    if (e->fwd_prior_gen != e->prior_gen)
-        return fail(e, DSAC_ERR_ARG, "%s: the pose priors were changed (dsac_set_pose_priors_device) after the forward pass", who);
     return DSAC_OK;
 }
 
@@ -944,14 +1026,14 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
     cudaStream_t stream = (cudaStream_t)stream_v;
     const dsac_config& c = e->cfg;
     const size_t o = (size_t)off, Hh = (size_t)c.n_hyps, Nn = DSAC_N;
-    const Cam* cams = e->cams_n ? e->d_cams + o : nullptr;   // per-frame cameras: those of this range's frames
-    const bool guided = e->g_n > 0;                           // guided sampling: this range's frames of the tables
+    // the variant flags of the pass, which index the kernel tables
+    const int cam = e->pass.set_n[SET_CAMS] > 0, guided = e->pass.set_n[SET_LOGITS] > 0, rgbd = e->pass.rgbd();
+    const Cam* cams = cam ? e->d_cams + o : nullptr;          // per-frame cameras: those of this range's frames
     const GuidedGen gg{guided ? e->d_g_cum + o * DSAC_N : nullptr, guided ? e->d_g_bad + o : nullptr};
-    const bool rgbd = e->depth_n > 0;                         // RGB-D pass: this range's frames of the eye coordinates
-    const double* eye = rgbd ? e->d_eye + o * Nn * 3 : nullptr;
+    const double* eye = rgbd ? e->d_eye + o * Nn * 3 : nullptr;   // RGB-D pass: this range's frames of the eye coordinates
     // pose priors: the streams draw n_hyps - prior_k hypotheses into the first slots of each frame, k_prior_inject fills the rest
-    const int prior_k = e->prior_n ? e->prior_k : 0;
-    const bool gate = prior_k > 0 && e->prior_gate;
+    const int prior_k = e->pass.prior_k;
+    const int gate = prior_k > 0 && e->prior_gate;
     const int draw_h = c.n_hyps - prior_k;
 
     if (e->stages & DSAC_STAGE_SAMPLE) {
@@ -960,8 +1042,7 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             const int ps = pix_shared ? 0 : DSAC_N * 2;
             const Cam cam0{c.focal, c.cx, c.cy};
             const uint32_t* gbad = guided ? gg.bad : nullptr;
-            if (cams) k_rgbd_eye_cam<<<(unsigned)n, KE_THREADS, 0, stream>>>(e->d_depth + o * Nn, d_pix, ps, cam0, cams, gbad, e->d_eye + o * Nn * 3, e->d_rgbd_skip + o);
-            else k_rgbd_eye<<<(unsigned)n, KE_THREADS, 0, stream>>>(e->d_depth + o * Nn, d_pix, ps, cam0, nullptr, gbad, e->d_eye + o * Nn * 3, e->d_rgbd_skip + o);
+            k_rgbd_eye_tab[cam]<<<(unsigned)n, KE_THREADS, 0, stream>>>(e->d_depth + o * Nn, d_pix, ps, cam0, cams, gbad, e->d_eye + o * Nn * 3, e->d_rgbd_skip + o);
             e->launches++;
         }
         SampleParams sp;
@@ -980,16 +1061,7 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
         sp.prior_k = gate ? prior_k : 0; sp.prior_chi2 = gate ? e->prior_chi2 : 0.0;
         // the monolithic sampler: the whole pass, or the resume tail of the split sampler's rounds
         auto launch_sample = [&](const SampleParams& s) {
-            const dim3 g(c.n_streams, n);
-            const size_t sm = sizeof(K1Smem);
-            if (gate && rgbd && cams) k_sample_rgbd_cam_gate<<<g, K1_THREADS, sm, stream>>>(s);
-            else if (gate && rgbd) k_sample_rgbd_gate<<<g, K1_THREADS, sm, stream>>>(s);
-            else if (gate && cams) k_sample_cam_gate<<<g, K1_THREADS, sm, stream>>>(s);
-            else if (gate) k_sample_gate<<<g, K1_THREADS, sm, stream>>>(s);
-            else if (rgbd && cams) k_sample_rgbd_cam<<<g, K1_THREADS, sm, stream>>>(s);
-            else if (rgbd) k_sample_rgbd<<<g, K1_THREADS, sm, stream>>>(s);
-            else if (cams) k_sample_cam<<<g, K1_THREADS, sm, stream>>>(s);
-            else k_sample<<<g, K1_THREADS, sm, stream>>>(s);
+            k_sample_tab[cam][rgbd][gate]<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(s);
         };
         if (!e->k1_mode) {
             launch_sample(sp);
@@ -1086,8 +1158,7 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             {
                 // (guided passes read no MT19937 stream: nothing to seed)
                 const int cell_blocks = (int)(((size_t)n * Nn + 255) / 256), seed_blocks = guided ? 0 : (int)((n_slots + 31) / 32);
-                if (cams) k1_cells_cam<<<(unsigned)(cell_blocks + seed_blocks), 256, 0, stream>>>(q, n, seed_blocks);
-                else k1_cells<<<(unsigned)(cell_blocks + seed_blocks), 256, 0, stream>>>(q, n, seed_blocks);
+                k1_cells_tab[cam]<<<(unsigned)(cell_blocks + seed_blocks), 256, 0, stream>>>(q, n, seed_blocks);
             }
             mark(0);
             e->launches++;
@@ -1134,8 +1205,7 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
                             k1_filter<<<fgrid, K1F_THREADS, sizeof(K1FSmem), stream>>>(qf);
                         }
                         mark(1);
-                        if (gate) k1_solve_gate<<<e->k1_solve_grid, K1V_THREADS, 0, stream>>>(qf);
-                        else k1_solve<<<e->k1_solve_grid, K1V_THREADS, 0, stream>>>(qf);
+                        k1_solve_tab[0][gate][0]<<<e->k1_solve_grid, K1V_THREADS, 0, stream>>>(qf);
                         mark(2);
                         e->launches += 2;
                     }
@@ -1175,16 +1245,12 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
                         if (!batch && solve_side != side && set >= 2) CU(cudaStreamWaitEvent(side, k_ev_solve[set - 2], 0));   // the flag-queue region is free again
                     }
                     if (rgbd) {   // the acceptance test writes the accept bits itself: no flag queue, no solve
-                        if (gate && cams) k1_kabsch_cam_gate<<<fgrid, K1F_THREADS, 0, side>>>(q);
-                        else if (gate) k1_kabsch_gate<<<fgrid, K1F_THREADS, 0, side>>>(q);
-                        else if (cams) k1_kabsch_cam<<<fgrid, K1F_THREADS, 0, side>>>(q);
-                        else k1_kabsch<<<fgrid, K1F_THREADS, 0, side>>>(q);
+                        k1_kabsch_tab[cam][gate]<<<fgrid, K1F_THREADS, 0, side>>>(q);
                         if (!overlap) mark(1);
                         e->launches += 2;
                         continue;
                     }
-                    if (cams) k1_filter_cam<<<fgrid, K1F_THREADS, sizeof(K1FSmem), side>>>(q);
-                    else k1_filter<<<fgrid, K1F_THREADS, sizeof(K1FSmem), side>>>(q);
+                    k1_filter_tab[cam]<<<fgrid, K1F_THREADS, sizeof(K1FSmem), side>>>(q);
                     if (!overlap) mark(1);
                     e->launches += 2;
                     if (!solve_now) continue;
@@ -1192,15 +1258,8 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
                         CU(cudaEventRecord(k_ev_filt[set], side));
                         CU(cudaStreamWaitEvent(solve_side, k_ev_filt[set], 0));
                     }
-                    const bool group4 = few && e->k1_solve_group4;
-                    if (gate && cams && group4) k1_solve4_cam_gate<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
-                    else if (gate && cams) k1_solve_cam_gate<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
-                    else if (gate && group4) k1_solve4_gate<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
-                    else if (gate) k1_solve_gate<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
-                    else if (cams && group4) k1_solve4_cam<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
-                    else if (cams) k1_solve_cam<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
-                    else if (group4) k1_solve4<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
-                    else k1_solve<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
+                    const int group4 = few && e->k1_solve_group4;
+                    k1_solve_tab[cam][gate][group4]<<<e->k1_solve_grid, K1V_THREADS, 0, solve_side>>>(q);
                     if (solve_side != side) CU(cudaEventRecord(k_ev_solve[set], solve_side));
                     if (!overlap) mark(2);
                     e->launches++;
@@ -1213,14 +1272,7 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             mark(0);
             sp.resume = q.state;   // streams the rounds left unfinished (normally none) continue in the monolithic kernel
             const dim3 gt(c.n_streams, n);   // ... or in guided steps
-            if (gate && guided && rgbd && cams) k1_gtail_rgbd_cam_gate<<<gt, KG_THREADS, 0, stream>>>(q, gg);
-            else if (gate && guided && rgbd) k1_gtail_rgbd_gate<<<gt, KG_THREADS, 0, stream>>>(q, gg);
-            else if (gate && guided && cams) k1_gtail_cam_gate<<<gt, KG_THREADS, 0, stream>>>(q, gg);
-            else if (gate && guided) k1_gtail_gate<<<gt, KG_THREADS, 0, stream>>>(q, gg);
-            else if (rgbd && guided && cams) k1_gtail_rgbd_cam<<<gt, KG_THREADS, 0, stream>>>(q, gg);
-            else if (rgbd && guided) k1_gtail_rgbd<<<gt, KG_THREADS, 0, stream>>>(q, gg);
-            else if (guided && cams) k1_gtail_cam<<<gt, KG_THREADS, 0, stream>>>(q, gg);
-            else if (guided) k1_gtail<<<gt, KG_THREADS, 0, stream>>>(q, gg);
+            if (guided) k1_gtail_tab[cam][rgbd][gate]<<<gt, KG_THREADS, 0, stream>>>(q, gg);
             else launch_sample(sp);
             mark(3);
             e->launches += 2;
@@ -1256,10 +1308,7 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
         kp.alpha = c.alpha;
         kp.external_scores = 0;
         dim3 grid(kp.tiles_per_frame, n);
-        if (cams && e->d_diffmaps) k_score_cam<true><<<grid, K2_THREADS, 0, stream>>>(kp);
-        else if (cams) k_score_cam<false><<<grid, K2_THREADS, 0, stream>>>(kp);
-        else if (e->d_diffmaps) k_score<true><<<grid, K2_THREADS, 0, stream>>>(kp);
-        else k_score<false><<<grid, K2_THREADS, 0, stream>>>(kp);
+        k_score_tab[cam][e->d_diffmaps.get() != nullptr]<<<grid, K2_THREADS, 0, stream>>>(kp);
         e->launches++;
         CU(cudaGetLastError());
         if (e->hook) {
@@ -1275,12 +1324,7 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
         }
     }
     if (e->stages & DSAC_STAGE_REFINE) {
-        RefineParams rp;
-        memset(&rp, 0, sizeof(rp));
-        rp.coords = d_coords; rp.pix = d_pix; rp.pix_stride = pix_shared ? 0 : DSAC_N * 2;
-        rp.perm = e->d_perm;
-        rp.f = c.focal; rp.cx = c.cx; rp.cy = c.cy; rp.cams = cams;
-        rp.thr = c.thr2d; rp.inlier_count = c.inlier_count; rp.ref_steps = c.ref_steps;
+        RefineParams rp = refine_params(e, d_coords, d_pix, pix_shared, cams);
         rp.n_jobs = n;
         rp.job_init = e->d_avg + o * 6;
         rp.out_pose = e->d_ref + o * 6;
@@ -1351,15 +1395,7 @@ int dsac_forward_device(dsac_engine* e, int32_t n, int64_t frame0, const int16_t
     if (n < 1 || n > e->cfg.max_frames) return fail(e, DSAC_ERR_CAPACITY, "n_frames %d exceeds engine capacity %d", n, e->cfg.max_frames);
     if (!d_coords || !d_pix) return fail(e, DSAC_ERR_ARG, "null input");
     CU(cudaSetDevice(e->cfg.device));
-    if (int rc = cameras_begin_pass(e, n, (cudaStream_t)stream_v)) return rc;
-    e->cur_coords = d_coords;
-    e->cur_pix = d_pix;
-    e->cur_pix_shared = pix_shared;
-    e->cur_gt = d_gt_jp;
-    e->cur_n = n;
-    e->fwd_stages = e->stages;
-    e->dsac_n = 0;
-    e->cur_frame0 = frame0;
+    if (int rc = pass_begin(e, DSAC_PASS_SOFTAM, n, frame0, d_coords, d_pix, pix_shared, d_gt_jp, {(cudaStream_t)stream_v})) return rc;
     if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_forward_device: a submitted pass has not been awaited (dsac_forward_wait)");
     int rc = forward_split(e, n, frame0, d_coords, d_pix, pix_shared, d_gt_jp, (cudaStream_t)stream_v, true);
     if (rc != DSAC_OK) return rc;
@@ -1445,17 +1481,10 @@ static int forward_submit_impl(dsac_engine* e, int32_t n, int64_t frame0, const 
     if (n < 1 || n > e->cfg.max_frames) return fail(e, DSAC_ERR_CAPACITY, "n_frames %d exceeds engine capacity %d", n, e->cfg.max_frames);
     if (!coords || !pix) return fail(e, DSAC_ERR_ARG, "null input");
     CU(cudaSetDevice(e->cfg.device));
-    for (int c = 0; c < 4; c++)   // (every chunk's stream: DSAC_PIPE_CHUNKS)
-        if (int rc = cameras_begin_pass(e, n, e->pipe[c])) return rc;
+    if (int rc = pass_begin(e, DSAC_PASS_SOFTAM, n, frame0, e->d_coords, e->d_pix, pix_shared, gt_jp ? e->d_gt.get() : nullptr,
+                            {e->pipe[0], e->pipe[1], e->pipe[2], e->pipe[3]}))   // (every chunk's stream: DSAC_PIPE_CHUNKS)
+        return rc;
     const size_t N = DSAC_N;
-    e->cur_coords = e->d_coords;
-    e->cur_pix = e->d_pix;
-    e->cur_pix_shared = pix_shared;
-    e->cur_gt = gt_jp ? e->d_gt.get() : nullptr;
-    e->cur_n = n;
-    e->fwd_stages = e->stages;
-    e->dsac_n = 0;
-    e->cur_frame0 = frame0;
     // Frames are independent, so the batch is cut into up to 4 chunks, each on its own stream:
     // H2D(chunk) -> K1 -> K2 -> K4 -> D2H(chunk).  Copies of later chunks overlap the kernels of earlier
     // ones and the tail of one chunk's kernels is filled by the next chunk's CTAs.
@@ -1555,7 +1584,8 @@ static int forward_dsac_run(dsac_engine* e, int32_t n, int64_t frame0, const int
     if (!d_coords || !d_pix) return fail(e, DSAC_ERR_ARG, "null input");
     const dsac_config& c = e->cfg;
     CU(cudaSetDevice(c.device));
-    if (int rc = cameras_begin_pass(e, n, stream)) return rc;
+    // the record holds no pass until this one is complete: the soft-argmax backward does not apply to it
+    if (int rc = pass_begin(e, 0, n, frame0, d_coords, d_pix, pix_shared, d_gt, {stream})) return rc;
     const size_t N = DSAC_N, nn = (size_t)n, H = c.n_hyps, jobs = nn * H;
     // refine-all buffers: they grow together, and the job -> frame table is written whenever they do
     if (jobs > e->ra_jobs) {
@@ -1573,10 +1603,6 @@ static int forward_dsac_run(dsac_engine* e, int32_t n, int64_t frame0, const int
         e->ra_jobs = jobs;
     }
     if (want_imaps) CU(e->d_ra_imap.reserve(jobs * N * sizeof(int32_t)));
-    e->cur_coords = d_coords; e->cur_pix = d_pix; e->cur_pix_shared = pix_shared; e->cur_gt = d_gt;
-    e->cur_n = 0;   // the soft-argmax backward does not apply to this pass
-    e->dsac_n = 0;
-    e->cur_frame0 = frame0;
     const uint32_t saved = e->stages;
     e->stages = DSAC_STAGE_SAMPLE | DSAC_STAGE_SCORE;
     int rc = forward_range(e, 0, n, frame0, d_coords, d_pix, pix_shared, d_gt, stream);
@@ -1589,12 +1615,7 @@ static int forward_dsac_run(dsac_engine* e, int32_t n, int64_t frame0, const int
         CU(cudaMemsetAsync(e->d_ra_correct, 0, jobs * sizeof(int32_t), stream));
     }
     {   // every hypothesis is a refinement job starting from its own pose (cnn.h:1155-1218)
-        RefineParams rp;
-        memset(&rp, 0, sizeof(rp));
-        rp.coords = d_coords; rp.pix = d_pix; rp.pix_stride = pix_shared ? 0 : DSAC_N * 2;
-        rp.perm = e->d_perm;
-        rp.f = c.focal; rp.cx = c.cx; rp.cy = c.cy; rp.cams = e->cams_n ? e->d_cams.get() : nullptr;
-        rp.thr = c.thr2d; rp.inlier_count = c.inlier_count; rp.ref_steps = c.ref_steps;
+        RefineParams rp = pass_refine_params(e);
         rp.n_jobs = (int)jobs;
         rp.job_frame = e->d_ra_frame;
         rp.job_init = e->d_hyp_pose;
@@ -1605,7 +1626,7 @@ static int forward_dsac_run(dsac_engine* e, int32_t n, int64_t frame0, const int
             rp.gt_jp = d_gt;
             rp.loss = e->d_ra_loss; rp.rot_err = e->d_ra_rot; rp.t_err = e->d_ra_t; rp.correct = e->d_ra_correct;
         }
-        launch_refine(rp, (unsigned)jobs, stream, e->depth_n ? e->d_eye.get() : nullptr);
+        launch_refine(rp, (unsigned)jobs, stream, pass_eye(e));
         e->launches++;
         CU(cudaGetLastError());
     }
@@ -1623,7 +1644,7 @@ static int forward_dsac_run(dsac_engine* e, int32_t n, int64_t frame0, const int
         CU(cudaGetLastError());
     }
     CU(cudaEventRecord(e->ev_fwd, stream));   // the backward waits on this
-    e->dsac_n = n;
+    e->pass.kind = DSAC_PASS_DSAC;
     return DSAC_OK;
 }
 
@@ -1719,16 +1740,11 @@ int dsac_refined_jp6_device(dsac_engine* e, int32_t n, double* d_jp6, void* stre
     if (!e) return DSAC_ERR_ARG;
     if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_refined_jp6_device: a submitted pass has not been awaited (dsac_forward_wait)");
     if (!d_jp6) return fail(e, DSAC_ERR_ARG, "dsac_refined_jp6_device: null output");
-    if (int rc = cameras_unchanged(e, "dsac_refined_jp6_device")) return rc;
-    const double* pose;
-    size_t count;
-    if (n >= 1 && e->cur_n == n && e->cur_coords) {   // soft-argmax pass: one refined pose per frame
-        pose = e->d_ref; count = (size_t)n;
-    } else if (n >= 1 && e->dsac_n == n) {            // DSAC-variant pass: every hypothesis refined
-        pose = e->d_ra_pose; count = (size_t)n * e->cfg.n_hyps;
-    } else {
-        return fail(e, DSAC_ERR_ARG, "dsac_refined_jp6_device must follow a forward pass over the same %d frames", n);
-    }
+    if (int rc = pass_check(e, "dsac_refined_jp6_device", n, PASS_EITHER, SETTINGS_GEOMETRY)) return rc;
+    // a soft-argmax pass refines one pose per frame, the DSAC variant every hypothesis
+    const bool dsac = e->pass.kind == DSAC_PASS_DSAC;
+    const double* pose = dsac ? e->d_ra_pose.get() : e->d_ref.get();
+    const size_t count = (size_t)n * (dsac ? e->cfg.n_hyps : 1);
     CU(cudaSetDevice(e->cfg.device));
     cudaStream_t stream = (cudaStream_t)stream_v;
     CU(cudaStreamWaitEvent(stream, e->ev_fwd, 0));
@@ -2063,6 +2079,33 @@ int dsac_score_maps_device(dsac_engine* e, int32_t n_images, int32_t hyps_per_im
 }
 
 }  // extern "C"
+
+// One grow-only scratch block of views, each at 256-byte alignment, in the order given: the block grows to hold them,
+// then every view points at its slice.  ev (nullable): the block's last user, on any stream -- the host waits for it
+// before the block is re-allocated, `stream` otherwise.
+struct ScratchView {
+    size_t bytes;
+    void* view;
+    void (*set)(void* view, char* at);
+};
+template <class T> static ScratchView view(T*& v, size_t count) {
+    return {count * sizeof(T), &v, [](void* w, char* at) { *static_cast<T**>(w) = reinterpret_cast<T*>(at); }};
+}
+static int carve_scratch(dsac_engine* e, DevMem<char>& buf, std::initializer_list<ScratchView> views, cudaEvent_t ev = nullptr,
+                         cudaStream_t stream = nullptr) {
+    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    size_t total = 0;
+    for (const ScratchView& v : views) total += al(v.bytes);
+    if (ev && total > buf.bytes()) CU(cudaEventSynchronize(ev));
+    else if (ev) CU(cudaStreamWaitEvent(stream, ev, 0));
+    CU(buf.reserve(total));
+    char* p = buf;
+    for (const ScratchView& v : views) {
+        v.set(v.view, p);
+        p += al(v.bytes);
+    }
+    return DSAC_OK;
+}
 
 #include "backward_host.inc"
 #include "backward_dsac_host.inc"

@@ -166,14 +166,6 @@ __global__ void __launch_bounds__(KG_THREADS) k1_gtail_t(K1SplitParams q, Guided
         }
     }
 }
-constexpr auto k1_gtail = k1_gtail_t<false>;
-constexpr auto k1_gtail_cam = k1_gtail_t<true>;
-constexpr auto k1_gtail_rgbd = k1_gtail_t<false, true>;
-constexpr auto k1_gtail_rgbd_cam = k1_gtail_t<true, true>;
-constexpr auto k1_gtail_gate = k1_gtail_t<false, false, true>;
-constexpr auto k1_gtail_cam_gate = k1_gtail_t<true, false, true>;
-constexpr auto k1_gtail_rgbd_gate = k1_gtail_t<false, true, true>;
-constexpr auto k1_gtail_rgbd_cam_gate = k1_gtail_t<true, true, true>;
 
 struct GuidedLogpParams {
     const double* w;                 // [n][N] softmax of the logits

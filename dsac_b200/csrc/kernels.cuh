@@ -740,15 +740,6 @@ __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS) k_sample_t(SamplePa
     }
 }
 
-constexpr auto k_sample = k_sample_t<false>;
-constexpr auto k_sample_cam = k_sample_t<true>;
-constexpr auto k_sample_rgbd = k_sample_t<false, true>;
-constexpr auto k_sample_rgbd_cam = k_sample_t<true, true>;
-constexpr auto k_sample_gate = k_sample_t<false, false, true>;
-constexpr auto k_sample_cam_gate = k_sample_t<true, false, true>;
-constexpr auto k_sample_rgbd_gate = k_sample_t<false, true, true>;
-constexpr auto k_sample_rgbd_cam_gate = k_sample_t<true, true, true>;
-
 // ------------------------------------------------------------------ K2: fused scoring
 struct ScoreParams {
     const int16_t* coords;   // [n][N][3]

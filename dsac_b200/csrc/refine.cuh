@@ -432,19 +432,21 @@ __global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine_rgbd_rec_c
     k_refine_body<true, true, true>(p, eye, rec_sel, rec_count);
 }
 
+// the instantiations by per-frame camera (RefineParams::cams), one table per signature
+constexpr void (*k_refine_tab[2])(RefineParams) = {k_refine, k_refine_cam};
+constexpr void (*k_refine_rgbd_tab[2])(RefineParams, const double*) = {k_refine_rgbd, k_refine_rgbd_cam};
+constexpr void (*k_refine_rec_tab[2])(RefineParams, uint16_t*, int32_t*) = {k_refine_rec, k_refine_rec_cam};
+constexpr void (*k_refine_rgbd_rec_tab[2])(RefineParams, const double*, uint16_t*, int32_t*) = {k_refine_rgbd_rec, k_refine_rgbd_rec_cam};
+
 // one CTA per job, with the instantiation the parameters ask for; eye != null: an RGB-D pass
 inline void launch_refine(const RefineParams& p, unsigned jobs, cudaStream_t stream, const double* eye = nullptr) {
-    if (eye && p.cams) k_refine_rgbd_cam<<<jobs, K4_THREADS, 0, stream>>>(p, eye);
-    else if (eye) k_refine_rgbd<<<jobs, K4_THREADS, 0, stream>>>(p, eye);
-    else if (p.cams) k_refine_cam<<<jobs, K4_THREADS, 0, stream>>>(p);
-    else k_refine<<<jobs, K4_THREADS, 0, stream>>>(p);
+    if (eye) k_refine_rgbd_tab[p.cams != nullptr]<<<jobs, K4_THREADS, 0, stream>>>(p, eye);
+    else k_refine_tab[p.cams != nullptr]<<<jobs, K4_THREADS, 0, stream>>>(p);
 }
 inline void launch_refine_record(const RefineParams& p, unsigned jobs, cudaStream_t stream, const double* eye, uint16_t* rec_sel,
                                  int32_t* rec_count) {
-    if (eye && p.cams) k_refine_rgbd_rec_cam<<<jobs, K4_THREADS, 0, stream>>>(p, eye, rec_sel, rec_count);
-    else if (eye) k_refine_rgbd_rec<<<jobs, K4_THREADS, 0, stream>>>(p, eye, rec_sel, rec_count);
-    else if (p.cams) k_refine_rec_cam<<<jobs, K4_THREADS, 0, stream>>>(p, rec_sel, rec_count);
-    else k_refine_rec<<<jobs, K4_THREADS, 0, stream>>>(p, rec_sel, rec_count);
+    if (eye) k_refine_rgbd_rec_tab[p.cams != nullptr]<<<jobs, K4_THREADS, 0, stream>>>(p, eye, rec_sel, rec_count);
+    else k_refine_rec_tab[p.cams != nullptr]<<<jobs, K4_THREADS, 0, stream>>>(p, rec_sel, rec_count);
 }
 
 }  // namespace dsac

@@ -43,7 +43,5 @@ __global__ void __launch_bounds__(KE_THREADS) k_rgbd_eye_t(const float* __restri
     __syncthreads();
     if (threadIdx.x == 0) skip[frame] = (s_have < 4 ? ST_NO_DEPTH : 0u) | ((gbad && gbad[frame]) ? 32u /* DSAC_ST_BAD_WEIGHTS */ : 0u);
 }
-constexpr auto k_rgbd_eye = k_rgbd_eye_t<false>;
-constexpr auto k_rgbd_eye_cam = k_rgbd_eye_t<true>;
 
 }  // namespace dsac

@@ -1594,10 +1594,6 @@ __global__ void __launch_bounds__(K1F_THREADS) k1_kabsch_t(K1SplitParams q) {
         }
     }
 }
-constexpr auto k1_kabsch = k1_kabsch_t<false>;
-constexpr auto k1_kabsch_cam = k1_kabsch_t<true>;
-constexpr auto k1_kabsch_gate = k1_kabsch_t<false, true>;
-constexpr auto k1_kabsch_cam_gate = k1_kabsch_t<true, true>;
 
 // The generator is camera-free: the selection of k1_slot writes the rows (fR0 ft0), (fR1 ft1) of hyp_P with the engine's
 // focal length.  With a per-frame camera table this kernel, launched after the sampler, writes them again from the

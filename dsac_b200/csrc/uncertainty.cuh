@@ -122,10 +122,9 @@ __global__ void __launch_bounds__(UNC_THREADS) k_pose_uncertainty_rgbd(UncParams
 __global__ void __launch_bounds__(UNC_THREADS) k_pose_uncertainty_rgbd_cam(UncParams p) { k_pose_uncertainty_body<true, true>(p); }
 
 inline void launch_pose_uncertainty(const UncParams& p, unsigned jobs, cudaStream_t stream) {
-    if (p.eye && p.cams) k_pose_uncertainty_rgbd_cam<<<jobs, UNC_THREADS, 0, stream>>>(p);
-    else if (p.eye) k_pose_uncertainty_rgbd<<<jobs, UNC_THREADS, 0, stream>>>(p);
-    else if (p.cams) k_pose_uncertainty_cam<<<jobs, UNC_THREADS, 0, stream>>>(p);
-    else k_pose_uncertainty<<<jobs, UNC_THREADS, 0, stream>>>(p);
+    // [per-frame camera][RGB-D]
+    constexpr void (*tab[2][2])(UncParams) = {{k_pose_uncertainty, k_pose_uncertainty_rgbd}, {k_pose_uncertainty_cam, k_pose_uncertainty_rgbd_cam}};
+    tab[p.cams != nullptr][p.eye != nullptr]<<<jobs, UNC_THREADS, 0, stream>>>(p);
 }
 
 }  // namespace dsac
