@@ -362,6 +362,44 @@ def pose_modes(engine, n, max_modes, rot_rad, trans_mm):
     return out
 
 
+def rig_pose(engine, prediction, pix, cam_from_rig, n_cameras, frame0=0, cameras=None, sampling_logits=None, gt_jp=None):
+    """One pose per multi-camera rig (INTEGRATION.md, "Multi-camera rigs"): the n frames of `prediction` are R = n / C rigs
+    of C = n_cameras cameras, frame r C + c camera c of rig r, whose extrinsic cam_from_rig[r C + c] (float64 [n][6], a cv
+    pose: X_cam = R_c X_rig + t_c) is known.  cameras and sampling_logits as in softam_pose, per frame; gt_jp float64
+    [R][12] (the jp pose of the rig frame) adds loss, rot_err, t_err and correct.  A dict of device tensors on
+    torch.cuda.current_stream(), without autograd history: hyp_pose [n][H][6]; rig_hyp [R][C H][6], scores and sf
+    [R][C H]; entropy [R]; avg_pose and ref_pose [R][6] (cv poses of the rig); inlier_map int32 [n][1600]; steps_done int32,
+    status int32 [R]; and with gt_jp loss, rot_err, t_err float64 and correct int32 [R]."""
+    C = int(n_cameras)
+    n, pix, _, shared = _check_inputs(engine, prediction, pix, None, need_gt=False)
+    dev = prediction.device
+    if not 1 <= C <= _E.MAX_RIG_CAMERAS or n % C:
+        raise ValueError("n_cameras %d must be in [1, %d] and divide the %d frames" % (C, _E.MAX_RIG_CAMERAS, n))
+    R, H = n // C, engine.cfg.n_hyps
+    if cam_from_rig.dtype != torch.float64 or cam_from_rig.numel() != n * 6 or cam_from_rig.device != dev:
+        raise ValueError("cam_from_rig must be float64 [%d][6] on %s" % (n, dev))
+    if gt_jp is not None and (gt_jp.dtype != torch.float64 or gt_jp.numel() != R * 12 or gt_jp.device != dev):
+        raise ValueError("gt_jp must be float64 [%d][12] on %s" % (R, dev))
+    _set_cameras(engine, prediction, cameras)
+    _set_sampling(engine, prediction, sampling_logits)
+    stream = torch.cuda.current_stream(dev).cuda_stream
+    coords = _coords(engine, prediction.detach().contiguous(), stream)
+    ext = cam_from_rig.detach().contiguous()
+    gt = gt_jp.detach().contiguous() if gt_jp is not None else None
+    f64 = dict(dtype=torch.float64, device=dev)
+    i32 = dict(dtype=torch.int32, device=dev)
+    out = {"hyp_pose": torch.empty((n, H, 6), **f64), "rig_hyp": torch.empty((R, C * H, 6), **f64),
+           "scores": torch.empty((R, C * H), **f64), "sf": torch.empty((R, C * H), **f64), "entropy": torch.empty((R,), **f64),
+           "avg_pose": torch.empty((R, 6), **f64), "ref_pose": torch.empty((R, 6), **f64),
+           "inlier_map": torch.empty((n, _E.N), **i32), "steps_done": torch.empty((R,), **i32), "status": torch.empty((R,), **i32)}
+    if gt is not None:
+        out.update(loss=torch.empty((R,), **f64), rot_err=torch.empty((R,), **f64), t_err=torch.empty((R,), **f64),
+                   correct=torch.empty((R,), **i32))
+    engine.forward_rig_device(n, C, coords.data_ptr(), pix.data_ptr(), ext.data_ptr(), shared, gt.data_ptr() if gt is not None else None,
+                              int(frame0), stream, **{k: v.data_ptr() for k, v in out.items()})
+    return out
+
+
 class _SamplingLogProb(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logits, engine):

@@ -28,6 +28,7 @@
 #include "train.cuh"
 #include "uncertainty.cuh"
 #include "modes.cuh"
+#include "rig.cuh"
 #include "upstream.cuh"
 #include "objtrain.cuh"
 #include "scoretrain.cuh"
@@ -37,6 +38,8 @@ using namespace dsac;
 static_assert(sizeof(Cam) == sizeof(dsac_camera), "Cam mirrors dsac_camera");
 static_assert(PRIOR_MAX == DSAC_MAX_PRIORS && PRIOR_ST_BAD == DSAC_ST_BAD_PRIOR, "prior.cuh mirrors dsac_b200.h");
 static_assert(MODE_MAX == DSAC_MAX_MODES && DSAC_MAX_HYPS <= 1024, "modes.cuh mirrors dsac_b200.h");
+static_assert(RIG_MAX_CAMERAS == DSAC_MAX_RIG_CAMERAS && RIG_ST_BAD == DSAC_ST_BAD_RIG && DSAC_MAX_HYPS <= 2048,
+              "refine.cuh mirrors dsac_b200.h (a rig's selection codes a cell in 11 bits)");
 static_assert(sizeof(ObjCam) == sizeof(dsac_rgbd_camera) && offsetof(ObjCam, sensor_trans) == offsetof(dsac_rgbd_camera, sensor_trans) &&
                   offsetof(ObjCam, raw_data) == offsetof(dsac_rgbd_camera, raw_data),
               "ObjCam mirrors dsac_rgbd_camera");
@@ -61,6 +64,7 @@ static constexpr void (*k1_cells_tab[2])(K1SplitParams, int, int) = {k1_cells, k
 static constexpr void (*k_rgbd_eye_tab[2])(const float*, const int32_t*, int, Cam, const Cam*, const uint32_t*, double*, uint32_t*) = {
     k_rgbd_eye_t<false>, k_rgbd_eye_t<true>};
 static constexpr void (*k_score_tab[2][2])(ScoreParams) = {{k_score<false>, k_score<true>}, {k_score_cam<false>, k_score_cam<true>}};
+static constexpr void (*k_score_rig_tab[2])(ScoreParams) = {k_score_rig<false>, k_score_rig<true>};
 
 // Owners of the engine's CUDA resources, the only code here that frees any.  Each releases what it holds in its
 // destructor, is move-only, and converts to the raw pointer or handle for use at call sites.
@@ -139,7 +143,7 @@ struct Setting {
 // The forward pass the engine holds, which the backward passes and the pose queries read: its inputs and the snapshot
 // of the settings it ran with.
 struct Pass {
-    int32_t kind = 0;               // DSAC_PASS_SOFTAM, DSAC_PASS_DSAC, or 0: none
+    int32_t kind = 0;               // DSAC_PASS_SOFTAM, DSAC_PASS_DSAC, DSAC_PASS_RIG, or 0: none
     int n = 0;
     const int16_t* coords = nullptr;
     const int32_t* pix = nullptr;
@@ -255,6 +259,15 @@ struct dsac_engine {
     // ev_modes as the uncertainty scratch is by ev_unc
     DevMem<char> modes_buf;
     Event ev_modes;
+    // dsac_forward_rig_device: the extrinsics, the pool, its rows and scores and the per-rig results, views into rig_buf
+    // (grow-only, sized for max_frames frames of the largest pool asked for)
+    struct {
+        double *ext, *cam_scores, *hyp, *scores, *sf, *entropy, *avg, *ref, *loss, *rot, *terr;
+        float* P;
+        int32_t *imap, *steps, *correct;
+        uint32_t* status;
+    } rig = {};
+    DevMem<char> rig_buf;
     std::vector<DevMem<char>> bw_pool;   // device buffers of dsac_backward_dsac, kept across calls
     Stream pipe[4];                 // chunked H2D / compute / D2H pipeline of dsac_forward
     // tail split (dsac_set_tail_split): the whole sampler waves of a batch run on a high-priority side stream, the
@@ -520,6 +533,7 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
     for (int cam = 0; cam < 2; cam++) {
         CUC(cudaFuncSetAttribute(k_refine_tab[cam], cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
         CUC(cudaFuncSetAttribute(k_refine_rgbd_tab[cam], cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+        CUC(cudaFuncSetAttribute(k_refine_rig_tab[cam], cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
         if (const char* co = getenv("DSAC_K1_CARVEOUT"))
             CUC(cudaFuncSetAttribute(k_sample_tab[cam][0][0], cudaFuncAttributePreferredSharedMemoryCarveout, atoi(co)));
     }
@@ -1007,8 +1021,8 @@ static int seam_backward(dsac_engine* e, int n, const double* d_sog, cudaStream_
     return DSAC_OK;
 }
 
-static int pick_tile(const dsac_engine* e, int n_frames) {
-    int H = e->cfg.n_hyps, t = e->cfg.hyps_per_cta;
+static int pick_tile(const dsac_engine* e, int n_frames, int H) {
+    int t = e->cfg.hyps_per_cta;
     if (t <= 0) {
         // enough CTAs to fill the chip a few times over, but no smaller than 8 hypotheses
         t = 64;
@@ -1019,10 +1033,10 @@ static int pick_tile(const dsac_engine* e, int n_frames) {
     return t;
 }
 
-// Launches the forward stages for `n` frames whose per-frame engine buffers start at frame offset `off`
-// (inputs are passed already offset).  Used whole (off = 0) and per chunk by the pipelined host path.
+// Launches the forward stages `stages` (DSAC_STAGE_*) for `n` frames whose per-frame engine buffers start at frame offset
+// `off` (inputs are passed already offset).  Used whole (off = 0) and per chunk by the pipelined host path.
 static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0, const int16_t* d_coords, const int32_t* d_pix,
-                         int32_t pix_shared, const double* d_gt_jp, void* stream_v, int lane = 0) {
+                         int32_t pix_shared, const double* d_gt_jp, void* stream_v, uint32_t stages, int lane = 0) {
     cudaStream_t stream = (cudaStream_t)stream_v;
     const dsac_config& c = e->cfg;
     const size_t o = (size_t)off, Hh = (size_t)c.n_hyps, Nn = DSAC_N;
@@ -1036,7 +1050,7 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
     const int gate = prior_k > 0 && e->prior_gate;
     const int draw_h = c.n_hyps - prior_k;
 
-    if (e->stages & DSAC_STAGE_SAMPLE) {
+    if (stages & DSAC_STAGE_SAMPLE) {
         CU(cudaMemsetAsync(e->d_status + o, 0, (size_t)n * sizeof(uint32_t), stream));
         if (rgbd) {
             const int ps = pix_shared ? 0 : DSAC_N * 2;
@@ -1293,14 +1307,14 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             CU(cudaGetLastError());
         }
     }
-    if (e->stages & DSAC_STAGE_SCORE) {
+    if (stages & DSAC_STAGE_SCORE) {
         ScoreParams kp;
         kp.coords = d_coords; kp.pix = d_pix; kp.pix_stride = pix_shared ? 0 : DSAC_N * 2;
         kp.hyp_P = e->d_hyp_P + o * Hh * 12; kp.hyp_pose = e->d_hyp_pose + o * Hh * 6;
         kp.diffmaps = e->d_diffmaps ? e->d_diffmaps + o * Hh * Nn : nullptr; kp.scores = e->d_scores + o * Hh; kp.sf = e->d_sf + o * Hh; kp.entropy = e->d_entropy + o;
         kp.avg_pose = e->d_avg + o * 6; kp.frame_counter = e->d_frame_counter + o;
         kp.H = c.n_hyps;
-        kp.tile = pick_tile(e, n);
+        kp.tile = pick_tile(e, n, c.n_hyps);
         kp.tiles_per_frame = (c.n_hyps + kp.tile - 1) / kp.tile;
         kp.cxf = (float)c.cx; kp.cyf = (float)c.cy; kp.cams = cams;
         kp.thr = (float)c.thr2d;
@@ -1323,14 +1337,14 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             CU(cudaGetLastError());
         }
     }
-    if (e->stages & DSAC_STAGE_REFINE) {
+    if (stages & DSAC_STAGE_REFINE) {
         RefineParams rp = refine_params(e, d_coords, d_pix, pix_shared, cams);
         rp.n_jobs = n;
         rp.job_init = e->d_avg + o * 6;
         rp.out_pose = e->d_ref + o * 6;
         rp.inlier_map = e->d_inlier_map + o * Nn; rp.steps_done = e->d_steps_done + o; rp.n_perm_steps = e->d_n_perm + o;
         rp.status = e->d_status + o;
-        if ((e->stages & DSAC_STAGE_EVAL) && d_gt_jp) {
+        if ((stages & DSAC_STAGE_EVAL) && d_gt_jp) {
             rp.gt_jp = d_gt_jp;
             rp.loss = e->d_loss + o; rp.rot_err = e->d_rot_err + o; rp.t_err = e->d_t_err + o; rp.correct = e->d_correct + o;
         }
@@ -1348,9 +1362,10 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
 // then run next to the partial wave.  Fork / join with events, so for the caller everything still happens in
 // stream order on `stream`.  Frames are independent (disjoint slices of every engine buffer).
 static int forward_split(dsac_engine* e, int32_t n, int64_t frame0, const int16_t* d_coords, const int32_t* d_pix,
-                         int32_t pix_shared, const double* d_gt_jp, cudaStream_t stream, bool allow_split) {
+                         int32_t pix_shared, const double* d_gt_jp, cudaStream_t stream, bool allow_split, uint32_t stages) {
     int32_t n1 = 0;
-    if (allow_split && e->tail_split && !e->k1_mode && (e->stages & DSAC_STAGE_SAMPLE) && (e->stages & ~DSAC_STAGE_SAMPLE) && !e->hook) {
+    // (the tail split overlaps the later stages of the whole waves with the partial wave's sampler: it needs later stages)
+    if (allow_split && e->tail_split && !e->k1_mode && (stages & DSAC_STAGE_SAMPLE) && (stages & ~DSAC_STAGE_SAMPLE) && !e->hook) {
         const int per_wave = e->k1_slots / std::max(1, e->cfg.n_streams);   // frames per sampler wave
         if (per_wave >= 1 && n > per_wave && n % per_wave != 0) n1 = (n / per_wave) * per_wave;
     }
@@ -1361,30 +1376,30 @@ static int forward_split(dsac_engine* e, int32_t n, int64_t frame0, const int16_
     // the 50/50 split (40/60: 3.13 / 3.21 ms); tools/lane_probe.py compares more lanes.  Frames are independent and sampler streams keyed by the global frame index, so
     // results do not depend on the split.
     if (allow_split && e->k1_mode && e->k1_lanes && n >= 768 && e->lane1.main && !e->k1_profile && !e->d_k1_dbg && !e->k1_fused &&
-        !e->hook && (e->stages & DSAC_STAGE_SAMPLE)) {
+        !e->hook && (stages & DSAC_STAGE_SAMPLE)) {
         int32_t na = n / 2;
         if (const char* lf = getenv("DSAC_K1_LANE_FRAC")) na = std::max(1, std::min(n - 1, (int32_t)(atof(lf) * n)));   // development aid
         const size_t N = DSAC_N, f = (size_t)na;
         CU(cudaEventRecord(e->ev_fork, stream));
         CU(cudaStreamWaitEvent(e->lane1.main, e->ev_fork, 0));
         int rc = forward_range(e, na, n - na, frame0 + na, d_coords + f * N * 3, pix_shared ? d_pix : d_pix + f * N * 2, pix_shared,
-                               d_gt_jp ? d_gt_jp + f * 12 : nullptr, e->lane1.main, 1);
+                               d_gt_jp ? d_gt_jp + f * 12 : nullptr, e->lane1.main, stages, 1);
         cudaEventRecord(e->ev_join, e->lane1.main);   // the caller's stream joins the lane again whatever happens below
-        if (rc == DSAC_OK) rc = forward_range(e, 0, na, frame0, d_coords, d_pix, pix_shared, d_gt_jp, stream, 0);
+        if (rc == DSAC_OK) rc = forward_range(e, 0, na, frame0, d_coords, d_pix, pix_shared, d_gt_jp, stream, stages, 0);
         CU(cudaStreamWaitEvent(stream, e->ev_join, 0));
         return rc;
     }
-    if (n1 <= 0) return forward_range(e, 0, n, frame0, d_coords, d_pix, pix_shared, d_gt_jp, stream);
+    if (n1 <= 0) return forward_range(e, 0, n, frame0, d_coords, d_pix, pix_shared, d_gt_jp, stream, stages);
     const size_t N = DSAC_N, f = (size_t)n1;
     CU(cudaEventRecord(e->ev_fork, stream));
     CU(cudaStreamWaitEvent(e->hi, e->ev_fork, 0));
-    int rc = forward_range(e, 0, n1, frame0, d_coords, d_pix, pix_shared, d_gt_jp, e->hi);
+    int rc = forward_range(e, 0, n1, frame0, d_coords, d_pix, pix_shared, d_gt_jp, e->hi, stages);
     // whatever happens below, the caller's stream joins the side stream again: nothing may still be writing engine
     // buffers on e->hi when the caller sees this call's work as complete (or its error)
     cudaEventRecord(e->ev_join, e->hi);
     if (rc == DSAC_OK)
         rc = forward_range(e, n1, n - n1, frame0 + n1, d_coords + f * N * 3, pix_shared ? d_pix : d_pix + f * N * 2, pix_shared,
-                           d_gt_jp ? d_gt_jp + f * 12 : nullptr, stream);
+                           d_gt_jp ? d_gt_jp + f * 12 : nullptr, stream, stages);
     CU(cudaStreamWaitEvent(stream, e->ev_join, 0));
     return rc;
 }
@@ -1397,7 +1412,7 @@ int dsac_forward_device(dsac_engine* e, int32_t n, int64_t frame0, const int16_t
     CU(cudaSetDevice(e->cfg.device));
     if (int rc = pass_begin(e, DSAC_PASS_SOFTAM, n, frame0, d_coords, d_pix, pix_shared, d_gt_jp, {(cudaStream_t)stream_v})) return rc;
     if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_forward_device: a submitted pass has not been awaited (dsac_forward_wait)");
-    int rc = forward_split(e, n, frame0, d_coords, d_pix, pix_shared, d_gt_jp, (cudaStream_t)stream_v, true);
+    int rc = forward_split(e, n, frame0, d_coords, d_pix, pix_shared, d_gt_jp, (cudaStream_t)stream_v, true, e->stages);
     if (rc != DSAC_OK) return rc;
     CU(cudaEventRecord(e->ev_fwd, (cudaStream_t)stream_v));   // dsac_backward (engine stream) waits on this
     return DSAC_OK;
@@ -1522,9 +1537,9 @@ static int forward_submit_impl(dsac_engine* e, int32_t n, int64_t frame0, const 
         // pass already fills the partial wave and a high-priority stream would only delay it; mode 2: always)
         int rc = (chunks == 1)
                      ? forward_split(e, m, frame0, e->d_coords, e->d_pix, pix_shared, gt_jp ? e->d_gt.get() : nullptr, st,
-                                     blocking ? e->tail_split >= 1 : e->tail_split >= 2)
+                                     blocking ? e->tail_split >= 1 : e->tail_split >= 2, e->stages)
                      : forward_range(e, lo, m, frame0 + lo, e->d_coords + f * N * 3, pix_shared ? e->d_pix : e->d_pix + f * N * 2,
-                                     pix_shared, gt_jp ? e->d_gt + f * 12 : nullptr, st);
+                                     pix_shared, gt_jp ? e->d_gt + f * 12 : nullptr, st, e->stages);
         if (rc == DSAC_OK && out) {
             if (trace) cudaEventRecord(tev[2], st);
             rc = fetch_range(e, lo, m, out, st);
@@ -1603,10 +1618,7 @@ static int forward_dsac_run(dsac_engine* e, int32_t n, int64_t frame0, const int
         e->ra_jobs = jobs;
     }
     if (want_imaps) CU(e->d_ra_imap.reserve(jobs * N * sizeof(int32_t)));
-    const uint32_t saved = e->stages;
-    e->stages = DSAC_STAGE_SAMPLE | DSAC_STAGE_SCORE;
-    int rc = forward_range(e, 0, n, frame0, d_coords, d_pix, pix_shared, d_gt, stream);
-    e->stages = saved;
+    int rc = forward_range(e, 0, n, frame0, d_coords, d_pix, pix_shared, d_gt, stream, DSAC_STAGE_SAMPLE | DSAC_STAGE_SCORE);
     if (rc != DSAC_OK) return rc;
     if (!d_gt) {   // no ground truth: losses and errors are zero
         CU(cudaMemsetAsync(e->d_ra_loss, 0, jobs * sizeof(double), stream));
@@ -2111,3 +2123,4 @@ static int carve_scratch(dsac_engine* e, DevMem<char>& buf, std::initializer_lis
 #include "backward_dsac_host.inc"
 #include "uncertainty_host.inc"
 #include "modes_host.inc"
+#include "rig_host.inc"

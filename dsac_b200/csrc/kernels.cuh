@@ -662,10 +662,7 @@ __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS) k_sample_t(SamplePa
                 hp[3] = tvec[0]; hp[4] = tvec[1]; hp[5] = tvec[2];
                 double Rm[9];
                 rodrigues_v2m(rvec, Rm);  // getDiffMap -> cv::projectPoints rebuilds R from rvec
-                float4* P = reinterpret_cast<float4*>(p.hyp_P + hi * 12);
-                P[0] = make_float4((float)(p.f * Rm[0]), (float)(p.f * Rm[1]), (float)(p.f * Rm[2]), (float)(p.f * tvec[0]));
-                P[1] = make_float4((float)(p.f * Rm[3]), (float)(p.f * Rm[4]), (float)(p.f * Rm[5]), (float)(p.f * tvec[1]));
-                P[2] = make_float4((float)Rm[6], (float)Rm[7], (float)Rm[8], (float)tvec[2]);
+                pose_rows(p.f, Rm, tvec, p.hyp_P + hi * 12);
                 *reinterpret_cast<int4*>(p.img_idx + hi * 4) = make_int4(cells[0], cells[1], cells[2], cells[3]);
                 p.cand_idx[hi] = (int32_t)cand;
                 if (rank == quota - 1) {
@@ -916,7 +913,8 @@ __device__ __noinline__ void score_tile_guarded(const float* s_P, int nh, const 
 #ifndef K2_MIN_BLOCKS
 #define K2_MIN_BLOCKS 3
 #endif
-template <bool WRITE_DM, bool PER_FRAME>
+// TAIL = false (k_score_rig): the scores only, no softmax tail -- a multi-camera rig sums its cameras' scores first (rig.cuh)
+template <bool WRITE_DM, bool PER_FRAME, bool TAIL = true>
 __device__ __forceinline__ void k_score_body(const ScoreParams& p) {
     __shared__ __align__(128) float s_P[K2_MAX_TILE * 12];
     __shared__ __align__(8) unsigned long long s_bar;
@@ -973,6 +971,7 @@ __device__ __forceinline__ void k_score_body(const ScoreParams& p) {
     }
 
     // ---- last CTA of the frame runs the softmax / soft-argmax tail
+    if constexpr (!TAIL) return;
     __threadfence();
     __syncthreads();
     if (tid == 0) {
@@ -992,5 +991,8 @@ __global__ void __launch_bounds__(K2_THREADS, K2_MIN_BLOCKS) k_score(ScoreParams
 // the same with the per-frame principal points (ScoreParams::cams)
 template <bool WRITE_DM>
 __global__ void __launch_bounds__(K2_THREADS, K2_MIN_BLOCKS) k_score_cam(ScoreParams p) { k_score_body<WRITE_DM, true>(p); }
+// scores only (no diffmaps, no tail), with or without the per-frame principal points: the cameras of a multi-camera rig
+template <bool PER_FRAME>
+__global__ void __launch_bounds__(K2_THREADS, K2_MIN_BLOCKS) k_score_rig(ScoreParams p) { k_score_body<false, PER_FRAME, false>(p); }
 
 }  // namespace dsac

@@ -333,4 +333,51 @@ DSAC_HD void lm_point_contrib(const double* R, const double* J, const double* pa
     for (int a = 0; a < 6; a++) v[21 + a] += ju[a] * eu + jv[a] * ev;
 }
 
+// The same for a camera of a multi-camera rig: (R, param) is the rig pose, and the point's rig-frame position goes through
+// the camera's fixed extrinsic (Rc row-major, tc) before the projection; the Jacobian is the camera Jacobian chained
+// through Rc.  With Rc = I and tc = 0 every product with Rc and every sum with tc is exact, so the contribution equals
+// lm_point_contrib's bit for bit (up to the sign of zero terms).
+DSAC_HD void lm_point_contrib_ext(const double* R, const double* J, const double* param, const double* Rc, const double* tc, double X,
+                                  double Y, double Z, double pix_u, double pix_v, double f, double cx, double cy, double* v) {
+    const double xr = R[0] * X + R[1] * Y + R[2] * Z + param[3];
+    const double yr = R[3] * X + R[4] * Y + R[5] * Z + param[4];
+    const double zr = R[6] * X + R[7] * Y + R[8] * Z + param[5];
+    double x = Rc[0] * xr + Rc[1] * yr + Rc[2] * zr + tc[0];
+    double y = Rc[3] * xr + Rc[4] * yr + Rc[5] * zr + tc[1];
+    double z = Rc[6] * xr + Rc[7] * yr + Rc[8] * zr + tc[2];
+    z = z ? 1. / z : 1;
+    x *= z;
+    y *= z;
+    const double eu = (x * f + cx) - pix_u;
+    const double ev = (y * f + cy) - pix_v;
+    v[27] += eu * eu + ev * ev;
+    double ju[6], jv[6];
+#pragma unroll
+    for (int j = 0; j < 3; j++) {
+        const double ax = X * J[j * 9 + 0] + Y * J[j * 9 + 1] + Z * J[j * 9 + 2];
+        const double ay = X * J[j * 9 + 3] + Y * J[j * 9 + 4] + Z * J[j * 9 + 5];
+        const double az = X * J[j * 9 + 6] + Y * J[j * 9 + 7] + Z * J[j * 9 + 8];
+        const double dx0 = Rc[0] * ax + Rc[1] * ay + Rc[2] * az;
+        const double dy0 = Rc[3] * ax + Rc[4] * ay + Rc[5] * az;
+        const double dz0 = Rc[6] * ax + Rc[7] * ay + Rc[8] * az;
+        ju[j] = f * (z * (dx0 - x * dz0));
+        jv[j] = f * (z * (dy0 - y * dz0));
+    }
+#pragma unroll
+    for (int k = 0; k < 3; k++) {   // d(camera point)/dt = column k of Rc
+        ju[3 + k] = f * (z * (Rc[k] - x * Rc[6 + k]));
+        jv[3 + k] = f * (z * (Rc[3 + k] - y * Rc[6 + k]));
+    }
+    int k = 0;
+#pragma unroll
+    for (int a = 0; a < 6; a++)
+#pragma unroll
+        for (int b = a; b < 6; b++) {
+            v[k] += ju[a] * ju[b] + jv[a] * jv[b];
+            k++;
+        }
+#pragma unroll
+    for (int a = 0; a < 6; a++) v[21 + a] += ju[a] * eu + jv[a] * ev;
+}
+
 }  // namespace dsac

@@ -84,6 +84,23 @@ DSAC_HD void rodrigues_m2v(const double R[9], double r[3]) {
     }
 }
 
+// Multi-camera rigs: a camera's fixed extrinsic (Rc, tc) maps rig coordinates to camera coordinates, X_cam = Rc X_rig + tc.
+// The camera pose of rig pose (R, t): Rc R, Rc t + tc.  Rc = I and tc = 0 give (R, t) exactly.
+DSAC_HD void rig_compose(const double Rc[9], const double tc[3], const double R[9], const double t[3], double Ro[9], double to[3]) {
+    for (int i = 0; i < 3; i++) {
+        for (int j = 0; j < 3; j++) Ro[i * 3 + j] = Rc[i * 3] * R[j] + Rc[i * 3 + 1] * R[3 + j] + Rc[i * 3 + 2] * R[6 + j];
+        to[i] = Rc[i * 3] * t[0] + Rc[i * 3 + 1] * t[1] + Rc[i * 3 + 2] * t[2] + tc[i];
+    }
+}
+// The rig pose of camera pose (R, t): Rc^T R, Rc^T (t - tc), the inverse of rig_compose.
+DSAC_HD void rig_lift(const double Rc[9], const double tc[3], const double R[9], const double t[3], double Ro[9], double to[3]) {
+    const double d[3] = {t[0] - tc[0], t[1] - tc[1], t[2] - tc[2]};
+    for (int i = 0; i < 3; i++) {
+        for (int j = 0; j < 3; j++) Ro[i * 3 + j] = Rc[i] * R[j] + Rc[3 + i] * R[3 + j] + Rc[6 + i] * R[6 + j];
+        to[i] = Rc[i] * d[0] + Rc[3 + i] * d[1] + Rc[6 + i] * d[2];
+    }
+}
+
 // The angle (degrees) of a relative rotation from its trace, as maxloss.h and Hypothesis::calcAngularDistance compute
 // it: the trace clamped to [-1, 3], then 180 acos((trace - 1) / 2) / pi.
 DSAC_HD double rot_err_deg(double trace) {

@@ -179,10 +179,7 @@ __global__ void __launch_bounds__(128) k_prior_inject(PriorInjectParams p) {
         for (int m = 0; m < 6; m++) p.hyp_pose[hi * 6 + m] = po[m];
         double Rm[9];
         rodrigues_v2m(po, Rm);
-        float4* P = reinterpret_cast<float4*>(p.hyp_P + hi * 12);
-        P[0] = make_float4((float)(fc * Rm[0]), (float)(fc * Rm[1]), (float)(fc * Rm[2]), (float)(fc * po[3]));
-        P[1] = make_float4((float)(fc * Rm[3]), (float)(fc * Rm[4]), (float)(fc * Rm[5]), (float)(fc * po[4]));
-        P[2] = make_float4((float)Rm[6], (float)Rm[7], (float)Rm[8], (float)po[5]);
+        pose_rows(fc, Rm, po + 3, p.hyp_P + hi * 12);
         *reinterpret_cast<int4*>(p.img_idx + hi * 4) = make_int4(-1, -1, -1, -1);
         p.cand_idx[hi] = -1;
     }

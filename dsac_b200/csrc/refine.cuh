@@ -32,6 +32,8 @@ namespace dsac {
 constexpr int K4_THREADS = K4_THREADS_DEF;   // 2 warps per job: the work per job is small and mostly sequential
 constexpr int K4_WARPS = K4_THREADS / 32;
 constexpr int K4_MAX_INLIERS = 128;
+constexpr int RIG_MAX_CAMERAS = 8;            // DSAC_MAX_RIG_CAMERAS
+constexpr uint32_t RIG_ST_BAD = 256u;          // DSAC_ST_BAD_RIG
 static_assert(K4_THREADS % 32 == 0 && K4_THREADS >= 32 && K4_THREADS <= 256, "k_refine block size");
 
 struct RefineParams {
@@ -62,6 +64,12 @@ struct RefineParams {
     double* rot_err;
     double* t_err;
     int32_t* correct;
+};
+
+// A multi-camera rig's refinement (k_refine_rig): job r refines rig r over the camera frames r C .. r C + C - 1.
+struct RigRefine {
+    int C;
+    const double* ext;          // [n_frames][12] Rc (row-major) and tc of each camera frame (k_rig_lift)
 };
 
 __device__ __forceinline__ double dot3_plain(double a0, double b0, double a1, double b1, double a2, double b2, double c) {
@@ -130,18 +138,25 @@ __device__ double max_loss_dev(const double R1[9], const double t1[3], const dou
 // without), and the pose update is the Kabsch fit of the selected cells, scene to eye (kabsch_fit), in place of LM.
 // RECORD (the recording replay of dsac_set_coord_derivatives(DSAC_DERIV_IMPLICIT)): the cells the last accepted step fitted,
 // in selection order, go to rec_sel [n_jobs][K4_MAX_INLIERS] and their number to rec_count [n_jobs] (0: no step accepted).
-template <bool PER_FRAME, bool RGBD = false, bool RECORD = false>
+// RIG (k_refine_rig): the job is a rig of rig.C cameras, the pose the rig's.  The flags are those of every camera under its
+// composed pose (rig_compose), the selection is each camera's first inlier_count flagged cells in turn (entries cam << 11 |
+// cell), an LM point is reprojected in its own camera (lm_point_contrib_ext), and the inlier maps are the cameras' frames.
+// The cells are read from global memory rather than staged: C frames do not fit in shared memory.  A rig with
+// DSAC_ST_BAD_RIG in status gets zero outputs.
+template <bool PER_FRAME, bool RGBD = false, bool RECORD = false, bool RIG = false>
 __device__ __forceinline__ void k_refine_body(const RefineParams& p, const double* eye = nullptr, uint16_t* rec_sel = nullptr,
-                                              int32_t* rec_count = nullptr) {
+                                              int32_t* rec_count = nullptr, RigRefine rig = RigRefine{}) {
+    static_assert(!(RIG && (RGBD || RECORD)), "a rig refines RGB frames without recording");
+    constexpr int NC = RIG ? RIG_MAX_CAMERAS : 1;   // camera frames per job, at most
     // the frame's scene coordinates (int16 mm, this job's perturbation applied) and pixel positions, staged once per job:
     // every refinement step reads all of them for the inlier flags and the selected ones in each LM pass
-    __shared__ short s_cX[DSAC_N_CONST], s_cY[DSAC_N_CONST], s_cZ[DSAC_N_CONST];
-    __shared__ float s_fu[DSAC_N_CONST], s_fv[DSAC_N_CONST];
-    __shared__ uint32_t s_bits[DSAC_N_CONST / 32];
-    __shared__ unsigned char s_imap[DSAC_N_CONST];
-    __shared__ unsigned short s_sel[K4_MAX_INLIERS];
-    __shared__ double s_R[9], s_J[27], s_param[6], s_prev[6], s_pose[6], s_Rd[9];
-    __shared__ float s_Pf[12];
+    __shared__ short s_cX[RIG ? 1 : DSAC_N_CONST], s_cY[RIG ? 1 : DSAC_N_CONST], s_cZ[RIG ? 1 : DSAC_N_CONST];
+    __shared__ float s_fu[RIG ? 1 : DSAC_N_CONST], s_fv[RIG ? 1 : DSAC_N_CONST];
+    __shared__ uint32_t s_bits[NC * DSAC_N_CONST / 32];
+    __shared__ unsigned char s_imap[NC * DSAC_N_CONST];
+    __shared__ unsigned short s_sel[NC * K4_MAX_INLIERS];
+    __shared__ double s_R[9], s_J[27], s_param[6], s_prev[6], s_pose[6], s_Rd[RIG ? NC * 12 : 9];
+    __shared__ float s_Pf[NC * 12];
     __shared__ double s_red[K4_WARPS][32];
     __shared__ double s_sum[2][32];
     __shared__ int s_count, s_ctl;
@@ -150,8 +165,22 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p, const doubl
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int job = blockIdx.x;
-    const int frame = p.job_frame ? p.job_frame[job] : job;
+    const int frame = p.job_frame ? p.job_frame[job] : job;   // (RIG: the rig)
     if (frame < 0) return;  // unused job slot
+    const int n_cams = RIG ? rig.C : 1;
+    if constexpr (RIG) {
+        if (p.status[frame] & RIG_ST_BAD) {   // (uniform over the CTA)
+            if (tid < 6) p.out_pose[(size_t)job * 6 + tid] = 0.0;
+            if (p.inlier_map)
+                for (int i = tid; i < n_cams * DSAC_N_CONST; i += K4_THREADS) p.inlier_map[(size_t)job * n_cams * DSAC_N_CONST + i] = 0;
+            if (tid == 0) {
+                if (p.steps_done) p.steps_done[job] = 0;
+                if (p.n_perm_steps) p.n_perm_steps[job] = 0;
+                if (p.gt_jp) { p.loss[job] = 0; p.rot_err[job] = 0; p.t_err[job] = 0; p.correct[job] = 0; }
+            }
+            return;
+        }
+    }
     const Cam cam = frame_cam<PER_FRAME>(p, frame);
     const int16_t* coords = p.coords + (size_t)frame * DSAC_N_CONST * 3;
     const int32_t* pix = p.pix + (size_t)frame * p.pix_stride;
@@ -164,6 +193,9 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p, const doubl
                                            : (p.max_steps ? min(p.ref_steps, p.max_steps[frame]) : p.ref_steps);
 
     if (tid < 6) s_pose[tid] = p.job_init[(size_t)job * 6 + tid];
+    if constexpr (RIG)
+        for (int i = tid; i < n_cams * DSAC_N_CONST; i += K4_THREADS) s_imap[i] = 0;
+    else
     for (int i = tid; i < DSAC_N_CONST; i += K4_THREADS) {
         s_imap[i] = 0;
         int v[3];
@@ -183,6 +215,62 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p, const doubl
 
     // inlier flags of the current pose s_pose (getDiffMap, cnn_softam.h:319-362, reduced to "< threshold")
     auto inlier_flags = [&]() {
+        if constexpr (RIG) {
+            // every camera's composed pose (lane k < 12 stores element k: R row-major, then t) and its fp32 rows
+            if (warp == 0) {
+                double pose[6], R[9];
+#pragma unroll
+                for (int k = 0; k < 6; k++) pose[k] = s_pose[k];
+                rodrigues_v2m(pose, R);
+                for (int c = 0; c < n_cams; c++) {
+                    const int fr = frame * n_cams + c;
+                    const double* E = rig.ext + (size_t)fr * 12;
+                    double Rk[9], tk[3];
+                    rig_compose(E, E + 9, R, pose + 3, Rk, tk);
+                    const double fc = frame_cam<PER_FRAME>(p, fr).f;
+#pragma unroll
+                    for (int k = 0; k < 12; k++) {
+                        const int row = k >> 2, col = k & 3;
+                        const double v = (col < 3) ? Rk[row * 3 + col] : tk[row];
+                        if (lane == k) {
+                            s_Rd[c * 12 + k] = k < 9 ? Rk[k] : tk[k - 9];
+                            s_Pf[c * 12 + k] = (float)(row < 2 ? fc * v : v);
+                        }
+                    }
+                }
+            }
+            __syncthreads();
+            for (int base = 0; base < n_cams * DSAC_N_CONST; base += K4_THREADS) {
+                const int ci = base + tid;
+                bool flag = false;
+                if (ci < n_cams * DSAC_N_CONST) {   // (a warp never straddles two cameras: 1600 = 50 x 32)
+                    const int c = ci / DSAC_N_CONST, cell = ci - c * DSAC_N_CONST, fr = frame * n_cams + c;
+                    const Cam cm = frame_cam<PER_FRAME>(p, fr);
+                    const int16_t* co = p.coords + ((size_t)fr * DSAC_N_CONST + cell) * 3;
+                    const int32_t* px = p.pix + (size_t)fr * p.pix_stride + cell * 2;
+                    const float X = (float)__ldg(co), Y = (float)__ldg(co + 1), Z = (float)__ldg(co + 2);
+                    const float fu = (float)__ldg(px), fv = (float)__ldg(px + 1);
+                    const float ccx = (float)cm.cx, ccy = (float)cm.cy;
+                    float P[12];
+#pragma unroll
+                    for (int k = 0; k < 12; k++) P[k] = s_Pf[c * 12 + k];
+                    const int r = reproj_below_thr_fast(P, X, Y, Z, fu - ccx, fv - ccy, fabsf(ccx) + fabsf(ccy), thrf);
+                    if (r >= 0) {
+                        flag = (r != 0);
+                    } else {
+                        double Rd[9], t[3];
+#pragma unroll
+                        for (int k = 0; k < 9; k++) Rd[k] = s_Rd[c * 12 + k];
+                        t[0] = s_Rd[c * 12 + 9]; t[1] = s_Rd[c * 12 + 10]; t[2] = s_Rd[c * 12 + 11];
+                        flag = reproj_error_exact(Rd, t, (double)X, (double)Y, (double)Z, cm.f, cm.cx, cm.cy, fu, fv) < thrf;
+                    }
+                }
+                const uint32_t m = __ballot_sync(0xffffffffu, flag);
+                if (lane == 0 && base + warp * 32 < n_cams * DSAC_N_CONST) s_bits[(base >> 5) + warp] = m;
+            }
+            __syncthreads();
+            return;
+        }
         if (warp == 0) {
             double pose[6], R[9];
 #pragma unroll
@@ -229,12 +317,14 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p, const doubl
     constexpr int K4_PPT = (K4_MAX_INLIERS + K4_THREADS - 1) / K4_THREADS;
     float selX[K4_PPT], selY[K4_PPT], selZ[K4_PPT], selU[K4_PPT], selV[K4_PPT];
     auto load_selected = [&](int n) {
+        if constexpr (!RIG) {   // (RIG: read from global memory in each pass)
 #pragma unroll
-        for (int k = 0; k < K4_PPT; k++) {
-            const int i = tid + k * K4_THREADS;
-            const int c = (i < n) ? s_sel[i] : 0;
-            selX[k] = (float)s_cX[c]; selY[k] = (float)s_cY[c]; selZ[k] = (float)s_cZ[c];
-            selU[k] = s_fu[c]; selV[k] = s_fv[c];
+            for (int k = 0; k < K4_PPT; k++) {
+                const int i = tid + k * K4_THREADS;
+                const int c = (i < n) ? s_sel[i] : 0;
+                selX[k] = (float)s_cX[c]; selY[k] = (float)s_cY[c]; selZ[k] = (float)s_cZ[c];
+                selU[k] = s_fu[c]; selV[k] = s_fv[c];
+            }
         }
     };
 
@@ -244,11 +334,23 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p, const doubl
         double v[32];
 #pragma unroll
         for (int k = 0; k < 32; k++) v[k] = 0;
+        if constexpr (RIG) {   // (the points of each thread in the order of the loop below)
+            for (int i = tid; i < n; i += K4_THREADS) {
+                const int code = s_sel[i], c = code >> 11, cell = code & 2047, fr = frame * n_cams + c;
+                const Cam cm = frame_cam<PER_FRAME>(p, fr);
+                const int16_t* co = p.coords + ((size_t)fr * DSAC_N_CONST + cell) * 3;
+                const int32_t* px = p.pix + (size_t)fr * p.pix_stride + cell * 2;
+                const double* E = rig.ext + (size_t)fr * 12;
+                lm_point_contrib_ext(s_R, s_J, s_param, E, E + 9, (double)__ldg(co), (double)__ldg(co + 1), (double)__ldg(co + 2),
+                                     (double)(float)__ldg(px), (double)(float)__ldg(px + 1), cm.f, cm.cx, cm.cy, v);
+            }
+        } else {
 #pragma unroll
-        for (int k = 0; k < K4_PPT; k++)
-            if (tid + k * K4_THREADS < n)
-                lm_point_contrib(s_R, s_J, s_param, (double)selX[k], (double)selY[k], (double)selZ[k], (double)selU[k], (double)selV[k],
-                                 cam.f, cam.cx, cam.cy, v);
+            for (int k = 0; k < K4_PPT; k++)
+                if (tid + k * K4_THREADS < n)
+                    lm_point_contrib(s_R, s_J, s_param, (double)selX[k], (double)selY[k], (double)selZ[k], (double)selU[k], (double)selV[k],
+                                     cam.f, cam.cx, cam.cy, v);
+        }
         // transposed butterfly: after the step with offset `off` every lane keeps half of its values; lane L ends with sum L
 #pragma unroll
         for (int half = 16, off = 16; half >= 1; half >>= 1, off >>= 1) {
@@ -274,22 +376,30 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p, const doubl
     for (int rStep = 0; rStep < step_limit; rStep++) {
         n_perm++;
         // ---- ordered selection of the first inlier_count flagged cells of the step's permutation (cnn_softam.h:1117-1134)
+        // (RIG: every camera in turn, its cells appended to the previous cameras')
         if (warp == 0) {
             const uint16_t* perm = p.perm + (size_t)rStep * DSAC_N_CONST;
-            int count = 0;
-            for (int k0 = 0; k0 < DSAC_N_CONST && count < p.inlier_count; k0 += 32) {
-                const int c = __ldg(perm + k0 + lane);
-                bool flag = (s_bits[c >> 5] >> (c & 31)) & 1u;
-                if constexpr (RGBD) flag = flag && __ldg(eye + ((size_t)frame * DSAC_N_CONST + c) * 3 + 2) > 0.0;   // (NaN: no depth)
-                const uint32_t m = __ballot_sync(0xffffffffu, flag);
-                const int rank = count + __popc(m & ((1u << lane) - 1u));
-                if (flag && rank < p.inlier_count) {
-                    s_sel[rank] = (unsigned short)c;
-                    s_imap[c] += 1;  // cnn_softam.h:1129 (each cell appears once per permutation)
+            int total = 0;
+            for (int cc = 0; cc < n_cams; cc++) {
+                const uint32_t* bits = s_bits + cc * (DSAC_N_CONST / 32);
+                unsigned char* imap = s_imap + cc * DSAC_N_CONST;
+                unsigned short* sel = s_sel + total;
+                int count = 0;
+                for (int k0 = 0; k0 < DSAC_N_CONST && count < p.inlier_count; k0 += 32) {
+                    const int c = __ldg(perm + k0 + lane);
+                    bool flag = (bits[c >> 5] >> (c & 31)) & 1u;
+                    if constexpr (RGBD) flag = flag && __ldg(eye + ((size_t)frame * DSAC_N_CONST + c) * 3 + 2) > 0.0;   // (NaN: no depth)
+                    const uint32_t m = __ballot_sync(0xffffffffu, flag);
+                    const int rank = count + __popc(m & ((1u << lane) - 1u));
+                    if (flag && rank < p.inlier_count) {
+                        sel[rank] = (unsigned short)(RIG ? (cc << 11 | c) : c);
+                        imap[c] += 1;  // cnn_softam.h:1129 (each cell appears once per permutation)
+                    }
+                    count = min(count + __popc(m), p.inlier_count);
                 }
-                count = min(count + __popc(m), p.inlier_count);
+                total += count;
             }
-            if (lane == 0) s_count = count;
+            if (lane == 0) s_count = total;
         }
         __syncthreads();
         const int count = s_count;
@@ -382,7 +492,7 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p, const doubl
         if (tid == 0) rec_count[job] = rc;
     }
     if (p.inlier_map)
-        for (int i = tid; i < DSAC_N_CONST; i += K4_THREADS) p.inlier_map[(size_t)job * DSAC_N_CONST + i] = s_imap[i];
+        for (int i = tid; i < n_cams * DSAC_N_CONST; i += K4_THREADS) p.inlier_map[(size_t)job * n_cams * DSAC_N_CONST + i] = s_imap[i];
     if (tid == 0) {
         if (p.steps_done) p.steps_done[job] = steps_done;
         if (p.n_perm_steps) p.n_perm_steps[job] = n_perm;
@@ -432,11 +542,22 @@ __global__ void __launch_bounds__(K4_THREADS, K4_MIN_BLOCKS) k_refine_rgbd_rec_c
     k_refine_body<true, true, true>(p, eye, rec_sel, rec_count);
 }
 
+// multi-camera rigs: one job per rig (RefineParams::status, gt_jp and the outputs per rig; cams, coords and pix per frame)
+// (one CTA per rig, so a few hundred CTAs at most: the register budget of two CTAs per SM keeps the C-camera loops out of
+// local memory)
+__global__ void __launch_bounds__(K4_THREADS, 2) k_refine_rig(RefineParams p, RigRefine rig) {
+    k_refine_body<false, false, false, true>(p, nullptr, nullptr, nullptr, rig);
+}
+__global__ void __launch_bounds__(K4_THREADS, 2) k_refine_rig_cam(RefineParams p, RigRefine rig) {
+    k_refine_body<true, false, false, true>(p, nullptr, nullptr, nullptr, rig);
+}
+
 // the instantiations by per-frame camera (RefineParams::cams), one table per signature
 constexpr void (*k_refine_tab[2])(RefineParams) = {k_refine, k_refine_cam};
 constexpr void (*k_refine_rgbd_tab[2])(RefineParams, const double*) = {k_refine_rgbd, k_refine_rgbd_cam};
 constexpr void (*k_refine_rec_tab[2])(RefineParams, uint16_t*, int32_t*) = {k_refine_rec, k_refine_rec_cam};
 constexpr void (*k_refine_rgbd_rec_tab[2])(RefineParams, const double*, uint16_t*, int32_t*) = {k_refine_rgbd_rec, k_refine_rgbd_rec_cam};
+constexpr void (*k_refine_rig_tab[2])(RefineParams, RigRefine) = {k_refine_rig, k_refine_rig_cam};
 
 // one CTA per job, with the instantiation the parameters ask for; eye != null: an RGB-D pass
 inline void launch_refine(const RefineParams& p, unsigned jobs, cudaStream_t stream, const double* eye = nullptr) {

@@ -42,10 +42,7 @@ __device__ __forceinline__ void k1_write_hyp(const SampleParams& p, size_t hi, c
     hp[3] = tvec[0]; hp[4] = tvec[1]; hp[5] = tvec[2];
     double Rm[9];
     rodrigues_v2m(rvec, Rm);
-    float4* P = reinterpret_cast<float4*>(p.hyp_P + hi * 12);
-    P[0] = make_float4((float)(p.f * Rm[0]), (float)(p.f * Rm[1]), (float)(p.f * Rm[2]), (float)(p.f * tvec[0]));
-    P[1] = make_float4((float)(p.f * Rm[3]), (float)(p.f * Rm[4]), (float)(p.f * Rm[5]), (float)(p.f * tvec[1]));
-    P[2] = make_float4((float)Rm[6], (float)Rm[7], (float)Rm[8], (float)tvec[2]);
+    pose_rows(p.f, Rm, tvec, p.hyp_P + hi * 12);
     *reinterpret_cast<int4*>(p.img_idx + hi * 4) = make_int4(cells[0], cells[1], cells[2], cells[3]);
     p.cand_idx[hi] = (int32_t)cand;
 }
@@ -1606,9 +1603,7 @@ __global__ void __launch_bounds__(256) k1_focal_rows_cam(SampleParams p, int n_f
     const double rvec[3] = {hp[0], hp[1], hp[2]}, tvec[2] = {hp[3], hp[4]};
     double Rm[9];
     rodrigues_v2m(rvec, Rm);
-    float4* P = reinterpret_cast<float4*>(p.hyp_P + (size_t)i * 12);
-    P[0] = make_float4((float)(f * Rm[0]), (float)(f * Rm[1]), (float)(f * Rm[2]), (float)(f * tvec[0]));
-    P[1] = make_float4((float)(f * Rm[3]), (float)(f * Rm[4]), (float)(f * Rm[5]), (float)(f * tvec[1]));
+    pose_rows_f(f, Rm, tvec, p.hyp_P + (size_t)i * 12);
 }
 
 }  // namespace dsac

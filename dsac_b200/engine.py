@@ -17,7 +17,7 @@ STAGE_SAMPLE, STAGE_SCORE, STAGE_REFINE, STAGE_EVAL, STAGE_ALL = 1, 2, 4, 8, 15
 ST_SAMPLER_EXHAUSTED, ST_REFINE_ABORTED = 1, 2
 ST_BAD_WEIGHTS = 32          # DSAC_ST_BAD_WEIGHTS
 ST_NO_DEPTH = 64             # DSAC_ST_NO_DEPTH
-PASS_SOFTAM, PASS_DSAC = 1, 2   # DSAC_PASS_SOFTAM, DSAC_PASS_DSAC (dsac_last_pass)
+PASS_SOFTAM, PASS_DSAC, PASS_RIG = 1, 2, 3   # DSAC_PASS_SOFTAM, DSAC_PASS_DSAC, DSAC_PASS_RIG (dsac_last_pass)
 
 # every symbol include/dsac_b200.h declares
 EXPORTS = [
@@ -33,12 +33,14 @@ EXPORTS = [
     "dsac_score_draw_device", "dsac_score_maps_device", "dsac_shuffle_permutations",
     "dsac_set_sampling_logits_device", "dsac_set_cell_depth_device", "dsac_sampling_table_device", "dsac_sampling_log_prob_device",
     "dsac_sampling_log_prob_backward_device", "dsac_set_coord_derivatives", "dsac_pose_uncertainty_device",
-    "dsac_last_pass", "dsac_set_pose_priors_device", "dsac_pose_modes_device",
+    "dsac_last_pass", "dsac_set_pose_priors_device", "dsac_pose_modes_device", "dsac_forward_rig_device",
 ]
 
 ST_OBJ_DRAW_EXHAUSTED = 8    # DSAC_ST_OBJ_DRAW_EXHAUSTED
 ST_DEPTH_DROPPED = 16        # DSAC_ST_DEPTH_DROPPED
 ST_BAD_PRIOR = 128           # DSAC_ST_BAD_PRIOR
+ST_BAD_RIG = 256             # DSAC_ST_BAD_RIG
+MAX_RIG_CAMERAS = 8          # DSAC_MAX_RIG_CAMERAS
 MAX_PRIORS = 16              # DSAC_MAX_PRIORS
 MAX_MODES = 16               # DSAC_MAX_MODES
 OBJ_STATE_WORDS = 625        # one ThreadRand stream: std::mt19937's 624 words and its position
@@ -148,6 +150,14 @@ class PoseModesOut(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in _MODES_FIELDS]
 
 
+_RIG_FIELDS = ("hyp_pose", "rig_hyp", "scores", "sf", "entropy", "avg_pose", "ref_pose", "inlier_map", "steps_done", "status",
+               "loss", "rot_err", "t_err", "correct")
+
+
+class RigOut(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in _RIG_FIELDS]
+
+
 SCORE_HOOK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p)
 SCORE_BACKWARD_HOOK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p)
 
@@ -218,6 +228,8 @@ def load(build_if_missing=True):
     lib.dsac_last_pass.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
     lib.dsac_pose_modes_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_double, C.c_double, C.POINTER(PoseModesOut),
                                            C.c_void_p]
+    lib.dsac_forward_rig_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32,
+                                            C.c_void_p, C.c_void_p, C.POINTER(RigOut), C.c_void_p]
     lib.dsac_backward_pose_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]
     lib.dsac_backward_dsac_pose_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(BackwardDsacOut),
                                                    C.c_void_p, C.c_float, C.c_void_p]
@@ -644,12 +656,26 @@ class Engine:
         self._check(self.lib.dsac_pose_modes_device(self.h, n, max_modes, float(rot_rad), float(trans_mm), C.byref(raw),
                                                     C.c_void_p(stream) if stream else None))
 
+    def forward_rig_device(self, n, n_cameras, d_coords, d_pix, d_cam_from_rig, pix_shared=0, d_gt_rig=None, frame0=0,
+                           stream=None, **ptrs):
+        """dsac_forward_rig_device (raw device pointers as ints): one pose per rig of n_cameras cameras over n frames
+        (INTEGRATION.md, "Multi-camera rigs"); ptrs: device destinations of the fields of dsac_rig_out."""
+        raw = RigOut()
+        for k, v in ptrs.items():
+            if k not in _RIG_FIELDS:
+                raise KeyError(k)
+            setattr(raw, k, v)
+        self.passes += 1
+        self._check(self.lib.dsac_forward_rig_device(self.h, n, n_cameras, frame0, C.c_void_p(d_coords), C.c_void_p(d_pix),
+                                                     pix_shared, C.c_void_p(d_cam_from_rig), C.c_void_p(d_gt_rig) if d_gt_rig else None,
+                                                     C.byref(raw), C.c_void_p(stream) if stream else None))
+
     def last_pass(self, n):
-        """dsac_last_pass: "softam" or "dsac", the pipeline of the pass over n frames whose refined poses the engine holds
-        (what pose_uncertainty_device reads); raises if it holds none."""
+        """dsac_last_pass: "softam", "dsac" or "rig", the kind of the pass over n frames the engine holds (what
+        pose_uncertainty_device reads after the first two); raises if it holds none."""
         kind = C.c_int32(0)
         self._check(self.lib.dsac_last_pass(self.h, n, C.byref(kind)))
-        return {PASS_SOFTAM: "softam", PASS_DSAC: "dsac"}[kind.value]
+        return {PASS_SOFTAM: "softam", PASS_DSAC: "dsac", PASS_RIG: "rig"}[kind.value]
 
     def backward_pose_device(self, n, d_grad_ref, d_dloss_dobj=None, d_dloss_dpred=None, clamp=0.0, stream=None):
         """dsac_backward_pose_device (raw device pointers as ints): soft-argmax backward seeded by dOuter/d(refined jp6)."""

@@ -51,6 +51,7 @@ extern "C" {
 #define DSAC_ST_BAD_WEIGHTS 32u           /* guided sampling: a NaN or +inf logit, or fewer than 4 cells with weight > 0; nothing sampled */
 #define DSAC_ST_NO_DEPTH 64u              /* RGB-D pass: fewer than 4 cells with depth; nothing sampled */
 #define DSAC_ST_BAD_PRIOR 128u            /* a non-finite prior or an information matrix that is not positive definite; nothing sampled */
+#define DSAC_ST_BAD_RIG 256u              /* dsac_forward_rig_device: a non-finite extrinsic; the rig's outputs are zero */
 
 typedef struct dsac_engine dsac_engine;
 
@@ -426,6 +427,7 @@ int dsac_pose_uncertainty_device(dsac_engine* e, int32_t n_frames, const dsac_po
  * pass over n_frames. */
 #define DSAC_PASS_SOFTAM 1
 #define DSAC_PASS_DSAC 2
+#define DSAC_PASS_RIG 3            /* dsac_forward_rig_device: no backward pass or pose query reads it */
 int dsac_last_pass(dsac_engine* e, int32_t n_frames, int32_t* pipeline);
 
 /* Pose modes of the preceding pass (INTEGRATION.md, "Pose modes"): per frame up to M = max_modes distinct refined poses of
@@ -464,6 +466,48 @@ typedef struct dsac_pose_modes_out {   /* DEVICE pointers, each nullable; M = ma
 } dsac_pose_modes_out;
 int dsac_pose_modes_device(dsac_engine* e, int32_t n_frames, int32_t max_modes, double rot_rad, double trans_mm,
                            const dsac_pose_modes_out* d_out, void* stream);
+
+/* Multi-camera rigs (INTEGRATION.md, "Multi-camera rigs"): one pose per rig from several cameras with known extrinsics.
+ * The n_frames frames are R = n_frames / C rigs of C = n_cameras cameras; frame f = r*C + c is camera c of rig r, with the
+ * camera of frame f (dsac_set_cameras) and the extrinsic d_cam_from_rig[f] [n][6], a cv pose (rvec, tvec mm):
+ * X_cam = R_c X_rig + t_c.  H = n_hyps.
+ *   sample: every frame as dsac_forward_device samples it (hyp_pose, img_idx, cand_idx and n_candidates bit-identical);
+ *   lift:   camera c's hypothesis h becomes the rig pose R_r = R_c^T R_h, t_r = R_c^T (t_h - t_c), slot j = c*H + h of the
+ *           rig's pool of C*H (an extrinsic whose rvec is exactly zero keeps the hypothesis' rvec);
+ *   score:  score[r][j] = sum over c' = 0 .. C-1, in order, in fp64, of k_score's soft-inlier score of camera c' for the
+ *           pose T_c' o T_r (so at the same alpha the softmax is about C times sharper than one camera's); softmax,
+ *           entropy and soft-argmax over the pool as dsac_forward_device;
+ *   refine: from the soft-argmax pose, ref_steps steps: per camera in order its first <= inlier_count cells of the step's
+ *           permutation with reprojection error < thr2d under its composed pose, concatenated (fewer than 50 in all stop,
+ *           DSAC_ST_REFINE_ABORTED), then CvLevMarq's fit of the rig's 6 parameters over their reprojections;
+ *   eval:   with d_gt_rig_jp [R][12] (jp of the rig frame) and DSAC_STAGE_EVAL, loss, rot_err, t_err, correct per rig.
+ * status[r]: the OR of its frames' sampler bits, DSAC_ST_REFINE_ABORTED, and DSAC_ST_BAD_RIG when one of its extrinsics is
+ * not finite (all of that rig's outputs but hyp_pose are then zero).  C = 1 with zero extrinsics gives dsac_forward_device's
+ * results bit for bit.  Ordered on `stream`; the engine's pass becomes DSAC_PASS_RIG, which the backward passes,
+ * dsac_refined_jp6_device, dsac_pose_uncertainty_device and dsac_pose_modes_device refuse; the sampling log-probability
+ * stays valid.  DSAC_ERR_ARG, with the engine left as it was: n_frames % C != 0, C outside [1, DSAC_MAX_RIG_CAMERAS],
+ * C * n_hyps > DSAC_MAX_HYPS, a score hook, cell depth or pose priors set, a stage mask without sample, score or refine, a
+ * submitted pass that has not been awaited, or a NULL input or d_out. */
+#define DSAC_MAX_RIG_CAMERAS 8
+typedef struct dsac_rig_out {   /* DEVICE pointers, each nullable; R = n_frames / C, P = C * n_hyps */
+    double*   hyp_pose;    /* [n][H][6]  the frames' sampled hypotheses */
+    double*   rig_hyp;     /* [R][P][6]  the pool: rig poses (cv) */
+    double*   scores;      /* [R][P] */
+    double*   sf;          /* [R][P]     softmax */
+    double*   entropy;     /* [R] */
+    double*   avg_pose;    /* [R][6]     soft-argmax rig pose */
+    double*   ref_pose;    /* [R][6]     refined rig pose */
+    int32_t*  inlier_map;  /* [n][1600]  per camera frame */
+    int32_t*  steps_done;  /* [R] */
+    uint32_t* status;      /* [R]        DSAC_ST_* */
+    double*   loss;        /* [R] */
+    double*   rot_err;     /* [R] */
+    double*   t_err;       /* [R] */
+    int32_t*  correct;     /* [R] */
+} dsac_rig_out;
+int dsac_forward_rig_device(dsac_engine* e, int32_t n_frames, int32_t n_cameras, int64_t frame0, const int16_t* d_coords,
+                            const int32_t* d_pix, int32_t pix_shared, const double* d_cam_from_rig, const double* d_gt_rig_jp,
+                            const dsac_rig_out* d_out, void* stream);
 
 /* Soft-argmax backward seeded by d_grad_ref [n][6] = dOuter/d(refined jp6) instead of dLossMax.
  * No ground truth needed. dloss_dobj / dloss_dpred / clamp as in dsac_backward_device; clamp applies to the total. */
