@@ -9,6 +9,8 @@
     my_loss(pose).backward()                                        # prediction.grad, no ground truth needed
     unc = pose_uncertainty(engine, n)                               # covariances and support of the last pass's poses
     modes = pose_modes(engine, n, 4, 0.17, 100.0)                   # up to 4 distinct refined poses per frame
+    loss = rig_softam_loss(engine, prediction, pix, ext, C, gt_rig)  # one loss per rig of C cameras, [n / C]
+    pose = rig_softam_pose(engine, prediction, pix, ext, C)          # refined jp 6-vector per rig, [n / C][6]
 
 `prediction` is the coordinate CNN's output: float32 [n][1600][3] scene coordinates in metres on the engine's device,
 cell y*40+x.  It is the only input that receives a gradient.  The gradient is the one the reference hands to
@@ -362,6 +364,77 @@ def pose_modes(engine, n, max_modes, rot_rad, trans_mm):
     return out
 
 
+def _check_rig(engine, prediction, pix, cam_from_rig, n_cameras, gt_jp):
+    C = int(n_cameras)
+    n, pix, _, shared = _check_inputs(engine, prediction, pix, None, need_gt=False)
+    dev = prediction.device
+    if not 1 <= C <= _E.MAX_RIG_CAMERAS or n % C:
+        raise ValueError("n_cameras %d must be in [1, %d] and divide the %d frames" % (C, _E.MAX_RIG_CAMERAS, n))
+    R = n // C
+    if cam_from_rig.dtype != torch.float64 or cam_from_rig.numel() != n * 6 or cam_from_rig.device != dev:
+        raise ValueError("cam_from_rig must be float64 [%d][6] on %s" % (n, dev))
+    if gt_jp is not None and (gt_jp.dtype != torch.float64 or gt_jp.numel() != R * 12 or gt_jp.device != dev):
+        raise ValueError("gt_jp must be float64 [%d][12] on %s" % (R, dev))
+    return C, n, R, pix, shared
+
+
+class _RigSoftam(torch.autograd.Function):
+    """The rig pass with the loss per rig (gt_jp given) or the refined rig jp 6-vector (gt_jp None) as its output."""
+
+    @staticmethod
+    def forward(ctx, prediction, engine, pix, cam_from_rig, n_cameras, gt_jp, frame0, clamp):
+        C, n, R, pix, shared = _check_rig(engine, prediction, pix, cam_from_rig, n_cameras, gt_jp)
+        dev = prediction.device
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        coords = _coords(engine, prediction.detach().contiguous(), stream)
+        ext = cam_from_rig.detach().contiguous()
+        gt = gt_jp.detach().contiguous() if gt_jp is not None else None
+        if gt is not None:
+            out = torch.empty((R,), dtype=torch.float64, device=dev)
+            engine.forward_rig_device(n, C, coords.data_ptr(), pix.data_ptr(), ext.data_ptr(), shared, gt.data_ptr(), frame0, stream,
+                                      loss=out.data_ptr())
+        else:
+            out = torch.empty((R, 6), dtype=torch.float64, device=dev)
+            engine.forward_rig_device(n, C, coords.data_ptr(), pix.data_ptr(), ext.data_ptr(), shared, None, frame0, stream)
+            engine.rig_refined_jp6_device(n, out.data_ptr(), stream)
+        ctx.engine, ctx.pass_id, ctx.n, ctx.clamp, ctx.loss = engine, engine.passes, n, clamp, gt is not None
+        ctx.keep = (coords, pix, ext, gt)   # the rig backward reads the pass's inputs
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        g, grad = _grad_input(ctx, grad_out)
+        stream = torch.cuda.current_stream(g.device).cuda_stream
+        if ctx.loss:
+            ctx.engine.backward_rig_device(ctx.n, g.data_ptr(), None, grad.data_ptr(), ctx.clamp, stream)
+        else:
+            ctx.engine.backward_rig_pose_device(ctx.n, g.data_ptr(), None, grad.data_ptr(), ctx.clamp, stream)
+        return grad, None, None, None, None, None, None, None
+
+
+def rig_softam_loss(engine, prediction, pix, cam_from_rig, n_cameras, gt_jp, frame0=0, clamp=0.1, cameras=None,
+                    sampling_logits=None):
+    """Per-rig loss of the rig pass (rig_pose's rig layout; INTEGRATION.md, "Rig gradients"): dLossMax's loss of each refined
+    rig pose against gt_jp float64 [R][12], float64 [R]; differentiable with respect to `prediction` through every camera's
+    scene coordinates, by the implicit-function derivatives whatever the engine's set_coord_derivatives.  clamp, cameras
+    and sampling_logits as in softam_loss; with sampling_logits, sampling_log_prob gives the REINFORCE term of the rigs."""
+    if gt_jp is None:
+        raise ValueError("the loss needs the rig ground-truth poses gt_jp [R][12]")
+    _check_rig(engine, prediction, pix, cam_from_rig, n_cameras, gt_jp)
+    _set_cameras(engine, prediction, cameras)
+    _set_sampling(engine, prediction, sampling_logits)
+    return _RigSoftam.apply(prediction, engine, pix, cam_from_rig, int(n_cameras), gt_jp, int(frame0), float(clamp))
+
+
+def rig_softam_pose(engine, prediction, pix, cam_from_rig, n_cameras, frame0=0, clamp=0.1, cameras=None, sampling_logits=None):
+    """Refined pose of every rig as a jp 6-vector [rodrigues(R); t in mm] of the rig frame, float64 [R][6]; differentiable
+    with respect to `prediction` as rig_softam_loss.  Needs no ground truth."""
+    _check_rig(engine, prediction, pix, cam_from_rig, n_cameras, None)
+    _set_cameras(engine, prediction, cameras)
+    _set_sampling(engine, prediction, sampling_logits)
+    return _RigSoftam.apply(prediction, engine, pix, cam_from_rig, int(n_cameras), None, int(frame0), float(clamp))
+
+
 def rig_pose(engine, prediction, pix, cam_from_rig, n_cameras, frame0=0, cameras=None, sampling_logits=None, gt_jp=None):
     """One pose per multi-camera rig (INTEGRATION.md, "Multi-camera rigs"): the n frames of `prediction` are R = n / C rigs
     of C = n_cameras cameras, frame r C + c camera c of rig r, whose extrinsic cam_from_rig[r C + c] (float64 [n][6], a cv
@@ -370,16 +443,8 @@ def rig_pose(engine, prediction, pix, cam_from_rig, n_cameras, frame0=0, cameras
     torch.cuda.current_stream(), without autograd history: hyp_pose [n][H][6]; rig_hyp [R][C H][6], scores and sf
     [R][C H]; entropy [R]; avg_pose and ref_pose [R][6] (cv poses of the rig); inlier_map int32 [n][1600]; steps_done int32,
     status int32 [R]; and with gt_jp loss, rot_err, t_err float64 and correct int32 [R]."""
-    C = int(n_cameras)
-    n, pix, _, shared = _check_inputs(engine, prediction, pix, None, need_gt=False)
-    dev = prediction.device
-    if not 1 <= C <= _E.MAX_RIG_CAMERAS or n % C:
-        raise ValueError("n_cameras %d must be in [1, %d] and divide the %d frames" % (C, _E.MAX_RIG_CAMERAS, n))
-    R, H = n // C, engine.cfg.n_hyps
-    if cam_from_rig.dtype != torch.float64 or cam_from_rig.numel() != n * 6 or cam_from_rig.device != dev:
-        raise ValueError("cam_from_rig must be float64 [%d][6] on %s" % (n, dev))
-    if gt_jp is not None and (gt_jp.dtype != torch.float64 or gt_jp.numel() != R * 12 or gt_jp.device != dev):
-        raise ValueError("gt_jp must be float64 [%d][12] on %s" % (R, dev))
+    C, n, R, pix, shared = _check_rig(engine, prediction, pix, cam_from_rig, n_cameras, gt_jp)
+    dev, H = prediction.device, engine.cfg.n_hyps
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
     stream = torch.cuda.current_stream(dev).cuda_stream

@@ -636,7 +636,15 @@ __global__ void k_dscore_reduce(BwParams p) {
     }
 }
 
-__global__ void __launch_bounds__(K5_THREADS) k_dscore(BwParams p) {
+// The rig backward's form (k_dscore_rig): frame f = r C + c scores its rig's pool, p.H = P slots with the composed poses
+// T_c o T_j in hypjp [n][P][39]; the score output gradients are the rig's, sog [R][P], and the 1x6 sum over the cells goes
+// to w [n][P][6] in place of the support scatter, which crosses cameras (rig.cuh, k_rig_bw_support).
+struct RigDscore {
+    int C;
+    double* w;
+};
+template <bool RIG>
+__device__ __forceinline__ void k_dscore_body(const BwParams& p, const RigDscore& rig) {
     __shared__ double s_h[39];
     __shared__ double s_red[K5_WARPS][6];
     __shared__ double s_w[6];
@@ -660,7 +668,7 @@ __global__ void __launch_bounds__(K5_THREADS) k_dscore(BwParams p) {
         __syncthreads();
         if (tid < 39) s_h[tid] = p.s.hypjp[((size_t)frame * p.H + h) * 39 + tid];
         __syncthreads();
-        double go = p.s.sog[(size_t)frame * p.H + h];
+        double go = p.s.sog[(size_t)(RIG ? frame / rig.C : frame) * p.H + h];
         if (p.grad_clamp > 0) go = fmax(-p.grad_clamp, fmin(p.grad_clamp, go));   // train_score_softam.lua:97
         const double* R = s_h;       // jp rotation
         const double* t = s_h + 9;
@@ -737,7 +745,9 @@ __global__ void __launch_bounds__(K5_THREADS) k_dscore(BwParams p) {
         }
         __syncthreads();
         // supportPointGradients = w . dPNP_h (1x12) onto the 4 support cells (cnn_softam.h:632-642)
-        if (tid < 12) {
+        if constexpr (RIG) {
+            if (tid < 6) rig.w[((size_t)frame * p.H + h) * 6 + tid] = s_w[tid];
+        } else if (tid < 12) {
             const double* Jp = p.s.dpnp + ((size_t)frame * p.H + h) * 72;
             double s = 0;
             for (int k = 0; k < 6; k++) s += s_w[k] * Jp[k * 12 + tid];
@@ -759,6 +769,8 @@ __global__ void __launch_bounds__(K5_THREADS) k_dscore(BwParams p) {
         for (int k = 0; k < 3; k++) row[colb + k] += acc[j][k];
     }
 }
+__global__ void __launch_bounds__(K5_THREADS) k_dscore(BwParams p) { k_dscore_body<false>(p, RigDscore{}); }
+__global__ void __launch_bounds__(K5_THREADS) k_dscore_rig(BwParams p, RigDscore rig) { k_dscore_body<true>(p, rig); }
 
 // ------------------------------------------------------------------ implicit-function derivatives (DSAC_DERIV_IMPLICIT)
 // dRefine / dObj of a refined pose: the IFT of the last accepted refinement step's fit over the cells it fitted (ift.cuh),
@@ -789,8 +801,11 @@ struct IftScratch {
     int32_t* count = nullptr;    // [n]
 };
 
-template <bool PER_FRAME, bool RGBD>
-__device__ __forceinline__ void k_refine_ift_body(const IftParams& p) {
+// RIG (k_refine_ift_rig, the rig backward): job r is rig r of rig.C cameras, pose the rig's, sel entries cam << 11 | cell
+// at a stride of C K4_MAX_INLIERS (k_refine_rig_rec).  A cell is set up in its own camera frame and mapped to the rig frame
+// (ift_point_to_rig); its row is its camera frame's, and drefobj is [R][6][C N 3], camera-major.
+template <bool PER_FRAME, bool RGBD, bool RIG = false>
+__device__ __forceinline__ void k_refine_ift_body(const IftParams& p, RigRefine rig = RigRefine{}) {
     __shared__ double s_red[IFT_WARPS][32];
     __shared__ double s_W[36], s_v[6];
     __shared__ int s_ok;
@@ -800,13 +815,28 @@ __device__ __forceinline__ void k_refine_ift_body(const IftParams& p) {
     if (frame < 0) return;
     const Cam cam = frame_cam<PER_FRAME>(p, frame);
     const int cnt = p.count[job];
-    const uint16_t* sel = p.sel + (size_t)job * K4_MAX_INLIERS;
+    const int n_cams = RIG ? rig.C : 1;
+    const size_t width = (size_t)n_cams * DSAC_N_CONST * 3;   // row / drefobj columns of a job
+    const uint16_t* sel = p.sel + (size_t)job * n_cams * K4_MAX_INLIERS;
     const int16_t* coords = p.coords + (size_t)frame * DSAC_N_CONST * 3;
     const int32_t* pix = p.pix + (size_t)frame * p.pix_stride;
     double pose[6], R[9];
     for (int k = 0; k < 6; k++) pose[k] = p.pose[(size_t)job * 6 + k];
     rodrigues_v2m(pose, R);
     auto point = [&](int i, IftPoint& P) {
+        if constexpr (RIG) {
+            const int code = sel[i], fr = frame * n_cams + (code >> 11), cell = code & 2047;
+            const int16_t* co = p.coords + ((size_t)fr * DSAC_N_CONST + cell) * 3;
+            const int32_t* px = p.pix + (size_t)fr * p.pix_stride + cell * 2;
+            const double Y[3] = {(double)co[0], (double)co[1], (double)co[2]}, e[3] = {(double)px[0], (double)px[1], 0};
+            const double* E = rig.ext + (size_t)fr * 12;
+            double Rk[9], tk[3];
+            rig_compose(E, E + 9, R, pose + 3, Rk, tk);
+            const Cam cm = frame_cam<PER_FRAME>(p, fr);
+            ift_point_setup(Rk, tk, Y, e, cm.f, cm.cx, cm.cy, false, P);
+            ift_point_to_rig(E, P);
+            return;
+        }
         const int c = sel[i];
         const double Y[3] = {(double)coords[c * 3], (double)coords[c * 3 + 1], (double)coords[c * 3 + 2]};
         double e[3];
@@ -864,9 +894,9 @@ __device__ __forceinline__ void k_refine_ift_body(const IftParams& p) {
     }
     __syncthreads();
     const bool ok = s_ok != 0;
-    double* row = p.row ? p.row + (size_t)frame * DSAC_N_CONST * 3 : nullptr;
+    double* row = p.row ? p.row + (size_t)frame * width : nullptr;
     for (int i = tid; i < cnt; i += IFT_THREADS) {
-        const int c = sel[i];
+        const int c = RIG ? (sel[i] >> 11) * DSAC_N_CONST + (sel[i] & 2047) : sel[i];   // column / 3 within the job's width
         double o[3] = {0, 0, 0};
         if (ok) {
             IftPoint P;
@@ -882,7 +912,7 @@ __device__ __forceinline__ void k_refine_ift_body(const IftParams& p) {
                 double D[18];
                 ift_point_deriv(s_W, B, D);
                 for (int k = 0; k < 6; k++)
-                    for (int j = 0; j < 3; j++) p.drefobj[((size_t)frame * 6 + k) * DSAC_N_CONST * 3 + c * 3 + j] = D[k * 3 + j];
+                    for (int j = 0; j < 3; j++) p.drefobj[((size_t)frame * 6 + k) * width + c * 3 + j] = D[k * 3 + j];
             }
         }
         for (int j = 0; j < 3; j++) {
@@ -895,6 +925,9 @@ __global__ void __launch_bounds__(IFT_THREADS) k_refine_ift(IftParams p) { k_ref
 __global__ void __launch_bounds__(IFT_THREADS) k_refine_ift_cam(IftParams p) { k_refine_ift_body<true, false>(p); }
 __global__ void __launch_bounds__(IFT_THREADS) k_refine_ift_rgbd(IftParams p) { k_refine_ift_body<false, true>(p); }
 __global__ void __launch_bounds__(IFT_THREADS) k_refine_ift_rgbd_cam(IftParams p) { k_refine_ift_body<true, true>(p); }
+__global__ void __launch_bounds__(IFT_THREADS) k_refine_ift_rig(IftParams p, RigRefine rig) { k_refine_ift_body<false, false, true>(p, rig); }
+__global__ void __launch_bounds__(IFT_THREADS) k_refine_ift_rig_cam(IftParams p, RigRefine rig) { k_refine_ift_body<true, false, true>(p, rig); }
+constexpr void (*k_refine_ift_rig_tab[2])(IftParams, RigRefine) = {k_refine_ift_rig, k_refine_ift_rig_cam};
 
 inline void launch_refine_ift(const IftParams& p, unsigned jobs, cudaStream_t stream) {
     // [per-frame camera][RGB-D]

@@ -155,6 +155,7 @@ struct Pass {
     unsigned long long gen[SET_COUNT] = {};
     int set_n[SET_COUNT] = {};
     int prior_k = 0;                // priors per frame
+    int rig_c = 0;                  // a rig pass's cameras per rig (its gt: the rig ground truth, null without DSAC_STAGE_EVAL)
     bool rgbd() const { return set_n[SET_DEPTH] > 0; }
 };
 
@@ -268,6 +269,18 @@ struct dsac_engine {
         uint32_t* status;
     } rig = {};
     DevMem<char> rig_buf;
+    // dsac_backward_rig(_pose)_device: the soft-argmax backward's arrays over rigs and pools, the recording replay, the
+    // composed poses, w and the support vectors, in one grow-only block that no other call writes, ordered by ev_rig_bw as
+    // the uncertainty scratch is by ev_unc
+    struct {
+        BackwardScratch b;
+        double *rec_pose, *w, *u, *frame_grad;
+        uint16_t* rec_sel;
+        int32_t *rec_count, *n_perm;
+        uint32_t* status;
+    } rig_bw = {};
+    DevMem<char> rig_bw_buf;
+    Event ev_rig_bw;
     std::vector<DevMem<char>> bw_pool;   // device buffers of dsac_backward_dsac, kept across calls
     Stream pipe[4];                 // chunked H2D / compute / D2H pipeline of dsac_forward
     // tail split (dsac_set_tail_split): the whole sampler waves of a batch run on a high-priority side stream, the
@@ -648,6 +661,7 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
         CUC(cudaEventCreateWithFlags(e->ev_fwd.put(), cudaEventDisableTiming));
         CUC(cudaEventCreateWithFlags(e->ev_unc.put(), cudaEventDisableTiming));
         CUC(cudaEventCreateWithFlags(e->ev_modes.put(), cudaEventDisableTiming));
+        CUC(cudaEventCreateWithFlags(e->ev_rig_bw.put(), cudaEventDisableTiming));
         if (const char* ts = getenv("DSAC_TAIL_SPLIT")) e->tail_split = atoi(ts);
     }
 #undef CUC
@@ -758,10 +772,10 @@ static int pass_begin(dsac_engine* e, int32_t kind, int32_t n, int64_t frame0, c
     return DSAC_OK;
 }
 
-// What a consumer of the held pass needs.  kinds: a pass of the soft-argmax pipeline, the DSAC one, or either, over the
-// same n frames; or PASS_GUIDED, a guided pass over n frames.  settings (1 << SET_*): those whose change since the pass
-// makes it stale for the consumer.
-enum { PASS_SOFTAM = 1, PASS_DSAC = 2, PASS_EITHER = 3, PASS_GUIDED = 4 };
+// What a consumer of the held pass needs.  kinds: a pass of the soft-argmax pipeline, the DSAC one, or either, or a rig
+// pass, over the same n frames; or PASS_GUIDED, a guided pass over n frames.  settings (1 << SET_*): those whose change
+// since the pass makes it stale for the consumer.
+enum { PASS_SOFTAM = 1, PASS_DSAC = 2, PASS_EITHER = 3, PASS_GUIDED = 4, PASS_RIG = 8 };
 constexpr unsigned SETTINGS_GEOMETRY = 1u << SET_CAMS | 1u << SET_DEPTH | 1u << SET_PRIORS;
 constexpr unsigned SETTINGS_SAMPLING = 1u << SET_LOGITS | 1u << SET_DEPTH | 1u << SET_PRIORS;
 
@@ -784,10 +798,12 @@ static int pass_check(dsac_engine* e, const char* who, int32_t n, unsigned kinds
     // the consumers of either pipeline's poses report a stale setting before a missing pass, the backward passes after it
     if (kinds == PASS_EITHER)
         if (int rc = unchanged()) return rc;
-    const unsigned held = p.kind == DSAC_PASS_SOFTAM ? PASS_SOFTAM : p.kind == DSAC_PASS_DSAC ? PASS_DSAC : 0;
+    const unsigned held = p.kind == DSAC_PASS_SOFTAM ? PASS_SOFTAM : p.kind == DSAC_PASS_DSAC ? PASS_DSAC
+                        : p.kind == DSAC_PASS_RIG ? PASS_RIG : 0;
     if (n < 1 || p.n != n || !(held & kinds))
         return fail(e, DSAC_ERR_ARG, "%s must follow %s over the same %d frames", who,
-                    kinds == PASS_SOFTAM ? "a dsac_forward" : kinds == PASS_DSAC ? "a dsac_forward_dsac" : "a forward pass", n);
+                    kinds == PASS_SOFTAM ? "a dsac_forward" : kinds == PASS_DSAC ? "a dsac_forward_dsac"
+                    : kinds == PASS_RIG ? "a dsac_forward_rig_device" : "a forward pass", n);
     return kinds == PASS_EITHER ? DSAC_OK : unchanged();
 }
 
@@ -2124,3 +2140,4 @@ static int carve_scratch(dsac_engine* e, DevMem<char>& buf, std::initializer_lis
 #include "uncertainty_host.inc"
 #include "modes_host.inc"
 #include "rig_host.inc"
+#include "rig_backward_host.inc"

@@ -172,6 +172,117 @@ DSAC_HD void so3_jl_inv(const double r[3], double Ji[9]) {
         }
 }
 
+// Left Jacobian of SO(3) at rotation vector r: I + a [r]x + b [r]x^2, a = (1 - cos th) / th^2, b = (th - sin th) / th^3
+DSAC_HD void so3_jl(const double r[3], double J[9]) {
+    const double th2 = r[0] * r[0] + r[1] * r[1] + r[2] * r[2], th = sqrt(th2);
+    const double a = th < 1e-4 ? 0.5 - th2 / 24 : (1 - cos(th)) / th2;
+    const double b = th < 1e-4 ? 1.0 / 6 - th2 / 120 : (th - sin(th)) / (th2 * th);
+    const double K[9] = {0, -r[2], r[1], r[2], 0, -r[0], -r[1], r[0], 0};
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) {
+            double k2 = 0;
+            for (int k = 0; k < 3; k++) k2 += K[i * 3 + k] * K[k * 3 + j];
+            J[i * 3 + j] = (i == j ? 1.0 : 0.0) + a * K[i * 3 + j] + b * k2;
+        }
+}
+
+// d r_out / d r of r_out = log(A exp([r]x)) for a fixed rotation A: exp([Jl(r) dr]x) exp([r]x) = exp([r + dr]x) to first
+// order, and A exp([v]x) = exp([A v]x) A, so Jl(r_out) dr_out = A Jl(r) dr.  K = Jl(r_out)^-1 A Jl(r) (3 x 3).
+DSAC_HD void so3_left_mul_jac(const double A[9], const double r[3], const double r_out[3], double K[9]) {
+    double Jl[9], Ji[9], T[9];
+    so3_jl(r, Jl);
+    so3_jl_inv(r_out, Ji);
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) T[i * 3 + j] = A[i * 3] * Jl[j] + A[i * 3 + 1] * Jl[3 + j] + A[i * 3 + 2] * Jl[6 + j];
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) K[i * 3 + j] = Ji[i * 3] * T[j] + Ji[i * 3 + 1] * T[3 + j] + Ji[i * 3 + 2] * T[6 + j];
+}
+
+// ---- multi-camera rigs (the rig backward, rig.cuh).  A camera's extrinsic (Rc, tc) maps rig coordinates to its own,
+// X_cam = Rc X_rig + tc (pose_math.cuh's rig_compose / rig_lift).
+
+// The rig pool's lift as a function of the camera hypothesis, L = d lift(T, E) / d T (6 x 6, row-major) in the cv 6-vector
+// (rvec, tvec) in which the rig's soft-argmax averages its pool: lift (R, t) = (Rc^T R, Rc^T (t - tc)) has the rotation
+// block so3_left_mul_jac(Rc^T) and the translation block Rc^T.  r: the hypothesis' rvec.  An extrinsic rotation that is
+// exactly I (a zero rvec) gives L = I exactly, as the lift then keeps the hypothesis' rvec.
+DSAC_HD void rig_lift_jac(const double Rc[9], const double r[3], double L[36]) {
+    for (int k = 0; k < 36; k++) L[k] = 0;
+    bool ident = true;
+    for (int k = 0; k < 9; k++) ident = ident && Rc[k] == (k % 4 == 0 ? 1.0 : 0.0);
+    if (ident) {
+        for (int k = 0; k < 6; k++) L[k * 7] = 1;
+        return;
+    }
+    double Rt[9], Rh[9], Rr[9], rr[3], K[9];
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) Rt[i * 3 + j] = Rc[j * 3 + i];
+    rodrigues_v2m(r, Rh);
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) Rr[i * 3 + j] = Rt[i * 3] * Rh[j] + Rt[i * 3 + 1] * Rh[3 + j] + Rt[i * 3 + 2] * Rh[6 + j];
+    rodrigues_m2v(Rr, rr);
+    so3_left_mul_jac(Rt, r, rr, K);
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) {
+            L[i * 6 + j] = K[i * 3 + j];
+            L[(3 + i) * 6 + 3 + j] = Rt[i * 3 + j];
+        }
+}
+
+// Camera c's pose of the pool slot that camera c2's hypothesis T = (Rh, th) (cv) lifts to, as a function of T, both in the
+// jp 6-vector (rodrigues(D R), D t; D = diag(1, -1, -1)): T_c o lift(T, E_c2) = (A Rh, A th + b) with A = Rc Rc2^T, so
+// K = d jp(T_c o lift(T, E_c2)) / d jp(T) (6 x 6) has the rotation block so3_left_mul_jac(D A D) at the jp rotation
+// vectors and the translation block D A D.  same: c == c2, where the composition is T itself and K = I exactly.
+DSAC_HD void rig_cross_jac(const double Rc[9], const double Rc2[9], const double Rh[9], bool same, double K[36]) {
+    for (int k = 0; k < 36; k++) K[k] = 0;
+    if (same) {
+        for (int k = 0; k < 6; k++) K[k * 7] = 1;
+        return;
+    }
+    double A[9], Aj[9], Rj[9], Ro[9], r[3], ro[3], Kr[9];
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) A[i * 3 + j] = Rc[i * 3] * Rc2[j * 3] + Rc[i * 3 + 1] * Rc2[j * 3 + 1] + Rc[i * 3 + 2] * Rc2[j * 3 + 2];
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) {
+            Aj[i * 3 + j] = ((i == 0) == (j == 0) ? 1.0 : -1.0) * A[i * 3 + j];   // D A D
+            Rj[i * 3 + j] = (i == 0 ? 1.0 : -1.0) * Rh[i * 3 + j];                // D Rh
+        }
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) Ro[i * 3 + j] = Aj[i * 3] * Rj[j] + Aj[i * 3 + 1] * Rj[3 + j] + Aj[i * 3 + 2] * Rj[6 + j];
+    rodrigues_m2v(Rj, r);
+    rodrigues_m2v(Ro, ro);
+    so3_left_mul_jac(Aj, r, ro, Kr);
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) {
+            K[i * 6 + j] = Kr[i * 3 + j];
+            K[(3 + i) * 6 + 3 + j] = Aj[i * 3 + j];
+        }
+}
+
+// A rig's fit (k_refine_rig) over cells of several cameras: the residual of a cell of camera c is its camera-frame
+// residual at X_cam = Rc X + tc, X = R Y + t in the rig frame.  The map is linear, so a point set up in its camera frame
+// (ift_point_setup at the composed pose (Rc R, Rc t + tc)) becomes the rig frame's exactly: q = R Y = Rc^T q_cam,
+// g_m -> Rc^T g_m, gs -> Rc^T gs, Gs -> Rc^T Gs Rc.  ift_point_hess and ift_point_cross (with the rig's R) then
+// differentiate the rig pose.  An identity Rc changes no bit.
+DSAC_HD void ift_point_to_rig(const double Rc[9], IftPoint& P) {
+    double q[3];
+    for (int k = 0; k < 3; k++) q[k] = P.q[0] * Rc[k] + P.q[1] * Rc[3 + k] + P.q[2] * Rc[6 + k];
+    for (int k = 0; k < 3; k++) P.q[k] = q[k];
+    for (int m = 0; m < 3; m++) {
+        double g[3];
+        for (int k = 0; k < 3; k++) g[k] = P.g[m][0] * Rc[k] + P.g[m][1] * Rc[3 + k] + P.g[m][2] * Rc[6 + k];
+        for (int k = 0; k < 3; k++) P.g[m][k] = g[k];
+    }
+    double gs[3];
+    for (int k = 0; k < 3; k++) gs[k] = P.gs[0] * Rc[k] + P.gs[1] * Rc[3 + k] + P.gs[2] * Rc[6 + k];
+    const double G[9] = {P.Gs[0], P.Gs[1], P.Gs[2], P.Gs[1], P.Gs[3], P.Gs[4], P.Gs[2], P.Gs[4], P.Gs[5]};
+    double T[9];   // G Rc
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) T[i * 3 + j] = G[i * 3] * Rc[j] + G[i * 3 + 1] * Rc[3 + j] + G[i * 3 + 2] * Rc[6 + j];
+    auto at = [&](int i, int j) { return Rc[i] * T[j] + Rc[3 + i] * T[3 + j] + Rc[6 + i] * T[6 + j]; };   // (Rc^T G Rc)_ij
+    P.Gs[0] = at(0, 0); P.Gs[1] = at(0, 1); P.Gs[2] = at(0, 2); P.Gs[3] = at(1, 1); P.Gs[4] = at(1, 2); P.Gs[5] = at(2, 2);
+    for (int k = 0; k < 3; k++) P.gs[k] = gs[k];
+}
+
 // M = d jp6 / d xi (6 x 6, row-major) at the cv pose (rvec, tvec); R gets the cv rotation
 DSAC_HD void ift_jp_jacobian(const double pose[6], double R[9], double M[36]) {
     rodrigues_v2m(pose, R);

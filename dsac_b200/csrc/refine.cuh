@@ -142,11 +142,12 @@ __device__ double max_loss_dev(const double R1[9], const double t1[3], const dou
 // composed pose (rig_compose), the selection is each camera's first inlier_count flagged cells in turn (entries cam << 11 |
 // cell), an LM point is reprojected in its own camera (lm_point_contrib_ext), and the inlier maps are the cameras' frames.
 // The cells are read from global memory rather than staged: C frames do not fit in shared memory.  A rig with
-// DSAC_ST_BAD_RIG in status gets zero outputs.
+// DSAC_ST_BAD_RIG in status gets zero outputs.  RIG with RECORD (k_refine_rig_rec, the rig backward) records those entries
+// at a stride of C K4_MAX_INLIERS per rig.
 template <bool PER_FRAME, bool RGBD = false, bool RECORD = false, bool RIG = false>
 __device__ __forceinline__ void k_refine_body(const RefineParams& p, const double* eye = nullptr, uint16_t* rec_sel = nullptr,
                                               int32_t* rec_count = nullptr, RigRefine rig = RigRefine{}) {
-    static_assert(!(RIG && (RGBD || RECORD)), "a rig refines RGB frames without recording");
+    static_assert(!(RIG && RGBD), "a rig refines RGB frames");
     constexpr int NC = RIG ? RIG_MAX_CAMERAS : 1;   // camera frames per job, at most
     // the frame's scene coordinates (int16 mm, this job's perturbation applied) and pixel positions, staged once per job:
     // every refinement step reads all of them for the inlier flags and the selected ones in each LM pass
@@ -161,7 +162,7 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p, const doubl
     __shared__ double s_sum[2][32];
     __shared__ int s_count, s_ctl;
     __shared__ int s_rec_count;                               // (RECORD only)
-    __shared__ unsigned short s_rec[RECORD ? K4_MAX_INLIERS : 1];
+    __shared__ unsigned short s_rec[RECORD ? NC * K4_MAX_INLIERS : 1];
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int job = blockIdx.x;
@@ -177,6 +178,7 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p, const doubl
                 if (p.steps_done) p.steps_done[job] = 0;
                 if (p.n_perm_steps) p.n_perm_steps[job] = 0;
                 if (p.gt_jp) { p.loss[job] = 0; p.rot_err[job] = 0; p.t_err[job] = 0; p.correct[job] = 0; }
+                if constexpr (RECORD) rec_count[job] = 0;
             }
             return;
         }
@@ -488,7 +490,8 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p, const doubl
     if (tid < 6) p.out_pose[(size_t)job * 6 + tid] = s_pose[tid];
     if constexpr (RECORD) {
         const int rc = s_rec_count;
-        for (int i = tid; i < rc; i += K4_THREADS) rec_sel[(size_t)job * K4_MAX_INLIERS + i] = s_rec[i];
+        const size_t stride = RIG ? (size_t)n_cams * K4_MAX_INLIERS : (size_t)K4_MAX_INLIERS;
+        for (int i = tid; i < rc; i += K4_THREADS) rec_sel[(size_t)job * stride + i] = s_rec[i];
         if (tid == 0) rec_count[job] = rc;
     }
     if (p.inlier_map)
@@ -551,6 +554,13 @@ __global__ void __launch_bounds__(K4_THREADS, 2) k_refine_rig(RefineParams p, Ri
 __global__ void __launch_bounds__(K4_THREADS, 2) k_refine_rig_cam(RefineParams p, RigRefine rig) {
     k_refine_body<true, false, false, true>(p, nullptr, nullptr, nullptr, rig);
 }
+// the rig's recording replay (rec_sel [n_jobs][C K4_MAX_INLIERS] of entries cam << 11 | cell, rec_count [n_jobs])
+__global__ void __launch_bounds__(K4_THREADS, 2) k_refine_rig_rec(RefineParams p, RigRefine rig, uint16_t* rec_sel, int32_t* rec_count) {
+    k_refine_body<false, false, true, true>(p, nullptr, rec_sel, rec_count, rig);
+}
+__global__ void __launch_bounds__(K4_THREADS, 2) k_refine_rig_rec_cam(RefineParams p, RigRefine rig, uint16_t* rec_sel, int32_t* rec_count) {
+    k_refine_body<true, false, true, true>(p, nullptr, rec_sel, rec_count, rig);
+}
 
 // the instantiations by per-frame camera (RefineParams::cams), one table per signature
 constexpr void (*k_refine_tab[2])(RefineParams) = {k_refine, k_refine_cam};
@@ -558,6 +568,7 @@ constexpr void (*k_refine_rgbd_tab[2])(RefineParams, const double*) = {k_refine_
 constexpr void (*k_refine_rec_tab[2])(RefineParams, uint16_t*, int32_t*) = {k_refine_rec, k_refine_rec_cam};
 constexpr void (*k_refine_rgbd_rec_tab[2])(RefineParams, const double*, uint16_t*, int32_t*) = {k_refine_rgbd_rec, k_refine_rgbd_rec_cam};
 constexpr void (*k_refine_rig_tab[2])(RefineParams, RigRefine) = {k_refine_rig, k_refine_rig_cam};
+constexpr void (*k_refine_rig_rec_tab[2])(RefineParams, RigRefine, uint16_t*, int32_t*) = {k_refine_rig_rec, k_refine_rig_rec_cam};
 
 // one CTA per job, with the instantiation the parameters ask for; eye != null: an RGB-D pass
 inline void launch_refine(const RefineParams& p, unsigned jobs, cudaStream_t stream, const double* eye = nullptr) {

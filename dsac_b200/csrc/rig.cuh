@@ -8,10 +8,19 @@
 //   k_score_rig  (k_score without its softmax tail) every camera frame against its rig's pool of P = C H poses;
 //   k_rig_tail   the rig's score of slot j is the sum of its cameras' scores in camera order, then softargmax_tail;
 //   k_refine_rig the refinement of the soft-argmax rig pose over all cameras' cells (refine.cuh).
+// The rig backward (dsac_backward_rig_device, rig_backward_host.inc) is the soft-argmax backward's implicit chain over the
+// pool: k_bw_prep_implicit, k_refine_rig_rec and the 12 dRefineHyp jobs of k_refine_rig, k_bw_combine_implicit and
+// k_refine_ift_rig per rig; k_dpnp_ift per frame; then
+//   k_rig_bw_hypjp    the composed pose T_c o T_j of every (frame, slot) in jp with its Rodrigues Jacobian;
+//   k_dscore_rig      every camera frame against its rig's pool: the direct part into the frame's row, w per (frame, slot);
+//   k_rig_bw_support  per (frame, hypothesis) the 1x6 of path I (dLdAvg L_j) and of path II (sum_c w K_c,j);
+//   k_rig_bw_scatter  per frame, hypotheses in order: both through dPNP onto the minimal set's cells.
 #pragma once
 #include <cuda_runtime.h>
 
+#include "backward.cuh"
 #include "camera.cuh"
+#include "ift.cuh"
 #include "kernels.cuh"
 #include "pose_math.cuh"
 #include "refine.cuh"
@@ -127,6 +136,125 @@ __global__ void __launch_bounds__(K2_THREADS) k_rig_tail(RigTailParams p) {
     }
     __syncthreads();
     softargmax_tail(p.sp, r, s_red);
+}
+
+struct RigBwParams {
+    int C, H, P, fix_q4;
+    const double* ext;          // [n][12] Rc (row-major), tc (k_rig_lift)
+    const double* rig_hyp;      // [R][P][6] the pool (cv)
+    const double* hyp_pose;     // [n][H][6] the frames' hypotheses (cv)
+    const int32_t* img_idx;     // [n][H][4]
+    const double* sf;           // [R][P]
+    const uint32_t* status;     // [R]
+    const double* dldavg;       // [R][6] dLoss/dAvg (k_bw_combine_implicit)
+    const double* dpnp;         // [n][H][72] (k_dpnp_ift)
+    const double* w;            // [n][P][6] (k_dscore_rig)
+    double* hypjp;              // [n][P][39]
+    double* u;                  // [n][H][12] the two 1x6 of each hypothesis' support scatter
+    double* row;                // [n][N * 3]
+};
+constexpr int RIG_BW_THREADS = 128;
+
+// Grid (ceil(P / 128), n): camera frame f's pose of pool slot j, T_c o T_j, as k_dscore reads a hypothesis (write_hypjp):
+// R, t of cv2our and the Rodrigues Jacobian at its rotation vector.  An identity extrinsic changes no bit (rig_compose),
+// so with C = 1 this is write_hypjp's output.
+__global__ void __launch_bounds__(RIG_BW_THREADS) k_rig_bw_hypjp(RigBwParams p) {
+    const int j = blockIdx.x * RIG_BW_THREADS + threadIdx.x, f = blockIdx.y;
+    if (j >= p.P) return;
+    const double* hp = p.rig_hyp + ((size_t)(f / p.C) * p.P + j) * 6;
+    const double* E = p.ext + (size_t)f * 12;
+    double Rr[9], R[9], t[3], rod[3], Rt[9], J[27];
+    rodrigues_v2m(hp, Rr);
+    rig_compose(E, E + 9, Rr, hp + 3, R, t);
+    // cv2our_dev on the composed pose
+    t[1] = -t[1]; t[2] = -t[2];
+    for (int k = 3; k < 9; k++) R[k] = -R[k];
+    const double det = R[0] * (R[4] * R[8] - R[5] * R[7]) - R[1] * (R[3] * R[8] - R[5] * R[6]) + R[2] * (R[3] * R[7] - R[4] * R[6]);
+    if (det < 0) {
+        for (int k = 0; k < 9; k++) R[k] = -R[k];
+        for (int k = 0; k < 3; k++) t[k] = -t[k];
+    }
+    if (t[0] != t[0] || t[1] != t[1] || t[2] != t[2]) t[0] = t[1] = t[2] = 0;
+    rodrigues_m2v(R, rod);
+    rodrigues_jac(rod, Rt, J);
+    double* hj = p.hypjp + ((size_t)f * p.P + j) * 39;
+    for (int k = 0; k < 9; k++) hj[k] = R[k];
+    for (int k = 0; k < 3; k++) hj[9 + k] = t[k];
+    for (int k = 0; k < 27; k++) hj[12 + k] = J[k];
+}
+
+// Grid (ceil(H / 128), n): hypothesis h of frame f' = r C + c' (pool slot j = c' H + h) moves, through its minimal set, the
+// pool pose j.  Path I's 1x6 is dLdAvg_r L_j (the slot's sf_j is applied in the scatter, as k_bw_scatter_pnp applies it),
+// path II's sum over the rig's cameras c of w[r C + c][j] K_c,j (rig_lift_jac, rig_cross_jac in ift.cuh).  A bad rig's are
+// zero.
+__global__ void __launch_bounds__(RIG_BW_THREADS) k_rig_bw_support(RigBwParams p) {
+    const int h = blockIdx.x * RIG_BW_THREADS + threadIdx.x, f = blockIdx.y;
+    if (h >= p.H) return;
+    const int C = p.C, r = f / C, c2 = f - r * C, j = c2 * p.H + h;
+    double* u = p.u + ((size_t)f * p.H + h) * 12;
+    if (p.status[r] & RIG_ST_BAD) {
+        for (int k = 0; k < 12; k++) u[k] = 0.0;
+        return;
+    }
+    const double* hp = p.hyp_pose + ((size_t)f * p.H + h) * 6;
+    const double* E2 = p.ext + (size_t)f * 12;
+    double M[36], Rh[9], o[12];
+    rig_lift_jac(E2, hp, M);
+    const double* dld = p.dldavg + (size_t)r * 6;
+    for (int m = 0; m < 6; m++) {
+        double s = 0;
+        for (int k = 0; k < 6; k++) s += dld[k] * M[k * 6 + m];
+        o[m] = s;
+        o[6 + m] = 0;
+    }
+    rodrigues_v2m(hp, Rh);
+    for (int c = 0; c < C; c++) {
+        rig_cross_jac(p.ext + (size_t)(r * C + c) * 12, E2, Rh, c == c2, M);
+        const double* w = p.w + ((size_t)(r * C + c) * p.P + j) * 6;
+        for (int m = 0; m < 6; m++) {
+            double s = 0;
+            for (int k = 0; k < 6; k++) s += w[k] * M[k * 6 + m];
+            o[6 + m] += s;
+        }
+    }
+    for (int k = 0; k < 12; k++) u[k] = o[k];
+}
+
+// One warp per frame f': its hypotheses in order, lanes 0..11 = (point, channel) of the minimal set, dPNP applied to
+// both 1x6 of k_rig_bw_support -- path I onto the cells as k_bw_scatter_pnp puts them, path II in the layout of quirk
+// Q4 as k_dscore's support scatter (fix_q4) -- with no atomics, so the rows are run-to-run identical.  Last in the chain:
+// it zeroes the rows of a bad rig's frames.
+__global__ void __launch_bounds__(32) k_rig_bw_scatter(RigBwParams p) {
+    const int f = blockIdx.x, lane = threadIdx.x, r = f / p.C, c2 = f - r * p.C;
+    double* row = p.row + (size_t)f * DSAC_N_CONST * 3;
+    if (p.status[r] & RIG_ST_BAD) {
+        for (int i = lane; i < DSAC_N_CONST * 3; i += 32) row[i] = 0.0;
+        return;
+    }
+    if (lane >= 12) return;
+    for (int h = 0; h < p.H; h++) {
+        const size_t fh = (size_t)f * p.H + h;
+        const int c = p.img_idx[fh * 4 + lane / 3];
+        const double* J = p.dpnp + fh * 72;
+        const double* u = p.u + fh * 12;
+        const double sf = p.sf[(size_t)r * p.P + c2 * p.H + h];
+        double s1 = 0, s2 = 0;
+        for (int k = 0; k < 6; k++) s1 += u[k] * (sf * J[k * 12 + lane]);
+        for (int k = 0; k < 6; k++) s2 += u[6 + k] * J[k * 12 + lane];
+        if (c >= 0) row[c * 3 + lane % 3] += s1;
+        __syncwarp(0xfff);
+        if (c >= 0) {
+            const int x = c % DSAC_GRID_CONST, y = c / DSAC_GRID_CONST;
+            row[(p.fix_q4 ? c : x * DSAC_GRID_CONST + y) * 3 + lane % 3] += s2;   // quirk Q4
+        }
+        __syncwarp(0xfff);
+    }
+}
+
+// the per-rig loss gradient [R] read per frame [n], as k_e2e_grad indexes it
+__global__ void k_rig_frame_grad(const double* __restrict__ g, int C, int n, double* __restrict__ out) {
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f < n) out[f] = g[f / C];
 }
 
 }  // namespace dsac

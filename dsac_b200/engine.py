@@ -34,6 +34,7 @@ EXPORTS = [
     "dsac_set_sampling_logits_device", "dsac_set_cell_depth_device", "dsac_sampling_table_device", "dsac_sampling_log_prob_device",
     "dsac_sampling_log_prob_backward_device", "dsac_set_coord_derivatives", "dsac_pose_uncertainty_device",
     "dsac_last_pass", "dsac_set_pose_priors_device", "dsac_pose_modes_device", "dsac_forward_rig_device",
+    "dsac_backward_rig_device", "dsac_backward_rig_pose_device", "dsac_rig_refined_jp6_device",
 ]
 
 ST_OBJ_DRAW_EXHAUSTED = 8    # DSAC_ST_OBJ_DRAW_EXHAUSTED
@@ -158,6 +159,13 @@ class RigOut(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in _RIG_FIELDS]
 
 
+_RIG_BW_FIELDS = ("dloss_dref", "dref_dhyp", "score_grads", "dref_dobj")
+
+
+class RigBackwardOut(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in _RIG_BW_FIELDS]
+
+
 SCORE_HOOK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p)
 SCORE_BACKWARD_HOOK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p)
 
@@ -230,6 +238,10 @@ def load(build_if_missing=True):
                                            C.c_void_p]
     lib.dsac_forward_rig_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32,
                                             C.c_void_p, C.c_void_p, C.POINTER(RigOut), C.c_void_p]
+    lib.dsac_backward_rig_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float,
+                                             C.POINTER(RigBackwardOut), C.c_void_p]
+    lib.dsac_backward_rig_pose_device.argtypes = lib.dsac_backward_rig_device.argtypes
+    lib.dsac_rig_refined_jp6_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.dsac_backward_pose_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]
     lib.dsac_backward_dsac_pose_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(BackwardDsacOut),
                                                    C.c_void_p, C.c_float, C.c_void_p]
@@ -669,6 +681,39 @@ class Engine:
         self._check(self.lib.dsac_forward_rig_device(self.h, n, n_cameras, frame0, C.c_void_p(d_coords), C.c_void_p(d_pix),
                                                      pix_shared, C.c_void_p(d_cam_from_rig), C.c_void_p(d_gt_rig) if d_gt_rig else None,
                                                      C.byref(raw), C.c_void_p(stream) if stream else None))
+
+    def _rig_diag(self, ptrs):
+        raw = RigBackwardOut()
+        for k, v in ptrs.items():
+            if k not in _RIG_BW_FIELDS:
+                raise KeyError(k)
+            setattr(raw, k, v)
+        return raw
+
+    def backward_rig_device(self, n, d_loss_grad=None, d_dloss_dobj=None, d_dloss_dpred=None, clamp=0.0, stream=None, **ptrs):
+        """dsac_backward_rig_device (raw device pointers as ints): the loss form of the rig backward after forward_rig_device
+        over n frames (INTEGRATION.md, "Rig gradients"); d_loss_grad [R] (None: 1); ptrs: device destinations of the fields
+        of dsac_rig_backward_out (dloss_dref, dref_dhyp, score_grads, dref_dobj)."""
+        raw = self._rig_diag(ptrs)
+        self._check(self.lib.dsac_backward_rig_device(self.h, n, C.c_void_p(d_loss_grad) if d_loss_grad else None,
+                                                      C.c_void_p(d_dloss_dobj) if d_dloss_dobj else None,
+                                                      C.c_void_p(d_dloss_dpred) if d_dloss_dpred else None, C.c_float(clamp),
+                                                      C.byref(raw), C.c_void_p(stream) if stream else None))
+
+    def backward_rig_pose_device(self, n, d_grad_ref, d_dloss_dobj=None, d_dloss_dpred=None, clamp=0.0, stream=None, **ptrs):
+        """dsac_backward_rig_pose_device (raw device pointers as ints): the rig backward seeded by dOuter/d(refined rig jp6)
+        [R][6]; ptrs as backward_rig_device."""
+        raw = self._rig_diag(ptrs)
+        self._check(self.lib.dsac_backward_rig_pose_device(self.h, n, C.c_void_p(d_grad_ref) if d_grad_ref else None,
+                                                           C.c_void_p(d_dloss_dobj) if d_dloss_dobj else None,
+                                                           C.c_void_p(d_dloss_dpred) if d_dloss_dpred else None, C.c_float(clamp),
+                                                           C.byref(raw), C.c_void_p(stream) if stream else None))
+
+    def rig_refined_jp6_device(self, n, d_jp6, stream=None):
+        """dsac_rig_refined_jp6_device (raw device pointers as ints): jp 6-vectors [R][6] of the refined rig poses of the
+        preceding forward_rig_device over n frames."""
+        self._check(self.lib.dsac_rig_refined_jp6_device(self.h, n, C.c_void_p(d_jp6) if d_jp6 else None,
+                                                         C.c_void_p(stream) if stream else None))
 
     def last_pass(self, n):
         """dsac_last_pass: "softam", "dsac" or "rig", the kind of the pass over n frames the engine holds (what

@@ -427,7 +427,7 @@ int dsac_pose_uncertainty_device(dsac_engine* e, int32_t n_frames, const dsac_po
  * pass over n_frames. */
 #define DSAC_PASS_SOFTAM 1
 #define DSAC_PASS_DSAC 2
-#define DSAC_PASS_RIG 3            /* dsac_forward_rig_device: no backward pass or pose query reads it */
+#define DSAC_PASS_RIG 3            /* dsac_forward_rig_device: read by the rig backward and dsac_rig_refined_jp6_device only */
 int dsac_last_pass(dsac_engine* e, int32_t n_frames, int32_t* pipeline);
 
 /* Pose modes of the preceding pass (INTEGRATION.md, "Pose modes"): per frame up to M = max_modes distinct refined poses of
@@ -483,11 +483,12 @@ int dsac_pose_modes_device(dsac_engine* e, int32_t n_frames, int32_t max_modes, 
  *   eval:   with d_gt_rig_jp [R][12] (jp of the rig frame) and DSAC_STAGE_EVAL, loss, rot_err, t_err, correct per rig.
  * status[r]: the OR of its frames' sampler bits, DSAC_ST_REFINE_ABORTED, and DSAC_ST_BAD_RIG when one of its extrinsics is
  * not finite (all of that rig's outputs but hyp_pose are then zero).  C = 1 with zero extrinsics gives dsac_forward_device's
- * results bit for bit.  Ordered on `stream`; the engine's pass becomes DSAC_PASS_RIG, which the backward passes,
- * dsac_refined_jp6_device, dsac_pose_uncertainty_device and dsac_pose_modes_device refuse; the sampling log-probability
- * stays valid.  DSAC_ERR_ARG, with the engine left as it was: n_frames % C != 0, C outside [1, DSAC_MAX_RIG_CAMERAS],
- * C * n_hyps > DSAC_MAX_HYPS, a score hook, cell depth or pose priors set, a stage mask without sample, score or refine, a
- * submitted pass that has not been awaited, or a NULL input or d_out. */
+ * results bit for bit.  Ordered on `stream`; the engine's pass becomes DSAC_PASS_RIG, which the ordinary backward passes,
+ * dsac_refined_jp6_device, dsac_pose_uncertainty_device and dsac_pose_modes_device refuse; the rig backward below and
+ * dsac_rig_refined_jp6_device read it, and the sampling log-probability stays valid.  DSAC_ERR_ARG, with the engine left
+ * as it was: n_frames % C != 0, C outside [1, DSAC_MAX_RIG_CAMERAS], C * n_hyps > DSAC_MAX_HYPS, a score hook, cell depth
+ * or pose priors set, a stage mask without sample, score or refine, a submitted pass that has not been awaited, or a NULL
+ * input or d_out. */
 #define DSAC_MAX_RIG_CAMERAS 8
 typedef struct dsac_rig_out {   /* DEVICE pointers, each nullable; R = n_frames / C, P = C * n_hyps */
     double*   hyp_pose;    /* [n][H][6]  the frames' sampled hypotheses */
@@ -508,6 +509,38 @@ typedef struct dsac_rig_out {   /* DEVICE pointers, each nullable; R = n_frames 
 int dsac_forward_rig_device(dsac_engine* e, int32_t n_frames, int32_t n_cameras, int64_t frame0, const int16_t* d_coords,
                             const int32_t* d_pix, int32_t pix_shared, const double* d_cam_from_rig, const double* d_gt_rig_jp,
                             const dsac_rig_out* d_out, void* stream);
+
+/* Rig gradients (INTEGRATION.md, "Rig gradients"): the backward of the preceding dsac_forward_rig_device over the same
+ * n_frames, whose inputs (coords, pix, extrinsics, gt) must still be valid.  The soft-argmax backward's chain in implicit
+ * mode (dsac_set_coord_derivatives does not apply: a rig is always differentiated by the implicit function theorem), with
+ * every per-hypothesis quantity lifted to the rig's pool of P = C * n_hyps: dRefineHyp by 12 replays of the rig
+ * refinement, the direct term by the IFT of its last accepted step over every camera's cells, the support term of each
+ * pool slot through the lift's Jacobian and the frame's dPNP, and the score term of every camera frame against its rig's
+ * pool (its support part crossing to the camera whose hypothesis the slot lifts).  Quirks Q3, Q4 (fix_q4), Q7, Q10 and
+ * Q12 as in dsac_backward_device.  A rig with DSAC_ST_BAD_RIG gets zero rows for all its frames.
+ * All pointers are DEVICE pointers, ordered on `stream` after the pass by an event; nothing is synchronised.
+ *   dsac_backward_rig_device: dLossMax of the refined rig pose against the pass's d_gt_rig_jp, times d_loss_grad [R]
+ *     (NULL = 1 per rig); the pass must have had d_gt_rig_jp and DSAC_STAGE_EVAL.
+ *   dsac_backward_rig_pose_device: seeded by d_grad_ref [R][6] = dOuter / d(refined rig jp6) (dsac_rig_refined_jp6_device).
+ *   d_dloss_dobj [n][N][3] and d_dloss_dpred [n][N][3], clamp: as dsac_backward_device, per camera frame; NULL = not written.
+ *   d_diag (nullable, each field nullable) as dsac_backward_out, per rig.
+ * The calls have their own scratch: they change no output of the pass and no result of a later call.  DSAC_ERR_ARG, with the
+ * engine left as it was: not after a dsac_forward_rig_device over the same n_frames, cameras, cell depth or pose priors
+ * changed since the pass, a submitted pass that has not been awaited, the loss form after a pass without ground truth or
+ * without DSAC_STAGE_EVAL, or a NULL d_grad_ref. */
+typedef struct dsac_rig_backward_out {   /* DEVICE pointers, each nullable; R = n_frames / C, P = C * n_hyps */
+    double* dloss_dref;       /* [R][6]   dLossMax of the refined rig pose, or the seed */
+    double* dref_dhyp;        /* [R][36]  d refined jp6 / d soft-argmax rig pose (cv) */
+    double* score_grads;      /* [R][P]   score output gradients over the pool */
+    double* dref_dobj;        /* [R][6][C*N*3] d refined jp6 / d scene coordinates, camera c's columns at c*N*3 */
+} dsac_rig_backward_out;
+int dsac_backward_rig_device(dsac_engine* e, int32_t n_frames, const double* d_loss_grad, double* d_dloss_dobj,
+                             float* d_dloss_dpred, float clamp, const dsac_rig_backward_out* d_diag, void* stream);
+int dsac_backward_rig_pose_device(dsac_engine* e, int32_t n_frames, const double* d_grad_ref, double* d_dloss_dobj,
+                                  float* d_dloss_dpred, float clamp, const dsac_rig_backward_out* d_diag, void* stream);
+/* jp 6-vectors [R][6] of the refined rig poses of the preceding dsac_forward_rig_device over n_frames (refusals as the rig
+ * backward's, and a NULL d_jp6). */
+int dsac_rig_refined_jp6_device(dsac_engine* e, int32_t n_frames, double* d_jp6, void* stream);
 
 /* Soft-argmax backward seeded by d_grad_ref [n][6] = dOuter/d(refined jp6) instead of dLossMax.
  * No ground truth needed. dloss_dobj / dloss_dpred / clamp as in dsac_backward_device; clamp applies to the total. */
