@@ -364,6 +364,46 @@ def pose_modes(engine, n, max_modes, rot_rad, trans_mm):
     return out
 
 
+def _set_rig_priors(engine, prediction, n_cameras, priors):
+    if priors is None:
+        return
+    poses, info, gate = priors
+    C = int(n_cameras)
+    R = prediction.shape[0] // C
+    if poses.dtype != torch.float64 or poses.dim() != 3 or poses.shape[0] != R or poses.shape[2] != 6 \
+            or poses.device != prediction.device:
+        raise ValueError("rig_priors poses must be float64 [%d][k][6] on %s, got %s %s on %s"
+                         % (R, prediction.device, poses.dtype, tuple(poses.shape), poses.device))
+    k = poses.shape[1]
+    if info is not None and (info.dtype != torch.float64 or tuple(info.shape) != (R, k, 6, 6) or info.device != prediction.device):
+        raise ValueError("rig_priors info must be float64 [%d][%d][6][6] on %s, got %s %s on %s"
+                         % (R, k, prediction.device, info.dtype, tuple(info.shape), info.device))
+    pc = poses.detach().contiguous()
+    ic = info.detach().contiguous() if info is not None else None
+    stream = torch.cuda.current_stream(prediction.device)
+    engine.set_rig_pose_priors_device(prediction.shape[0], C, k, pc.data_ptr(), ic.data_ptr() if ic is not None else None,
+                                      float(gate), stream.cuda_stream)
+    pc.record_stream(stream)
+    if ic is not None:
+        ic.record_stream(stream)
+
+
+def rig_pose_uncertainty(engine, n, n_cameras):
+    """Covariance of each refined rig pose of the engine's last rig pass over n frames of n_cameras cameras (INTEGRATION.md,
+    "Rig tracking"), a dict of device tensors on torch.cuda.current_stream(), one entry per rig (R = n / n_cameras):
+    cov_jp6 and cov_xi float64 [R][6][6], sigma2 float64 [R], n_fit, support and ok int32 [R], as pose_uncertainty's in the
+    rig chart.  inv(cov_xi + Q) is an information matrix for rig_priors=.  These outputs carry no autograd history."""
+    dev = torch.device("cuda", engine.cfg.device)
+    R = n // int(n_cameras)
+    out = {k: torch.empty((R, 6, 6), dtype=torch.float64, device=dev) for k in ("cov_jp6", "cov_xi")}
+    out["sigma2"] = torch.empty((R,), dtype=torch.float64, device=dev)
+    for k in ("n_fit", "support", "ok"):
+        out[k] = torch.empty((R,), dtype=torch.int32, device=dev)
+    engine.rig_pose_uncertainty_device(n, int(n_cameras), torch.cuda.current_stream(dev).cuda_stream,
+                                       **{k: v.data_ptr() for k, v in out.items()})
+    return out
+
+
 def _check_rig(engine, prediction, pix, cam_from_rig, n_cameras, gt_jp):
     C = int(n_cameras)
     n, pix, _, shared = _check_inputs(engine, prediction, pix, None, need_gt=False)
@@ -413,40 +453,49 @@ class _RigSoftam(torch.autograd.Function):
 
 
 def rig_softam_loss(engine, prediction, pix, cam_from_rig, n_cameras, gt_jp, frame0=0, clamp=0.1, cameras=None,
-                    sampling_logits=None):
+                    sampling_logits=None, rig_priors=None):
     """Per-rig loss of the rig pass (rig_pose's rig layout; INTEGRATION.md, "Rig gradients"): dLossMax's loss of each refined
     rig pose against gt_jp float64 [R][12], float64 [R]; differentiable with respect to `prediction` through every camera's
     scene coordinates, by the implicit-function derivatives whatever the engine's set_coord_derivatives.  clamp, cameras
-    and sampling_logits as in softam_loss; with sampling_logits, sampling_log_prob gives the REINFORCE term of the rigs."""
+    and sampling_logits as in softam_loss; with sampling_logits, sampling_log_prob gives the REINFORCE term of the rigs.
+    rig_priors as in rig_pose; the priors are constants of the gradient."""
     if gt_jp is None:
         raise ValueError("the loss needs the rig ground-truth poses gt_jp [R][12]")
     _check_rig(engine, prediction, pix, cam_from_rig, n_cameras, gt_jp)
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
+    _set_rig_priors(engine, prediction, n_cameras, rig_priors)
     return _RigSoftam.apply(prediction, engine, pix, cam_from_rig, int(n_cameras), gt_jp, int(frame0), float(clamp))
 
 
-def rig_softam_pose(engine, prediction, pix, cam_from_rig, n_cameras, frame0=0, clamp=0.1, cameras=None, sampling_logits=None):
+def rig_softam_pose(engine, prediction, pix, cam_from_rig, n_cameras, frame0=0, clamp=0.1, cameras=None, sampling_logits=None,
+                    rig_priors=None):
     """Refined pose of every rig as a jp 6-vector [rodrigues(R); t in mm] of the rig frame, float64 [R][6]; differentiable
     with respect to `prediction` as rig_softam_loss.  Needs no ground truth."""
     _check_rig(engine, prediction, pix, cam_from_rig, n_cameras, None)
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
+    _set_rig_priors(engine, prediction, n_cameras, rig_priors)
     return _RigSoftam.apply(prediction, engine, pix, cam_from_rig, int(n_cameras), None, int(frame0), float(clamp))
 
 
-def rig_pose(engine, prediction, pix, cam_from_rig, n_cameras, frame0=0, cameras=None, sampling_logits=None, gt_jp=None):
+def rig_pose(engine, prediction, pix, cam_from_rig, n_cameras, frame0=0, cameras=None, sampling_logits=None, gt_jp=None,
+             rig_priors=None):
     """One pose per multi-camera rig (INTEGRATION.md, "Multi-camera rigs"): the n frames of `prediction` are R = n / C rigs
     of C = n_cameras cameras, frame r C + c camera c of rig r, whose extrinsic cam_from_rig[r C + c] (float64 [n][6], a cv
     pose: X_cam = R_c X_rig + t_c) is known.  cameras and sampling_logits as in softam_pose, per frame; gt_jp float64
     [R][12] (the jp pose of the rig frame) adds loss, rot_err, t_err and correct.  A dict of device tensors on
     torch.cuda.current_stream(), without autograd history: hyp_pose [n][H][6]; rig_hyp [R][C H][6], scores and sf
     [R][C H]; entropy [R]; avg_pose and ref_pose [R][6] (cv poses of the rig); inlier_map int32 [n][1600]; steps_done int32,
-    status int32 [R]; and with gt_jp loss, rot_err, t_err float64 and correct int32 [R]."""
+    status int32 [R]; and with gt_jp loss, rot_err, t_err float64 and correct int32 [R].
+    rig_priors = (poses float64 [R][k][6] cv rig poses, info float64 [R][k][6][6] or None, gate) puts k rig poses per rig
+    into every camera's hypotheses (INTEGRATION.md, "Rig tracking"); sticky like pose_priors=: None leaves the engine's
+    setting as it is, and Engine.set_rig_pose_priors_device(n, n_cameras, 0, None) clears it."""
     C, n, R, pix, shared = _check_rig(engine, prediction, pix, cam_from_rig, n_cameras, gt_jp)
     dev, H = prediction.device, engine.cfg.n_hyps
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
+    _set_rig_priors(engine, prediction, C, rig_priors)
     stream = torch.cuda.current_stream(dev).cuda_stream
     coords = _coords(engine, prediction.detach().contiguous(), stream)
     ext = cam_from_rig.detach().contiguous()
@@ -462,6 +511,7 @@ def rig_pose(engine, prediction, pix, cam_from_rig, n_cameras, frame0=0, cameras
                    correct=torch.empty((R,), **i32))
     engine.forward_rig_device(n, C, coords.data_ptr(), pix.data_ptr(), ext.data_ptr(), shared, gt.data_ptr() if gt is not None else None,
                               int(frame0), stream, **{k: v.data_ptr() for k, v in out.items()})
+    engine._rig_inputs = (coords, pix, ext, gt)   # rig_pose_uncertainty reads the pass's inputs: alive until the next rig_pose
     return out
 
 

@@ -38,7 +38,8 @@ using namespace dsac;
 static_assert(sizeof(Cam) == sizeof(dsac_camera), "Cam mirrors dsac_camera");
 static_assert(PRIOR_MAX == DSAC_MAX_PRIORS && PRIOR_ST_BAD == DSAC_ST_BAD_PRIOR, "prior.cuh mirrors dsac_b200.h");
 static_assert(MODE_MAX == DSAC_MAX_MODES && DSAC_MAX_HYPS <= 1024, "modes.cuh mirrors dsac_b200.h");
-static_assert(RIG_MAX_CAMERAS == DSAC_MAX_RIG_CAMERAS && RIG_ST_BAD == DSAC_ST_BAD_RIG && DSAC_MAX_HYPS <= 2048,
+static_assert(RIG_MAX_CAMERAS == DSAC_MAX_RIG_CAMERAS && RIG_ST_BAD == DSAC_ST_BAD_RIG && DSAC_MAX_HYPS <= 2048 &&
+                  RIG_ST_SPOILED == (DSAC_ST_BAD_RIG | DSAC_ST_BAD_PRIOR),
               "refine.cuh mirrors dsac_b200.h (a rig's selection codes a cell in 11 bits)");
 static_assert(sizeof(ObjCam) == sizeof(dsac_rgbd_camera) && offsetof(ObjCam, sensor_trans) == offsetof(dsac_rgbd_camera, sensor_trans) &&
                   offsetof(ObjCam, raw_data) == offsetof(dsac_rgbd_camera, raw_data),
@@ -129,8 +130,9 @@ class Handle {
 using Stream = Handle<cudaStream_t, cudaStreamDestroy>;
 using Event = Handle<cudaEvent_t, cudaEventDestroy>;
 
-// The per-frame settings of the following passes, indices into dsac_engine::set.
-enum { SET_CAMS, SET_LOGITS, SET_DEPTH, SET_PRIORS, SET_COUNT };
+// The per-frame settings of the following passes, indices into dsac_engine::set.  SET_RIG_PRIORS is read by the rig pass
+// only; every other forward pass refuses to start while it is set.
+enum { SET_CAMS, SET_LOGITS, SET_DEPTH, SET_PRIORS, SET_RIG_PRIORS, SET_COUNT };
 
 // One per-frame setting: the frames it covers (0: off), a generation that changes with every update, and the event
 // recorded after an update's copy or kernel, which a pass waits for before it reads the setting's buffers.
@@ -155,6 +157,13 @@ struct Pass {
     unsigned long long gen[SET_COUNT] = {};
     int set_n[SET_COUNT] = {};
     int prior_k = 0;                // priors per frame
+    // the prior tables the sampler and k_prior_inject read: the pose priors' (dsac_set_pose_priors_device), or a rig pass's
+    // composition of the rig pose priors with its extrinsics (k_rig_prior_prep)
+    const double* prior_pose = nullptr;     // [n][prior_k][6]
+    const PriorGate* prior_tab = nullptr;   // [n][prior_k] (a gate only)
+    const uint32_t* prior_bad = nullptr;    // [n]
+    bool prior_gate = false;
+    double prior_chi2 = 0;
     int rig_c = 0;                  // a rig pass's cameras per rig (its gt: the rig ground truth, null without DSAC_STAGE_EVAL)
     bool rgbd() const { return set_n[SET_DEPTH] > 0; }
 };
@@ -202,6 +211,13 @@ struct dsac_engine {
     int prior_k = 0;
     bool prior_gate = false;
     double prior_chi2 = 0;
+    // rig pose priors (dsac_set_rig_pose_priors_device): k rig poses per rig of rig_prior_c cameras, sized once for max_frames
+    // x DSAC_MAX_PRIORS on first use; each rig pass composes them with its extrinsics into its own scratch (e->rig)
+    DevMem<double> d_rig_prior_pose;  // [R][k][6] cv rig poses
+    DevMem<double> d_rig_prior_info;  // [R][k][36] information matrices in the rig chart (a gate only)
+    int rig_prior_k = 0, rig_prior_c = 0;
+    bool rig_prior_gate = false;
+    double rig_prior_chi2 = 0;
     // per-dataset cameras of the pre-training data paths (dsac_set_dataset_cameras), indexed by dataset frame; grow-only.
     // ds_cams_n == 0: no table.  ds_cam0 is entry 0 on the host: the frame size and raw_data every entry shares.
     DevMem<ObjCam> d_ds_cams;
@@ -254,6 +270,7 @@ struct dsac_engine {
     // dsac_pose_uncertainty_device: its own recording replay (pose, cells, count per job), shared with no backward so
     // that a call changes no later result; ev_unc is recorded after a call's last launch and the next call waits on it
     IftScratch unc;
+    uint32_t* unc_status = nullptr;   // [R] dsac_rig_pose_uncertainty_device: the rig status its replay ORs the abort bit into
     DevMem<char> unc_buf;
     Event ev_unc;
     // dsac_pose_modes_device: its seeds, recording replay and covariances in one grow-only block of its own, ordered by
@@ -267,6 +284,9 @@ struct dsac_engine {
         float* P;
         int32_t *imap, *steps, *correct;
         uint32_t* status;
+        double* prior_pose;         // [n][k][6] the rig pose priors composed per frame (k_rig_prior_prep), k of the setting
+        PriorGate* prior_tab;       // [n][k]
+        uint32_t* prior_bad;        // [n]
     } rig = {};
     DevMem<char> rig_buf;
     // dsac_backward_rig(_pose)_device: the soft-argmax backward's arrays over rigs and pools, the recording replay, the
@@ -745,23 +765,32 @@ static const struct {
     {"dsac_set_sampling_logits_device", "frames of the sampling logits (dsac_set_sampling_logits_device)", "sampling logits were"},
     {"dsac_set_cell_depth_device", "frames of the cell depth (dsac_set_cell_depth_device)", "cell depth was"},
     {"dsac_set_pose_priors_device", "frames of the pose priors (dsac_set_pose_priors_device)", "pose priors were"},
+    {"dsac_set_rig_pose_priors_device", "frames of the rig pose priors (dsac_set_rig_pose_priors_device)", "rig pose priors were"},
 };
 
 // The start every forward entry point shares: the batch matches each setting in force, each of `streams` waits for the
 // settings' updates, and the record of the pass takes its inputs and the settings' snapshot.  A pipeline's entry point
-// sets the record's kind once the engine holds a pass of it.
+// sets the record's kind once the engine holds a pass of it.  rig: the rig pass, the only one that reads the rig pose
+// priors; any other refuses while they are set rather than ignore them.
 static int pass_begin(dsac_engine* e, int32_t kind, int32_t n, int64_t frame0, const int16_t* coords, const int32_t* pix,
-                      int32_t pix_shared, const double* gt, std::initializer_list<cudaStream_t> streams) {
+                      int32_t pix_shared, const double* gt, std::initializer_list<cudaStream_t> streams, bool rig = false) {
     Pass p;
     for (int i = 0; i < SET_COUNT; i++) {
         const Setting& s = e->set[i];
+        if (i == SET_RIG_PRIORS && s.n && !rig)
+            return fail(e, DSAC_ERR_ARG, "rig pose priors are set (%s), which only dsac_forward_rig_device reads: clear them first",
+                        k_setting[i].setter);
         if (s.n && n != s.n) return fail(e, DSAC_ERR_ARG, "n_frames %d differs from the %d %s", n, s.n, k_setting[i].frames);
         if (s.n)
             for (cudaStream_t st : streams) CU(cudaStreamWaitEvent(st, s.ev, 0));
         p.gen[i] = s.gen;
         p.set_n[i] = s.n;
     }
-    p.prior_k = e->set[SET_PRIORS].n ? e->prior_k : 0;
+    if (e->set[SET_PRIORS].n) {
+        p.prior_k = e->prior_k;
+        p.prior_pose = e->d_prior_pose; p.prior_tab = e->d_prior_tab; p.prior_bad = e->d_prior_bad;
+        p.prior_gate = e->prior_gate; p.prior_chi2 = e->prior_chi2;
+    }
     p.kind = kind;
     p.n = n;
     p.coords = coords; p.pix = pix; p.pix_shared = pix_shared; p.gt = gt;
@@ -878,7 +907,8 @@ static int sampling_log_prob_run(dsac_engine* e, const char* who, int32_t n, dou
                                  void* stream_v) {
     if (!e) return DSAC_ERR_ARG;
     if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "%s: a submitted pass has not been awaited (dsac_forward_wait)", who);
-    if (int rc = pass_check(e, who, n, PASS_GUIDED, SETTINGS_SAMPLING)) return rc;
+    const unsigned rig_priors = e->pass.kind == DSAC_PASS_RIG ? 1u << SET_RIG_PRIORS : 0u;   // (a rig pass's consumers only)
+    if (int rc = pass_check(e, who, n, PASS_GUIDED, SETTINGS_SAMPLING | rig_priors)) return rc;
     if ((!d_logp && !d_grad_logp) || (d_grad_logp && !d_grad)) return fail(e, DSAC_ERR_ARG, "%s: null output", who);
     cudaStream_t stream = (cudaStream_t)stream_v;
     CU(cudaSetDevice(e->cfg.device));
@@ -1062,8 +1092,9 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
     const GuidedGen gg{guided ? e->d_g_cum + o * DSAC_N : nullptr, guided ? e->d_g_bad + o : nullptr};
     const double* eye = rgbd ? e->d_eye + o * Nn * 3 : nullptr;   // RGB-D pass: this range's frames of the eye coordinates
     // pose priors: the streams draw n_hyps - prior_k hypotheses into the first slots of each frame, k_prior_inject fills the rest
-    const int prior_k = e->pass.prior_k;
-    const int gate = prior_k > 0 && e->prior_gate;
+    const Pass& ps = e->pass;
+    const int prior_k = ps.prior_k;
+    const int gate = prior_k > 0 && ps.prior_gate;
     const int draw_h = c.n_hyps - prior_k;
 
     if (stages & DSAC_STAGE_SAMPLE) {
@@ -1087,8 +1118,8 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
         { const char* g = getenv("DSAC_K1_A2_GENERIC"); sp.a2_generic = (g && g[0] == '1') ? 1 : 0; }
         sp.resume = nullptr;
         sp.eye = eye; sp.skip_frame = rgbd ? e->d_rgbd_skip + o : nullptr;
-        sp.prior_tab = gate ? e->d_prior_tab + o * prior_k : nullptr; sp.prior_bad = gate ? e->d_prior_bad + o : nullptr;
-        sp.prior_k = gate ? prior_k : 0; sp.prior_chi2 = gate ? e->prior_chi2 : 0.0;
+        sp.prior_tab = gate ? ps.prior_tab + o * prior_k : nullptr; sp.prior_bad = gate ? ps.prior_bad + o : nullptr;
+        sp.prior_k = gate ? prior_k : 0; sp.prior_chi2 = gate ? ps.prior_chi2 : 0.0;
         // the monolithic sampler: the whole pass, or the resume tail of the split sampler's rounds
         auto launch_sample = [&](const SampleParams& s) {
             k_sample_tab[cam][rgbd][gate]<<<dim3(c.n_streams, n), K1_THREADS, sizeof(K1Smem), stream>>>(s);
@@ -1314,7 +1345,7 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
         }
         if (prior_k) {   // the prior slots behind the sampled ones, or the empty frames of a bad setting
             PriorInjectParams ip;
-            ip.poses = e->d_prior_pose + o * prior_k * 6; ip.bad = e->d_prior_bad + o;
+            ip.poses = ps.prior_pose + o * prior_k * 6; ip.bad = ps.prior_bad + o;
             ip.k = prior_k; ip.H = c.n_hyps; ip.T = c.n_streams; ip.skip = c.stream_skip; ip.f = c.focal; ip.cams = cams;
             ip.hyp_pose = sp.hyp_pose; ip.hyp_P = sp.hyp_P; ip.img_idx = sp.img_idx; ip.cand_idx = sp.cand_idx;
             ip.stream_ncand = sp.stream_ncand; ip.stream_endpos = sp.stream_endpos; ip.status = sp.status;
@@ -2141,3 +2172,4 @@ static int carve_scratch(dsac_engine* e, DevMem<char>& buf, std::initializer_lis
 #include "modes_host.inc"
 #include "rig_host.inc"
 #include "rig_backward_host.inc"
+#include "rig_tracking_host.inc"

@@ -125,6 +125,43 @@ DSAC_HD bool prior_entry(const double pose[6], const double* info, PriorGate& g)
     return ok;
 }
 
+// A rig prior (R_j, t_j) seen from camera frame f of its rig, whose extrinsic is the cv pose ext (X_cam = R_c X_rig + t_c):
+// the pose T_c o T_j = (R_c R_j, R_c t_j + t_c) and, for a non-null info, Lambda_f = B Lambda_j B^T with B = blockdiag(R_c,
+// R_c).  A camera hypothesis lifted to the rig, (R_r, t_r), has xi_cam = B xi_rig against these, so the camera-frame gate is
+// the rig-frame gate of the lifted hypothesis.  An extrinsic whose rvec is exactly zero (R_c = I exactly) keeps the prior's
+// rvec and information bits, as k_rig_lift keeps a hypothesis' rvec.  False when an entry of ext is not finite.
+DSAC_HD bool rig_prior_compose(const double ext[6], const double pose[6], const double* info, double out_pose[6], double* out_info) {
+    bool ok = true;
+    for (int m = 0; m < 6; m++) ok = ok && isfinite(ext[m]);
+    double Rc[9], Rj[9], R[9];
+    rodrigues_v2m(ext, Rc);
+    rodrigues_v2m(pose, Rj);
+    rig_compose(Rc, ext + 3, Rj, pose + 3, R, out_pose + 3);
+    const bool ident = ext[0] == 0.0 && ext[1] == 0.0 && ext[2] == 0.0;
+    if (ident) {
+        for (int m = 0; m < 3; m++) out_pose[m] = pose[m];
+    } else {
+        rodrigues_m2v(R, out_pose);
+    }
+    if (!info) return ok;
+    if (ident) {
+        for (int m = 0; m < 36; m++) out_info[m] = info[m];
+        return ok;
+    }
+    double T[36];   // B Lambda_j, then (B Lambda_j) B^T: B's two blocks are R_c
+    for (int i = 0; i < 6; i++)
+        for (int j = 0; j < 6; j++) {
+            const int bi = i / 3 * 3, ri = i % 3;
+            T[i * 6 + j] = Rc[ri * 3] * info[bi * 6 + j] + Rc[ri * 3 + 1] * info[(bi + 1) * 6 + j] + Rc[ri * 3 + 2] * info[(bi + 2) * 6 + j];
+        }
+    for (int i = 0; i < 6; i++)
+        for (int j = 0; j < 6; j++) {
+            const int bj = j / 3 * 3, rj = j % 3;
+            out_info[i * 6 + j] = T[i * 6 + bj] * Rc[rj * 3] + T[i * 6 + bj + 1] * Rc[rj * 3 + 1] + T[i * 6 + bj + 2] * Rc[rj * 3 + 2];
+        }
+    return ok;
+}
+
 #if defined(__CUDACC__) && !defined(DSAC_HOST_ONLY)
 }  // namespace dsac
 #include "camera.cuh"
@@ -190,6 +227,39 @@ __global__ void __launch_bounds__(128) k_prior_inject(PriorInjectParams p) {
         p.stream_endpos[(size_t)f * p.T + s] = (s == 0) ? p.skip : 0u;
     }
     if (tid == 0 && bad) p.status[f] = (p.status[f] & ~1u) | PRIOR_ST_BAD;
+}
+
+// dsac_set_rig_pose_priors_device, at each rig pass: the per-frame tables k_prior_inject and the gate read, composed with the
+// pass's extrinsics.  Frame f = r C + c of a rig of C cameras gets prior j of rig r as T_c o T_j (rig_prior_compose).
+struct RigPriorParams {
+    int C, k;                   // cameras per rig, priors per rig
+    const double* cam_from_rig; // [n][6] the pass's extrinsics
+    const double* poses;        // [R][k][6] rig priors (cv)
+    const double* info;         // [R][k][36] or null
+    double* out_pose;           // [n][k][6]
+    PriorGate* tab;             // [n][k]
+    uint32_t* bad;              // [n] DSAC_ST_BAD_PRIOR or 0
+};
+constexpr int RIG_PRIOR_THREADS = 128;   // >= RIG_MAX_CAMERAS x PRIOR_MAX
+static_assert(RIG_PRIOR_THREADS >= 8 * PRIOR_MAX, "one thread per (camera, prior) of a rig");
+
+// One CTA per rig, thread c k + j for camera c's prior j.  A rig whose composed entries prior_entry refuses, or one of whose
+// extrinsics is not finite, is bad in all its frames.
+__global__ void __launch_bounds__(RIG_PRIOR_THREADS) k_rig_prior_prep(RigPriorParams p) {
+    const int r = blockIdx.x, t = threadIdx.x, C = p.C, k = p.k;
+    bool ok = true;
+    if (t < C * k) {
+        const int c = t / k, j = t - c * k;
+        const size_t f = (size_t)r * C + c, src = (size_t)r * k + j, dst = f * k + j;
+        double pose[6], info[36];
+        ok = rig_prior_compose(p.cam_from_rig + f * 6, p.poses + src * 6, p.info ? p.info + src * 36 : nullptr, pose, info);
+        PriorGate g;
+        ok = prior_entry(pose, p.info ? info : nullptr, g) && ok;
+        p.tab[dst] = g;
+        for (int m = 0; m < 6; m++) p.out_pose[dst * 6 + m] = pose[m];
+    }
+    const int any_bad = __syncthreads_or(!ok);
+    if (t < C) p.bad[(size_t)r * C + t] = any_bad ? PRIOR_ST_BAD : 0u;
 }
 
 #endif

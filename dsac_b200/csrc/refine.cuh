@@ -34,6 +34,8 @@ constexpr int K4_WARPS = K4_THREADS / 32;
 constexpr int K4_MAX_INLIERS = 128;
 constexpr int RIG_MAX_CAMERAS = 8;            // DSAC_MAX_RIG_CAMERAS
 constexpr uint32_t RIG_ST_BAD = 256u;          // DSAC_ST_BAD_RIG
+// a rig whose outputs are zero: a non-finite extrinsic, or a bad rig prior (DSAC_ST_BAD_RIG | DSAC_ST_BAD_PRIOR)
+constexpr uint32_t RIG_ST_SPOILED = RIG_ST_BAD | 128u;
 static_assert(K4_THREADS % 32 == 0 && K4_THREADS >= 32 && K4_THREADS <= 256, "k_refine block size");
 
 struct RefineParams {
@@ -142,7 +144,7 @@ __device__ double max_loss_dev(const double R1[9], const double t1[3], const dou
 // composed pose (rig_compose), the selection is each camera's first inlier_count flagged cells in turn (entries cam << 11 |
 // cell), an LM point is reprojected in its own camera (lm_point_contrib_ext), and the inlier maps are the cameras' frames.
 // The cells are read from global memory rather than staged: C frames do not fit in shared memory.  A rig with
-// DSAC_ST_BAD_RIG in status gets zero outputs.  RIG with RECORD (k_refine_rig_rec, the rig backward) records those entries
+// DSAC_ST_BAD_RIG or DSAC_ST_BAD_PRIOR in status gets zero outputs.  RIG with RECORD (k_refine_rig_rec, the rig backward) records those entries
 // at a stride of C K4_MAX_INLIERS per rig.
 template <bool PER_FRAME, bool RGBD = false, bool RECORD = false, bool RIG = false>
 __device__ __forceinline__ void k_refine_body(const RefineParams& p, const double* eye = nullptr, uint16_t* rec_sel = nullptr,
@@ -170,7 +172,7 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p, const doubl
     if (frame < 0) return;  // unused job slot
     const int n_cams = RIG ? rig.C : 1;
     if constexpr (RIG) {
-        if (p.status[frame] & RIG_ST_BAD) {   // (uniform over the CTA)
+        if (p.status[frame] & RIG_ST_SPOILED) {   // (uniform over the CTA)
             if (tid < 6) p.out_pose[(size_t)job * 6 + tid] = 0.0;
             if (p.inlier_map)
                 for (int i = tid; i < n_cams * DSAC_N_CONST; i += K4_THREADS) p.inlier_map[(size_t)job * n_cams * DSAC_N_CONST + i] = 0;

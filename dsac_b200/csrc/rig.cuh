@@ -40,18 +40,28 @@ struct RigLiftParams {
     double* rig_hyp;                // [R][P][6] the pool's rig poses
     float* rig_P;                   // [n][P][12] rows of pool pose j in camera frame f
     uint32_t* status;               // [R]
+    const double* prior_pose;       // [R][prior_k][6] the rig pose priors (dsac_set_rig_pose_priors_device), or null
+    int prior_k;                    // 0: none
 };
 
 // Grid (ceil(P / 256), R): thread j of rig r lifts pool slot j and writes its rows in each camera of the rig.  A rig with a
-// non-finite extrinsic gets DSAC_ST_BAD_RIG and zero pool poses (its rows stay finite; k_rig_tail zeroes its scores).  An
-// extrinsic whose rvec is exactly zero has Rc = I exactly (rodrigues_v2m), so the lift is exact and the hypothesis keeps
-// its rvec bits rather than a round trip through the matrix.
+// non-finite extrinsic gets DSAC_ST_BAD_RIG and zero pool poses (its rows stay finite; k_rig_tail zeroes its scores), and so
+// does a rig whose frames carry DSAC_ST_BAD_PRIOR (a bad rig prior, k_rig_prior_prep).  An extrinsic whose rvec is exactly
+// zero has Rc = I exactly (rodrigues_v2m), so the lift is exact and the hypothesis keeps its rvec bits rather than a round
+// trip through the matrix.  With rig priors, camera c's prior slot H - k + j is pool slot c H + H - k + j and takes rig
+// prior j's own bits, so the pool holds C copies of each prior.
 __global__ void __launch_bounds__(RIG_LIFT_THREADS) k_rig_lift(RigLiftParams p) {
     __shared__ double s_ext[RIG_MAX_CAMERAS][12];
     __shared__ int s_ident[RIG_MAX_CAMERAS];
     __shared__ int s_bad;
+    __shared__ uint32_t s_st;
     const int tid = threadIdx.x, r = blockIdx.y, C = p.C, P = C * p.H;
-    if (tid == 0) s_bad = 0;
+    if (tid == 0) {
+        s_bad = 0;
+        uint32_t st = 0;
+        for (int c = 0; c < C; c++) st |= p.frame_status[r * C + c];
+        s_st = st;
+    }
     __syncthreads();
     if (tid < C) {
         const double* e = p.cam_from_rig + (size_t)(r * C + tid) * 6;
@@ -71,29 +81,32 @@ __global__ void __launch_bounds__(RIG_LIFT_THREADS) k_rig_lift(RigLiftParams p) 
         s_ident[tid] = v[0] == 0.0 && v[1] == 0.0 && v[2] == 0.0;
     }
     __syncthreads();
-    const bool bad = s_bad != 0;
+    const bool bad = s_bad != 0 || (s_st & RIG_ST_SPOILED) != 0;
     if (blockIdx.x == 0) {
         if (tid < C)
             for (int k = 0; k < 12; k++) p.ext[(size_t)(r * C + tid) * 12 + k] = s_ext[tid][k];
-        if (tid == 0) {
-            uint32_t st = bad ? RIG_ST_BAD : 0u;
-            for (int c = 0; c < C; c++) st |= p.frame_status[r * C + c];
-            p.status[r] = st;
-        }
+        if (tid == 0) p.status[r] = s_st | (s_bad ? RIG_ST_BAD : 0u);
     }
     const int j = blockIdx.x * RIG_LIFT_THREADS + tid;
     if (j >= P) return;
-    const int c = j / p.H, h = j - c * p.H;
-    double hp[6] = {0, 0, 0, 0, 0, 0};
-    if (!bad)
-        for (int k = 0; k < 6; k++) hp[k] = p.hyp_pose[((size_t)(r * C + c) * p.H + h) * 6 + k];
-    double Rh[9], Rr[9], tr[3], rr[3];
-    rodrigues_v2m(hp, Rh);
-    rig_lift(s_ext[c], s_ext[c] + 9, Rh, hp + 3, Rr, tr);
-    if (s_ident[c]) {
-        rr[0] = hp[0]; rr[1] = hp[1]; rr[2] = hp[2];
+    const int c = j / p.H, h = j - c * p.H, hk = h - (p.H - p.prior_k);
+    double Rr[9], tr[3], rr[3];
+    if (hk >= 0 && !bad) {   // a prior slot: the rig prior itself
+        const double* pp = p.prior_pose + ((size_t)r * p.prior_k + hk) * 6;
+        for (int k = 0; k < 3; k++) { rr[k] = pp[k]; tr[k] = pp[3 + k]; }
+        rodrigues_v2m(rr, Rr);
     } else {
-        rodrigues_m2v(Rr, rr);
+        double hp[6] = {0, 0, 0, 0, 0, 0};
+        if (!bad)
+            for (int k = 0; k < 6; k++) hp[k] = p.hyp_pose[((size_t)(r * C + c) * p.H + h) * 6 + k];
+        double Rh[9];
+        rodrigues_v2m(hp, Rh);
+        rig_lift(s_ext[c], s_ext[c] + 9, Rh, hp + 3, Rr, tr);
+        if (s_ident[c]) {
+            rr[0] = hp[0]; rr[1] = hp[1]; rr[2] = hp[2];
+        } else {
+            rodrigues_m2v(Rr, rr);
+        }
     }
     double* o = p.rig_hyp + ((size_t)r * P + j) * 6;
     if (bad)
@@ -121,7 +134,7 @@ struct RigTailParams {
 __global__ void __launch_bounds__(K2_THREADS) k_rig_tail(RigTailParams p) {
     __shared__ double s_red[8 * K2_WARPS];
     const int r = blockIdx.x, tid = threadIdx.x, P = p.sp.H, C = p.C;
-    const bool bad = (p.status[r] & RIG_ST_BAD) != 0;
+    const bool bad = (p.status[r] & RIG_ST_SPOILED) != 0;
     for (int j = tid; j < P; j += K2_THREADS) {
         const double* cs = p.cam_scores + (size_t)r * C * P + j;
         double s = cs[0];
@@ -192,7 +205,7 @@ __global__ void __launch_bounds__(RIG_BW_THREADS) k_rig_bw_support(RigBwParams p
     if (h >= p.H) return;
     const int C = p.C, r = f / C, c2 = f - r * C, j = c2 * p.H + h;
     double* u = p.u + ((size_t)f * p.H + h) * 12;
-    if (p.status[r] & RIG_ST_BAD) {
+    if (p.status[r] & RIG_ST_SPOILED) {
         for (int k = 0; k < 12; k++) u[k] = 0.0;
         return;
     }
@@ -227,7 +240,7 @@ __global__ void __launch_bounds__(RIG_BW_THREADS) k_rig_bw_support(RigBwParams p
 __global__ void __launch_bounds__(32) k_rig_bw_scatter(RigBwParams p) {
     const int f = blockIdx.x, lane = threadIdx.x, r = f / p.C, c2 = f - r * p.C;
     double* row = p.row + (size_t)f * DSAC_N_CONST * 3;
-    if (p.status[r] & RIG_ST_BAD) {
+    if (p.status[r] & RIG_ST_SPOILED) {
         for (int i = lane; i < DSAC_N_CONST * 3; i += 32) row[i] = 0.0;
         return;
     }

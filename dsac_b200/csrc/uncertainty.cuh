@@ -38,17 +38,39 @@ constexpr int UNC_THREADS = 64, UNC_WARPS = UNC_THREADS / 32;
 // (score_pair_error on the pose's fp32 projection rows, built as k1_write_hyp builds them) below thr2d, every cell with
 // or without depth.  The 23 sums are reduced with the transposed butterfly, then the warps in order; one lane does the 6x6
 // work in fp64.
-template <bool PER_FRAME, bool RGBD>
-__device__ __forceinline__ void k_pose_uncertainty_body(const UncParams& p) {
+// RIG (k_pose_uncertainty_rig, dsac_rig_pose_uncertainty_device): job r is rig r of rig.C cameras, pose the rig's, sel
+// entries cam << 11 | cell at a stride of C K4_MAX_INLIERS (k_refine_rig_rec).  A cell is set up in its own camera frame at
+// the composed pose and mapped to the rig frame (ift_point_to_rig), as k_refine_ift_rig does; the support counts the cells
+// of every camera under its composed pose.  A rig with DSAC_ST_BAD_RIG or DSAC_ST_BAD_PRIOR in rig_status gets zeros.
+template <bool PER_FRAME, bool RGBD, bool RIG = false>
+__device__ __forceinline__ void k_pose_uncertainty_body(const UncParams& p, RigRefine rig = RigRefine{},
+                                                        const uint32_t* rig_status = nullptr) {
+    static_assert(!(RIG && RGBD), "a rig refines RGB frames");
     __shared__ double s_red[UNC_WARPS][32];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int job = blockIdx.x;
     const int frame = job / p.jobs_per_frame;
     const Cam cam = frame_cam<PER_FRAME>(p, frame);
     const int cnt = p.count[job];
-    const uint16_t* sel = p.sel + (size_t)job * K4_MAX_INLIERS;
+    const int n_cams = RIG ? rig.C : 1;
+    const uint16_t* sel = p.sel + (size_t)job * n_cams * K4_MAX_INLIERS;
     const int16_t* coords = p.coords + (size_t)frame * DSAC_N_CONST * 3;
     const int32_t* pix = p.pix + (size_t)frame * p.pix_stride;
+    if constexpr (RIG) {
+        if (rig_status[job] & RIG_ST_SPOILED) {   // (uniform over the CTA)
+            if (tid < 36) {
+                if (p.cov_xi) p.cov_xi[(size_t)job * 36 + tid] = 0.0;
+                if (p.cov_jp6) p.cov_jp6[(size_t)job * 36 + tid] = 0.0;
+            }
+            if (tid == 0) {
+                if (p.sigma2) p.sigma2[job] = 0.0;
+                if (p.n_fit) p.n_fit[job] = 0;
+                if (p.support) p.support[job] = 0;
+                if (p.ok) p.ok[job] = 0;
+            }
+            return;
+        }
+    }
     double pose[6], R[9];
     for (int k = 0; k < 6; k++) pose[k] = p.pose[(size_t)job * 6 + k];
     rodrigues_v2m(pose, R);
@@ -56,6 +78,21 @@ __device__ __forceinline__ void k_pose_uncertainty_body(const UncParams& p) {
 #pragma unroll
     for (int k = 0; k < 32; k++) v[k] = 0;
     for (int i = tid; i < cnt; i += UNC_THREADS) {
+        if constexpr (RIG) {
+            const int code = sel[i], fr = job * n_cams + (code >> 11), cell = code & 2047;
+            const int16_t* co = p.coords + ((size_t)fr * DSAC_N_CONST + cell) * 3;
+            const int32_t* px = p.pix + (size_t)fr * p.pix_stride + cell * 2;
+            const double Y[3] = {(double)co[0], (double)co[1], (double)co[2]}, e[3] = {(double)px[0], (double)px[1], 0};
+            const double* E = rig.ext + (size_t)fr * 12;
+            double Rk[9], tk[3];
+            rig_compose(E, E + 9, R, pose + 3, Rk, tk);
+            const Cam cm = frame_cam<PER_FRAME>(p, fr);
+            IftPoint P;
+            ift_point_setup(Rk, tk, Y, e, cm.f, cm.cx, cm.cy, false, P);
+            ift_point_to_rig(E, P);
+            ift_point_gn(P, v);
+            continue;
+        }
         const int c = sel[i];
         const double Y[3] = {(double)coords[c * 3], (double)coords[c * 3 + 1], (double)coords[c * 3 + 2]};
         double e[3];
@@ -69,7 +106,30 @@ __device__ __forceinline__ void k_pose_uncertainty_body(const UncParams& p) {
         ift_point_setup(R, pose + 3, Y, e, cam.f, cam.cx, cam.cy, RGBD, P);
         ift_point_gn(P, v);
     }
-    {   // support
+    if constexpr (RIG) {   // support over every camera, under its composed pose (the rows k_rig_lift gives k_score)
+        int sup = 0;
+        for (int c2 = 0; c2 < n_cams; c2++) {
+            const int fr = job * n_cams + c2;
+            const double* E = rig.ext + (size_t)fr * 12;
+            double Rk[9], tk[3];
+            rig_compose(E, E + 9, R, pose + 3, Rk, tk);
+            const Cam cm = frame_cam<PER_FRAME>(p, fr);
+            const float r0x = (float)(cm.f * Rk[0]), r0y = (float)(cm.f * Rk[1]), r0z = (float)(cm.f * Rk[2]), r0w = (float)(cm.f * tk[0]);
+            const float r1x = (float)(cm.f * Rk[3]), r1y = (float)(cm.f * Rk[4]), r1z = (float)(cm.f * Rk[5]), r1w = (float)(cm.f * tk[1]);
+            const float r2x = (float)Rk[6], r2y = (float)Rk[7], r2z = (float)Rk[8], r2w = (float)tk[2];
+            const float cxf = (float)cm.cx, cyf = (float)cm.cy;
+            const int16_t* co = p.coords + (size_t)fr * DSAC_N_CONST * 3;
+            const int32_t* px = p.pix + (size_t)fr * p.pix_stride;
+            for (int c = tid; c < DSAC_N_CONST; c += UNC_THREADS) {
+                float az;
+                const float err = score_pair_error<true>(r0x, r0y, r0z, r0w, r1x, r1y, r1z, r1w, r2x, r2y, r2z, r2w, (float)co[c * 3],
+                                                         (float)co[c * 3 + 1], (float)co[c * 3 + 2], (float)px[c * 2] - cxf,
+                                                         (float)px[c * 2 + 1] - cyf, &az);
+                sup += err < p.thr ? 1 : 0;
+            }
+        }
+        v[22] = (double)sup;
+    } else {   // support
         const float r0x = (float)(cam.f * R[0]), r0y = (float)(cam.f * R[1]), r0z = (float)(cam.f * R[2]), r0w = (float)(cam.f * pose[3]);
         const float r1x = (float)(cam.f * R[3]), r1y = (float)(cam.f * R[4]), r1z = (float)(cam.f * R[5]), r1w = (float)(cam.f * pose[4]);
         const float r2x = (float)R[6], r2y = (float)R[7], r2z = (float)R[8], r2w = (float)pose[5];
@@ -120,6 +180,13 @@ __global__ void __launch_bounds__(UNC_THREADS) k_pose_uncertainty(UncParams p) {
 __global__ void __launch_bounds__(UNC_THREADS) k_pose_uncertainty_cam(UncParams p) { k_pose_uncertainty_body<true, false>(p); }
 __global__ void __launch_bounds__(UNC_THREADS) k_pose_uncertainty_rgbd(UncParams p) { k_pose_uncertainty_body<false, true>(p); }
 __global__ void __launch_bounds__(UNC_THREADS) k_pose_uncertainty_rgbd_cam(UncParams p) { k_pose_uncertainty_body<true, true>(p); }
+__global__ void __launch_bounds__(UNC_THREADS) k_pose_uncertainty_rig(UncParams p, RigRefine rig, const uint32_t* status) {
+    k_pose_uncertainty_body<false, false, true>(p, rig, status);
+}
+__global__ void __launch_bounds__(UNC_THREADS) k_pose_uncertainty_rig_cam(UncParams p, RigRefine rig, const uint32_t* status) {
+    k_pose_uncertainty_body<true, false, true>(p, rig, status);
+}
+constexpr void (*k_pose_uncertainty_rig_tab[2])(UncParams, RigRefine, const uint32_t*) = {k_pose_uncertainty_rig, k_pose_uncertainty_rig_cam};
 
 inline void launch_pose_uncertainty(const UncParams& p, unsigned jobs, cudaStream_t stream) {
     // [per-frame camera][RGB-D]

@@ -35,6 +35,7 @@ EXPORTS = [
     "dsac_sampling_log_prob_backward_device", "dsac_set_coord_derivatives", "dsac_pose_uncertainty_device",
     "dsac_last_pass", "dsac_set_pose_priors_device", "dsac_pose_modes_device", "dsac_forward_rig_device",
     "dsac_backward_rig_device", "dsac_backward_rig_pose_device", "dsac_rig_refined_jp6_device",
+    "dsac_rig_pose_uncertainty_device", "dsac_set_rig_pose_priors_device",
 ]
 
 ST_OBJ_DRAW_EXHAUSTED = 8    # DSAC_ST_OBJ_DRAW_EXHAUSTED
@@ -242,6 +243,9 @@ def load(build_if_missing=True):
                                              C.POINTER(RigBackwardOut), C.c_void_p]
     lib.dsac_backward_rig_pose_device.argtypes = lib.dsac_backward_rig_device.argtypes
     lib.dsac_rig_refined_jp6_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.dsac_rig_pose_uncertainty_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(PoseUncertaintyOut), C.c_void_p]
+    lib.dsac_set_rig_pose_priors_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_double,
+                                                    C.c_void_p]
     lib.dsac_backward_pose_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]
     lib.dsac_backward_dsac_pose_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(BackwardDsacOut),
                                                    C.c_void_p, C.c_float, C.c_void_p]
@@ -714,6 +718,27 @@ class Engine:
         preceding forward_rig_device over n frames."""
         self._check(self.lib.dsac_rig_refined_jp6_device(self.h, n, C.c_void_p(d_jp6) if d_jp6 else None,
                                                          C.c_void_p(stream) if stream else None))
+
+    def set_rig_pose_priors_device(self, n, n_cameras, k, d_poses, d_info=None, gate=0.0, stream=None):
+        """dsac_set_rig_pose_priors_device: k cv rig poses per rig, float64 [n / n_cameras][k][6] on the device (raw pointer as
+        int), join the pools of the following forward_rig_device passes over n frames of n_cameras cameras; d_info (float64
+        [n / n_cameras][k][6][6] information matrices in the rig chart, or None) gates every camera's sampled hypotheses at
+        the chi^2 bound `gate` (INTEGRATION.md, "Rig tracking").  d_poses None / 0 clears them."""
+        self._check(self.lib.dsac_set_rig_pose_priors_device(self.h, n if d_poses else 0, n_cameras if d_poses else 0,
+                                                             k if d_poses else 0, C.c_void_p(d_poses) if d_poses else None,
+                                                             C.c_void_p(d_info) if d_info else None, float(gate),
+                                                             C.c_void_p(stream) if stream else None))
+
+    def rig_pose_uncertainty_device(self, n, n_cameras, stream=None, **ptrs):
+        """dsac_rig_pose_uncertainty_device (raw device pointers as ints): the covariance of each refined rig pose of the
+        preceding forward_rig_device over n frames of n_cameras cameras; ptrs: device destinations of the fields of
+        dsac_pose_uncertainty_out, one entry per rig ([R] and [R][6][6], R = n / n_cameras)."""
+        raw = PoseUncertaintyOut()
+        for k, v in ptrs.items():
+            if k not in _UNC_FIELDS:
+                raise KeyError(k)
+            setattr(raw, k, v)
+        self._check(self.lib.dsac_rig_pose_uncertainty_device(self.h, n, n_cameras, C.byref(raw), C.c_void_p(stream) if stream else None))
 
     def last_pass(self, n):
         """dsac_last_pass: "softam", "dsac" or "rig", the kind of the pass over n frames the engine holds (what

@@ -427,7 +427,8 @@ int dsac_pose_uncertainty_device(dsac_engine* e, int32_t n_frames, const dsac_po
  * pass over n_frames. */
 #define DSAC_PASS_SOFTAM 1
 #define DSAC_PASS_DSAC 2
-#define DSAC_PASS_RIG 3            /* dsac_forward_rig_device: read by the rig backward and dsac_rig_refined_jp6_device only */
+#define DSAC_PASS_RIG 3            /* dsac_forward_rig_device: read by the rig backward, dsac_rig_refined_jp6_device and
+                                      dsac_rig_pose_uncertainty_device only */
 int dsac_last_pass(dsac_engine* e, int32_t n_frames, int32_t* pipeline);
 
 /* Pose modes of the preceding pass (INTEGRATION.md, "Pose modes"): per frame up to M = max_modes distinct refined poses of
@@ -541,6 +542,49 @@ int dsac_backward_rig_pose_device(dsac_engine* e, int32_t n_frames, const double
 /* jp 6-vectors [R][6] of the refined rig poses of the preceding dsac_forward_rig_device over n_frames (refusals as the rig
  * backward's, and a NULL d_jp6). */
 int dsac_rig_refined_jp6_device(dsac_engine* e, int32_t n_frames, double* d_jp6, void* stream);
+
+/* Rig tracking (INTEGRATION.md, "Rig tracking"): the covariance of each refined rig pose, and rig pose priors, so that a rig
+ * runs the tracker loop of "Pose priors".
+ *
+ * dsac_rig_pose_uncertainty_device: "Pose uncertainty" lifted to the rig, one job per rig (jobs = R = n_frames / C) after a
+ * dsac_forward_rig_device over the same n_frames and n_cameras = C.  S is the set of cells, over all the rig's cameras, that
+ * the rig refinement's last accepted step fitted (a recording replay from the soft-argmax rig pose), m = |S|; r_i the
+ * reprojection residual of cell i in its own camera at the composed pose T_c o T_rig with its frame's camera (px); J_i =
+ * dr_i/dxi in the rig chart R = exp([w]x) R*, t = t* + tau.  cov_xi = sigma2 (sum_S J_i^T J_i)^-1, sigma2 = sum_S |r_i|^2 /
+ * (2m - 6), cov_jp6 = M cov_xi M^T at the rig pose (the jp 6-vector of dsac_rig_refined_jp6_device); support counts the
+ * cells of all C cameras (at most 1600 C) whose error in k_score's fp32 arithmetic at the composed pose is below thr2d; n_fit
+ * = m; ok as in dsac_pose_uncertainty_device.  A rig with DSAC_ST_BAD_RIG or DSAC_ST_BAD_PRIOR gets zeros in every output,
+ * ok, n_fit and support included.  C = 1 with a zero extrinsic gives dsac_pose_uncertainty_device's outputs after the
+ * ordinary pass bit for bit.  Ordered after the pass by an event, own scratch: it changes no later result.  DSAC_ERR_ARG,
+ * with the engine left as it was: not after a dsac_forward_rig_device over n_frames, n_cameras not the pass's C, cameras,
+ * cell depth, pose priors or rig pose priors changed since the pass, a submitted pass that has not been awaited, or d_out
+ * NULL.  The outputs are not differentiated. */
+int dsac_rig_pose_uncertainty_device(dsac_engine* e, int32_t n_frames, int32_t n_cameras, const dsac_pose_uncertainty_out* d_out,
+                                     void* stream);
+/* dsac_set_rig_pose_priors_device: k rig poses per rig join the pools of the following dsac_forward_rig_device passes over
+ * n_frames frames of n_cameras = C cameras.  d_poses: DEVICE float64 [R][k][6] cv rig poses (X_cam = R_c (R_j Y + t_j) +
+ * t_c); d_info: DEVICE float64 [R][k][6][6] information matrices in the rig chart R = exp([w]x) R_j, t = t_j + tau
+ * (inv(cov_xi + Q) of dsac_rig_pose_uncertainty_device is one), or NULL; gate a chi^2 bound, finite and > 0 with d_info.
+ * At each rig pass, with the pass's extrinsic (R_c, t_c) of frame f = r C + c, prior j of rig r becomes frame f's prior
+ * T_c o T_j = (R_c R_j, R_c t_j + t_c) (an extrinsic whose rvec is exactly zero keeps the prior's rvec bits) with
+ * information B Lambda_j B^T, B = blockdiag(R_c, R_c); frame f then samples exactly as dsac_forward_device samples it under
+ * dsac_set_pose_priors_device with those priors (quotas stream_chunk(n_hyps - k, n_streams, s), the gate an ordinary
+ * rejection, prior slot n_hyps - k + j of hyp_pose holding the composed pose).  Since xi_cam = B xi_rig for a camera
+ * hypothesis lifted to the rig, the camera-frame gate equals the rig-frame gate of the lifted hypothesis up to rounding.
+ * Camera c's prior slot lifts to pool slot c n_hyps + n_hyps - k + j, which holds rig prior j's own bits: the pool has C
+ * copies of each prior.  A rig whose extrinsics are not all finite, or one of whose composed entries has a non-finite
+ * value or a Lambda whose Cholesky has a pivot below 1e-12 of its diagonal entry, gets DSAC_ST_BAD_PRIOR in all its frames
+ * (nothing sampled) and in its status, and is treated as a DSAC_ST_BAD_RIG rig: its outputs but hyp_pose are zero, its
+ * backward rows are zero and its covariance is zeros; other rigs are unaffected.  Priors are constants of the rig backward.
+ * Copied on `stream` into engine-owned buffers; sticky; d_poses == NULL (other arguments ignored) clears the setting.  A rig
+ * pass over other n_frames or C refuses, and every other forward entry point (dsac_forward, _submit, _device,
+ * dsac_forward_dsac, _device) refuses while the setting is on.  The rig backward, dsac_rig_refined_jp6_device,
+ * dsac_rig_pose_uncertainty_device and dsac_sampling_log_prob*_device refuse a rig pass after which the setting changed.
+ * DSAC_ERR_ARG, with the engine left as it was: n_frames outside [1, max_frames] or not a multiple of C, C outside
+ * [1, DSAC_MAX_RIG_CAMERAS], k outside [1, min(n_hyps, DSAC_MAX_PRIORS)], a bad gate, or a submitted pass that has not been
+ * awaited. */
+int dsac_set_rig_pose_priors_device(dsac_engine* e, int32_t n_frames, int32_t n_cameras, int32_t k, const double* d_poses,
+                                    const double* d_info, double gate, void* stream);
 
 /* Soft-argmax backward seeded by d_grad_ref [n][6] = dOuter/d(refined jp6) instead of dLossMax.
  * No ground truth needed. dloss_dobj / dloss_dpred / clamp as in dsac_backward_device; clamp applies to the total. */
