@@ -98,7 +98,8 @@ def _set_sampling(engine, prediction, logits):
     engine._sampling_key = (id(logits), logits._version, engine.passes + 1)
 
 
-def _set_depth(engine, prediction, depth):
+def _set_depth(engine, prediction, depth, n_cameras=None):
+    # n_cameras: the rig passes' setting (set_rig_cell_depth_device) rather than the ordinary passes'
     if depth is None:
         return
     n = prediction.shape[0]
@@ -107,7 +108,10 @@ def _set_depth(engine, prediction, depth):
                          % (n, _E.N, prediction.device, depth.dtype, tuple(depth.shape), depth.device))
     copy = depth.detach().contiguous()
     stream = torch.cuda.current_stream(prediction.device)
-    engine.set_cell_depth_device(n, copy.data_ptr(), stream.cuda_stream)
+    if n_cameras is None:
+        engine.set_cell_depth_device(n, copy.data_ptr(), stream.cuda_stream)
+    else:
+        engine.set_rig_cell_depth_device(n, int(n_cameras), copy.data_ptr(), stream.cuda_stream)
     copy.record_stream(stream)
 
 
@@ -453,34 +457,36 @@ class _RigSoftam(torch.autograd.Function):
 
 
 def rig_softam_loss(engine, prediction, pix, cam_from_rig, n_cameras, gt_jp, frame0=0, clamp=0.1, cameras=None,
-                    sampling_logits=None, rig_priors=None):
+                    sampling_logits=None, rig_priors=None, cell_depth=None):
     """Per-rig loss of the rig pass (rig_pose's rig layout; INTEGRATION.md, "Rig gradients"): dLossMax's loss of each refined
     rig pose against gt_jp float64 [R][12], float64 [R]; differentiable with respect to `prediction` through every camera's
     scene coordinates, by the implicit-function derivatives whatever the engine's set_coord_derivatives.  clamp, cameras
     and sampling_logits as in softam_loss; with sampling_logits, sampling_log_prob gives the REINFORCE term of the rigs.
-    rig_priors as in rig_pose; the priors are constants of the gradient."""
+    rig_priors and cell_depth as in rig_pose; the priors and the depth are constants of the gradient."""
     if gt_jp is None:
         raise ValueError("the loss needs the rig ground-truth poses gt_jp [R][12]")
     _check_rig(engine, prediction, pix, cam_from_rig, n_cameras, gt_jp)
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
     _set_rig_priors(engine, prediction, n_cameras, rig_priors)
+    _set_depth(engine, prediction, cell_depth, n_cameras)
     return _RigSoftam.apply(prediction, engine, pix, cam_from_rig, int(n_cameras), gt_jp, int(frame0), float(clamp))
 
 
 def rig_softam_pose(engine, prediction, pix, cam_from_rig, n_cameras, frame0=0, clamp=0.1, cameras=None, sampling_logits=None,
-                    rig_priors=None):
+                    rig_priors=None, cell_depth=None):
     """Refined pose of every rig as a jp 6-vector [rodrigues(R); t in mm] of the rig frame, float64 [R][6]; differentiable
     with respect to `prediction` as rig_softam_loss.  Needs no ground truth."""
     _check_rig(engine, prediction, pix, cam_from_rig, n_cameras, None)
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
     _set_rig_priors(engine, prediction, n_cameras, rig_priors)
+    _set_depth(engine, prediction, cell_depth, n_cameras)
     return _RigSoftam.apply(prediction, engine, pix, cam_from_rig, int(n_cameras), None, int(frame0), float(clamp))
 
 
 def rig_pose(engine, prediction, pix, cam_from_rig, n_cameras, frame0=0, cameras=None, sampling_logits=None, gt_jp=None,
-             rig_priors=None):
+             rig_priors=None, cell_depth=None):
     """One pose per multi-camera rig (INTEGRATION.md, "Multi-camera rigs"): the n frames of `prediction` are R = n / C rigs
     of C = n_cameras cameras, frame r C + c camera c of rig r, whose extrinsic cam_from_rig[r C + c] (float64 [n][6], a cv
     pose: X_cam = R_c X_rig + t_c) is known.  cameras and sampling_logits as in softam_pose, per frame; gt_jp float64
@@ -490,12 +496,17 @@ def rig_pose(engine, prediction, pix, cam_from_rig, n_cameras, frame0=0, cameras
     status int32 [R]; and with gt_jp loss, rot_err, t_err float64 and correct int32 [R].
     rig_priors = (poses float64 [R][k][6] cv rig poses, info float64 [R][k][6][6] or None, gate) puts k rig poses per rig
     into every camera's hypotheses (INTEGRATION.md, "Rig tracking"); sticky like pose_priors=: None leaves the engine's
-    setting as it is, and Engine.set_rig_pose_priors_device(n, n_cameras, 0, None) clears it."""
+    setting as it is, and Engine.set_rig_pose_priors_device(n, n_cameras, 0, None) clears it.
+    cell_depth float32 [n][1600] (mm per cell of every camera frame, as cell_depth() gathers it) makes the rigs RGB-D:
+    Kabsch hypotheses per camera and a Kabsch refinement of the rig pose over every camera's cells with depth
+    (INTEGRATION.md, "RGB-D rigs"); sticky like rig_priors=, and Engine.set_rig_cell_depth_device(n, n_cameras, None)
+    clears it."""
     C, n, R, pix, shared = _check_rig(engine, prediction, pix, cam_from_rig, n_cameras, gt_jp)
     dev, H = prediction.device, engine.cfg.n_hyps
     _set_cameras(engine, prediction, cameras)
     _set_sampling(engine, prediction, sampling_logits)
     _set_rig_priors(engine, prediction, C, rig_priors)
+    _set_depth(engine, prediction, cell_depth, C)
     stream = torch.cuda.current_stream(dev).cuda_stream
     coords = _coords(engine, prediction.detach().contiguous(), stream)
     ext = cam_from_rig.detach().contiguous()

@@ -803,7 +803,8 @@ struct IftScratch {
 
 // RIG (k_refine_ift_rig, the rig backward): job r is rig r of rig.C cameras, pose the rig's, sel entries cam << 11 | cell
 // at a stride of C K4_MAX_INLIERS (k_refine_rig_rec).  A cell is set up in its own camera frame and mapped to the rig frame
-// (ift_point_to_rig); its row is its camera frame's, and drefobj is [R][6][C N 3], camera-major.
+// (ift_point_to_rig); its row is its camera frame's, and drefobj is [R][6][C N 3], camera-major.  RIG with RGBD
+// (k_refine_ift_rig_rgbd, RGB-D rigs): the residual is the cell's in its own camera frame, against its eye point.
 template <bool PER_FRAME, bool RGBD, bool RIG = false>
 __device__ __forceinline__ void k_refine_ift_body(const IftParams& p, RigRefine rig = RigRefine{}) {
     __shared__ double s_red[IFT_WARPS][32];
@@ -828,12 +829,17 @@ __device__ __forceinline__ void k_refine_ift_body(const IftParams& p, RigRefine 
             const int code = sel[i], fr = frame * n_cams + (code >> 11), cell = code & 2047;
             const int16_t* co = p.coords + ((size_t)fr * DSAC_N_CONST + cell) * 3;
             const int32_t* px = p.pix + (size_t)fr * p.pix_stride + cell * 2;
-            const double Y[3] = {(double)co[0], (double)co[1], (double)co[2]}, e[3] = {(double)px[0], (double)px[1], 0};
+            const double Y[3] = {(double)co[0], (double)co[1], (double)co[2]};
+            double e[3] = {(double)px[0], (double)px[1], 0};
+            if constexpr (RGBD) {
+                const double* ey = p.eye + ((size_t)fr * DSAC_N_CONST + cell) * 3;
+                e[0] = ey[0]; e[1] = ey[1]; e[2] = ey[2];
+            }
             const double* E = rig.ext + (size_t)fr * 12;
             double Rk[9], tk[3];
             rig_compose(E, E + 9, R, pose + 3, Rk, tk);
             const Cam cm = frame_cam<PER_FRAME>(p, fr);
-            ift_point_setup(Rk, tk, Y, e, cm.f, cm.cx, cm.cy, false, P);
+            ift_point_setup(Rk, tk, Y, e, cm.f, cm.cx, cm.cy, RGBD, P);
             ift_point_to_rig(E, P);
             return;
         }
@@ -927,7 +933,11 @@ __global__ void __launch_bounds__(IFT_THREADS) k_refine_ift_rgbd(IftParams p) { 
 __global__ void __launch_bounds__(IFT_THREADS) k_refine_ift_rgbd_cam(IftParams p) { k_refine_ift_body<true, true>(p); }
 __global__ void __launch_bounds__(IFT_THREADS) k_refine_ift_rig(IftParams p, RigRefine rig) { k_refine_ift_body<false, false, true>(p, rig); }
 __global__ void __launch_bounds__(IFT_THREADS) k_refine_ift_rig_cam(IftParams p, RigRefine rig) { k_refine_ift_body<true, false, true>(p, rig); }
-constexpr void (*k_refine_ift_rig_tab[2])(IftParams, RigRefine) = {k_refine_ift_rig, k_refine_ift_rig_cam};
+__global__ void __launch_bounds__(IFT_THREADS) k_refine_ift_rig_rgbd(IftParams p, RigRefine rig) { k_refine_ift_body<false, true, true>(p, rig); }
+__global__ void __launch_bounds__(IFT_THREADS) k_refine_ift_rig_rgbd_cam(IftParams p, RigRefine rig) { k_refine_ift_body<true, true, true>(p, rig); }
+// [per-frame camera][RGB-D]
+constexpr void (*k_refine_ift_rig_tab[2][2])(IftParams, RigRefine) = {{k_refine_ift_rig, k_refine_ift_rig_rgbd},
+                                                                     {k_refine_ift_rig_cam, k_refine_ift_rig_rgbd_cam}};
 
 inline void launch_refine_ift(const IftParams& p, unsigned jobs, cudaStream_t stream) {
     // [per-frame camera][RGB-D]

@@ -130,9 +130,9 @@ class Handle {
 using Stream = Handle<cudaStream_t, cudaStreamDestroy>;
 using Event = Handle<cudaEvent_t, cudaEventDestroy>;
 
-// The per-frame settings of the following passes, indices into dsac_engine::set.  SET_RIG_PRIORS is read by the rig pass
-// only; every other forward pass refuses to start while it is set.
-enum { SET_CAMS, SET_LOGITS, SET_DEPTH, SET_PRIORS, SET_RIG_PRIORS, SET_COUNT };
+// The per-frame settings of the following passes, indices into dsac_engine::set.  SET_RIG_PRIORS and SET_RIG_DEPTH are
+// read by the rig pass only; every other forward pass refuses to start while one of them is set.
+enum { SET_CAMS, SET_LOGITS, SET_DEPTH, SET_PRIORS, SET_RIG_PRIORS, SET_RIG_DEPTH, SET_COUNT };
 
 // One per-frame setting: the frames it covers (0: off), a generation that changes with every update, and the event
 // recorded after an update's copy or kernel, which a pass waits for before it reads the setting's buffers.
@@ -165,7 +165,10 @@ struct Pass {
     bool prior_gate = false;
     double prior_chi2 = 0;
     int rig_c = 0;                  // a rig pass's cameras per rig (its gt: the rig ground truth, null without DSAC_STAGE_EVAL)
-    bool rgbd() const { return set_n[SET_DEPTH] > 0; }
+    // the cell depth the pass read: the cell depth setting's (d_depth) or, in a rig pass, the rig cell depth's (d_rig_depth);
+    // null: an RGB pass
+    const float* depth = nullptr;
+    bool rgbd() const { return depth != nullptr; }
 };
 
 struct dsac_engine {
@@ -218,6 +221,10 @@ struct dsac_engine {
     int rig_prior_k = 0, rig_prior_c = 0;
     bool rig_prior_gate = false;
     double rig_prior_chi2 = 0;
+    // RGB-D rigs (dsac_set_rig_cell_depth_device): the rig passes' per-cell depth of rig_depth_c cameras per rig, sized once for
+    // max_frames on first use; the passes' eye coordinates go to d_eye as an ordinary RGB-D pass's
+    DevMem<float> d_rig_depth;       // [max_frames][N] (mm)
+    int rig_depth_c = 0;
     // per-dataset cameras of the pre-training data paths (dsac_set_dataset_cameras), indexed by dataset frame; grow-only.
     // ds_cams_n == 0: no table.  ds_cam0 is entry 0 on the host: the frame size and raw_data every entry shares.
     DevMem<ObjCam> d_ds_cams;
@@ -567,6 +574,9 @@ int dsac_engine_create(const dsac_config* cfg, dsac_engine** out) {
         CUC(cudaFuncSetAttribute(k_refine_tab[cam], cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
         CUC(cudaFuncSetAttribute(k_refine_rgbd_tab[cam], cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
         CUC(cudaFuncSetAttribute(k_refine_rig_tab[cam], cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+        // the RGB-D rig refinement stages its Kabsch fit's point pairs in dynamic shared memory (refine.cuh)
+        CUC(cudaFuncSetAttribute(k_refine_rig_rgbd_tab[cam], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rig_kabsch_smem(RIG_MAX_CAMERAS)));
+        CUC(cudaFuncSetAttribute(k_refine_rig_rgbd_rec_tab[cam], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rig_kabsch_smem(RIG_MAX_CAMERAS)));
         if (const char* co = getenv("DSAC_K1_CARVEOUT"))
             CUC(cudaFuncSetAttribute(k_sample_tab[cam][0][0], cudaFuncAttributePreferredSharedMemoryCarveout, atoi(co)));
     }
@@ -766,12 +776,13 @@ static const struct {
     {"dsac_set_cell_depth_device", "frames of the cell depth (dsac_set_cell_depth_device)", "cell depth was"},
     {"dsac_set_pose_priors_device", "frames of the pose priors (dsac_set_pose_priors_device)", "pose priors were"},
     {"dsac_set_rig_pose_priors_device", "frames of the rig pose priors (dsac_set_rig_pose_priors_device)", "rig pose priors were"},
+    {"dsac_set_rig_cell_depth_device", "frames of the rig cell depth (dsac_set_rig_cell_depth_device)", "rig cell depth was"},
 };
 
 // The start every forward entry point shares: the batch matches each setting in force, each of `streams` waits for the
 // settings' updates, and the record of the pass takes its inputs and the settings' snapshot.  A pipeline's entry point
 // sets the record's kind once the engine holds a pass of it.  rig: the rig pass, the only one that reads the rig pose
-// priors; any other refuses while they are set rather than ignore them.
+// priors and the rig cell depth; any other refuses while one of them is set rather than ignore it.
 static int pass_begin(dsac_engine* e, int32_t kind, int32_t n, int64_t frame0, const int16_t* coords, const int32_t* pix,
                       int32_t pix_shared, const double* gt, std::initializer_list<cudaStream_t> streams, bool rig = false) {
     Pass p;
@@ -779,6 +790,9 @@ static int pass_begin(dsac_engine* e, int32_t kind, int32_t n, int64_t frame0, c
         const Setting& s = e->set[i];
         if (i == SET_RIG_PRIORS && s.n && !rig)
             return fail(e, DSAC_ERR_ARG, "rig pose priors are set (%s), which only dsac_forward_rig_device reads: clear them first",
+                        k_setting[i].setter);
+        if (i == SET_RIG_DEPTH && s.n && !rig)
+            return fail(e, DSAC_ERR_ARG, "rig cell depth is set (%s), which only dsac_forward_rig_device reads: clear it first",
                         k_setting[i].setter);
         if (s.n && n != s.n) return fail(e, DSAC_ERR_ARG, "n_frames %d differs from the %d %s", n, s.n, k_setting[i].frames);
         if (s.n)
@@ -791,6 +805,8 @@ static int pass_begin(dsac_engine* e, int32_t kind, int32_t n, int64_t frame0, c
         p.prior_pose = e->d_prior_pose; p.prior_tab = e->d_prior_tab; p.prior_bad = e->d_prior_bad;
         p.prior_gate = e->prior_gate; p.prior_chi2 = e->prior_chi2;
     }
+    if (e->set[SET_DEPTH].n) p.depth = e->d_depth;
+    else if (e->set[SET_RIG_DEPTH].n) p.depth = e->d_rig_depth;   // (a rig pass: any other refused above)
     p.kind = kind;
     p.n = n;
     p.coords = coords; p.pix = pix; p.pix_shared = pix_shared; p.gt = gt;
@@ -907,8 +923,9 @@ static int sampling_log_prob_run(dsac_engine* e, const char* who, int32_t n, dou
                                  void* stream_v) {
     if (!e) return DSAC_ERR_ARG;
     if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "%s: a submitted pass has not been awaited (dsac_forward_wait)", who);
-    const unsigned rig_priors = e->pass.kind == DSAC_PASS_RIG ? 1u << SET_RIG_PRIORS : 0u;   // (a rig pass's consumers only)
-    if (int rc = pass_check(e, who, n, PASS_GUIDED, SETTINGS_SAMPLING | rig_priors)) return rc;
+    // (the rig settings: a rig pass's consumers only)
+    const unsigned rig_settings = e->pass.kind == DSAC_PASS_RIG ? 1u << SET_RIG_PRIORS | 1u << SET_RIG_DEPTH : 0u;
+    if (int rc = pass_check(e, who, n, PASS_GUIDED, SETTINGS_SAMPLING | rig_settings)) return rc;
     if ((!d_logp && !d_grad_logp) || (d_grad_logp && !d_grad)) return fail(e, DSAC_ERR_ARG, "%s: null output", who);
     cudaStream_t stream = (cudaStream_t)stream_v;
     CU(cudaSetDevice(e->cfg.device));
@@ -933,6 +950,19 @@ int dsac_sampling_log_prob_backward_device(dsac_engine* e, int32_t n, const doub
     return sampling_log_prob_run(e, "dsac_sampling_log_prob_backward_device", n, nullptr, d_grad_logp, d_grad_logits, stream);
 }
 
+// The update both cell depth settings share: the copy of n frames of depth into `buf` (sized once for max_frames), and the
+// eye coordinates and skip bits of the passes that read it.
+static int depth_update(dsac_engine* e, Setting& s, DevMem<float>& buf, int32_t n, const float* d_depth, cudaStream_t stream) {
+    CU(cudaSetDevice(e->cfg.device));
+    const size_t cells = (size_t)e->cfg.max_frames * DSAC_N;
+    CU(buf.reserve(cells * sizeof(float)));
+    CU(e->d_eye.reserve(cells * 3 * sizeof(double)));
+    CU(e->d_rgbd_skip.reserve((size_t)e->cfg.max_frames * sizeof(uint32_t)));
+    if (int rc = setting_begin(e, s, stream)) return rc;
+    CU(cudaMemcpyAsync(buf.get(), d_depth, (size_t)n * DSAC_N * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+    return setting_commit(e, s, n, stream);
+}
+
 int dsac_set_cell_depth_device(dsac_engine* e, int32_t n, const float* d_depth, void* stream_v) {
     if (!e) return DSAC_ERR_ARG;
     if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "dsac_set_cell_depth_device: a submitted pass has not been awaited (dsac_forward_wait)");
@@ -943,15 +973,7 @@ int dsac_set_cell_depth_device(dsac_engine* e, int32_t n, const float* d_depth, 
     }
     if (n < 1 || n > e->cfg.max_frames)
         return fail(e, DSAC_ERR_ARG, "dsac_set_cell_depth_device: n %d out of range [1,%d]", n, e->cfg.max_frames);
-    cudaStream_t stream = (cudaStream_t)stream_v;
-    CU(cudaSetDevice(e->cfg.device));
-    const size_t cells = (size_t)e->cfg.max_frames * DSAC_N;
-    CU(e->d_depth.reserve(cells * sizeof(float)));
-    CU(e->d_eye.reserve(cells * 3 * sizeof(double)));
-    CU(e->d_rgbd_skip.reserve((size_t)e->cfg.max_frames * sizeof(uint32_t)));
-    if (int rc = setting_begin(e, s, stream)) return rc;
-    CU(cudaMemcpyAsync(e->d_depth.get(), d_depth, (size_t)n * DSAC_N * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-    return setting_commit(e, s, n, stream);
+    return depth_update(e, s, e->d_depth, n, d_depth, (cudaStream_t)stream_v);
 }
 
 int dsac_set_pose_priors_device(dsac_engine* e, int32_t n, int32_t k, const double* d_poses, const double* d_info, double gate,
@@ -1103,7 +1125,7 @@ static int forward_range(dsac_engine* e, int32_t off, int32_t n, int64_t frame0,
             const int ps = pix_shared ? 0 : DSAC_N * 2;
             const Cam cam0{c.focal, c.cx, c.cy};
             const uint32_t* gbad = guided ? gg.bad : nullptr;
-            k_rgbd_eye_tab[cam]<<<(unsigned)n, KE_THREADS, 0, stream>>>(e->d_depth + o * Nn, d_pix, ps, cam0, cams, gbad, e->d_eye + o * Nn * 3, e->d_rgbd_skip + o);
+            k_rgbd_eye_tab[cam]<<<(unsigned)n, KE_THREADS, 0, stream>>>(e->pass.depth + o * Nn, d_pix, ps, cam0, cams, gbad, e->d_eye + o * Nn * 3, e->d_rgbd_skip + o);
             e->launches++;
         }
         SampleParams sp;

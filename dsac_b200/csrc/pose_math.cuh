@@ -100,6 +100,14 @@ DSAC_HD void rig_lift(const double Rc[9], const double tc[3], const double R[9],
         to[i] = Rc[i] * d[0] + Rc[3 + i] * d[1] + Rc[6 + i] * d[2];
     }
 }
+// The rig-frame point of camera-frame point e: Rc^T (e - tc), so that |Rc (R Y + t) + tc - e| = |R Y + t - Rc^T (e - tc)|.
+// An extrinsic rotation that is exactly I (a zero rvec) gives e - tc exactly, and with tc = 0 e itself.
+DSAC_HD void rig_point(const double Rc[9], const double tc[3], const double e[3], double o[3]) {
+    const double d[3] = {e[0] - tc[0], e[1] - tc[1], e[2] - tc[2]};
+    bool ident = true;
+    for (int k = 0; k < 9; k++) ident = ident && Rc[k] == (k % 4 == 0 ? 1.0 : 0.0);
+    for (int i = 0; i < 3; i++) o[i] = ident ? d[i] : Rc[i] * d[0] + Rc[3 + i] * d[1] + Rc[6 + i] * d[2];
+}
 
 // The angle (degrees) of a relative rotation from its trace, as maxloss.h and Hypothesis::calcAngularDistance compute
 // it: the trace clamped to [-1, 3], then 180 acos((trace - 1) / 2) / pi.

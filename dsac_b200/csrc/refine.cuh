@@ -146,10 +146,13 @@ __device__ double max_loss_dev(const double R1[9], const double t1[3], const dou
 // The cells are read from global memory rather than staged: C frames do not fit in shared memory.  A rig with
 // DSAC_ST_BAD_RIG or DSAC_ST_BAD_PRIOR in status gets zero outputs.  RIG with RECORD (k_refine_rig_rec, the rig backward) records those entries
 // at a stride of C K4_MAX_INLIERS per rig.
+// RIG with RGBD (k_refine_rig_rgbd, RGB-D rigs): eye holds every camera frame's eye points, each camera's selection takes
+// the cells with depth in its own frame, and the Kabsch fit maps the scene coordinates to the rig-frame eye points
+// Rc^T (e - tc) (rig_point), the exact minimiser of sum |Rc (R Y + t) + tc - e|^2.  Its C K4_MAX_INLIERS point pairs are
+// staged in dynamic shared memory of rig_kabsch_smem(C) bytes.
 template <bool PER_FRAME, bool RGBD = false, bool RECORD = false, bool RIG = false>
 __device__ __forceinline__ void k_refine_body(const RefineParams& p, const double* eye = nullptr, uint16_t* rec_sel = nullptr,
                                               int32_t* rec_count = nullptr, RigRefine rig = RigRefine{}) {
-    static_assert(!(RIG && RGBD), "a rig refines RGB frames");
     constexpr int NC = RIG ? RIG_MAX_CAMERAS : 1;   // camera frames per job, at most
     // the frame's scene coordinates (int16 mm, this job's perturbation applied) and pixel positions, staged once per job:
     // every refinement step reads all of them for the inlier flags and the selected ones in each LM pass
@@ -392,7 +395,10 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p, const doubl
                 for (int k0 = 0; k0 < DSAC_N_CONST && count < p.inlier_count; k0 += 32) {
                     const int c = __ldg(perm + k0 + lane);
                     bool flag = (bits[c >> 5] >> (c & 31)) & 1u;
-                    if constexpr (RGBD) flag = flag && __ldg(eye + ((size_t)frame * DSAC_N_CONST + c) * 3 + 2) > 0.0;   // (NaN: no depth)
+                    if constexpr (RGBD) {   // (NaN: no depth; RIG: in camera cc's frame)
+                        const size_t ef = RIG ? (size_t)frame * n_cams + cc : (size_t)frame;
+                        flag = flag && __ldg(eye + (ef * DSAC_N_CONST + c) * 3 + 2) > 0.0;
+                    }
                     const uint32_t m = __ballot_sync(0xffffffffu, flag);
                     const int rank = count + __popc(m & ((1u << lane) - 1u));
                     if (flag && rank < p.inlier_count) {
@@ -409,7 +415,28 @@ __device__ __forceinline__ void k_refine_body(const RefineParams& p, const doubl
         const int count = s_count;
         if (count < 50) break;  // cnn_softam.h:1136
 
-        if constexpr (RGBD) {
+        if constexpr (RGBD && RIG) {
+            // ---- Kabsch fit of the selected cells of every camera, scene to rig-frame eye point, in selection order
+            extern __shared__ double s_kdyn[];   // [C K4_MAX_INLIERS * 3] scene, then as many rig-frame eye coordinates
+            double* ka = s_kdyn;
+            double* kb = s_kdyn + (size_t)n_cams * K4_MAX_INLIERS * 3;
+            for (int i = tid; i < count; i += K4_THREADS) {
+                const int code = s_sel[i], fr = frame * n_cams + (code >> 11), cell = code & 2047;
+                const int16_t* co = p.coords + ((size_t)fr * DSAC_N_CONST + cell) * 3;
+                const double* E = rig.ext + (size_t)fr * 12;
+                ka[i * 3] = (double)__ldg(co); ka[i * 3 + 1] = (double)__ldg(co + 1); ka[i * 3 + 2] = (double)__ldg(co + 2);
+                rig_point(E, E + 9, eye + ((size_t)fr * DSAC_N_CONST + cell) * 3, kb + i * 3);
+            }
+            __syncthreads();
+            if (tid == 0) {
+                double R[9], t[3], r[3];
+                kabsch_fit(count, ka, kb, R, t);
+                rodrigues_m2v(R, r);
+                s_param[0] = r[0]; s_param[1] = r[1]; s_param[2] = r[2];
+                s_param[3] = t[0]; s_param[4] = t[1]; s_param[5] = t[2];
+            }
+            __syncthreads();
+        } else if constexpr (RGBD) {
             // ---- Kabsch fit of the selected cells: gathered in selection order, one thread fits
             __shared__ double s_ka[K4_MAX_INLIERS * 3], s_kb[K4_MAX_INLIERS * 3];
             for (int i = tid; i < count; i += K4_THREADS) {
@@ -572,6 +599,27 @@ constexpr void (*k_refine_rgbd_rec_tab[2])(RefineParams, const double*, uint16_t
 constexpr void (*k_refine_rig_tab[2])(RefineParams, RigRefine) = {k_refine_rig, k_refine_rig_cam};
 constexpr void (*k_refine_rig_rec_tab[2])(RefineParams, RigRefine, uint16_t*, int32_t*) = {k_refine_rig_rec, k_refine_rig_rec_cam};
 
+// RGB-D rigs: eye [n_frames][N][3] of every camera frame, and the dynamic shared memory of the Kabsch fit
+// (rig_kabsch_smem(rig.C) bytes; 48 KB at C = 8)
+constexpr size_t rig_kabsch_smem(int C) { return (size_t)2 * C * K4_MAX_INLIERS * 3 * sizeof(double); }
+__global__ void __launch_bounds__(K4_THREADS, 2) k_refine_rig_rgbd(RefineParams p, RigRefine rig, const double* eye) {
+    k_refine_body<false, true, false, true>(p, eye, nullptr, nullptr, rig);
+}
+__global__ void __launch_bounds__(K4_THREADS, 2) k_refine_rig_rgbd_cam(RefineParams p, RigRefine rig, const double* eye) {
+    k_refine_body<true, true, false, true>(p, eye, nullptr, nullptr, rig);
+}
+__global__ void __launch_bounds__(K4_THREADS, 2) k_refine_rig_rgbd_rec(RefineParams p, RigRefine rig, const double* eye, uint16_t* rec_sel,
+                                                                       int32_t* rec_count) {
+    k_refine_body<false, true, true, true>(p, eye, rec_sel, rec_count, rig);
+}
+__global__ void __launch_bounds__(K4_THREADS, 2) k_refine_rig_rgbd_rec_cam(RefineParams p, RigRefine rig, const double* eye, uint16_t* rec_sel,
+                                                                           int32_t* rec_count) {
+    k_refine_body<true, true, true, true>(p, eye, rec_sel, rec_count, rig);
+}
+constexpr void (*k_refine_rig_rgbd_tab[2])(RefineParams, RigRefine, const double*) = {k_refine_rig_rgbd, k_refine_rig_rgbd_cam};
+constexpr void (*k_refine_rig_rgbd_rec_tab[2])(RefineParams, RigRefine, const double*, uint16_t*, int32_t*) = {k_refine_rig_rgbd_rec,
+                                                                                                          k_refine_rig_rgbd_rec_cam};
+
 // one CTA per job, with the instantiation the parameters ask for; eye != null: an RGB-D pass
 inline void launch_refine(const RefineParams& p, unsigned jobs, cudaStream_t stream, const double* eye = nullptr) {
     if (eye) k_refine_rgbd_tab[p.cams != nullptr]<<<jobs, K4_THREADS, 0, stream>>>(p, eye);
@@ -581,6 +629,19 @@ inline void launch_refine_record(const RefineParams& p, unsigned jobs, cudaStrea
                                  int32_t* rec_count) {
     if (eye) k_refine_rgbd_rec_tab[p.cams != nullptr]<<<jobs, K4_THREADS, 0, stream>>>(p, eye, rec_sel, rec_count);
     else k_refine_rec_tab[p.cams != nullptr]<<<jobs, K4_THREADS, 0, stream>>>(p, rec_sel, rec_count);
+}
+// one CTA per rig (p.n_jobs jobs), with the instantiation the parameters ask for: eye != null an RGB-D rig, rec_sel != null the
+// recording replay.  (The engine raises the RGB-D forms' dynamic shared memory limit to rig_kabsch_smem(RIG_MAX_CAMERAS) at
+// creation: with their static shared memory it exceeds the default at C = 8.)
+inline void launch_refine_rig(const RefineParams& p, RigRefine rig, cudaStream_t stream, const double* eye = nullptr,
+                              uint16_t* rec_sel = nullptr, int32_t* rec_count = nullptr) {
+    const int cam = p.cams != nullptr;
+    const unsigned jobs = (unsigned)p.n_jobs;
+    const size_t smem = rig_kabsch_smem(rig.C);
+    if (eye && rec_sel) k_refine_rig_rgbd_rec_tab[cam]<<<jobs, K4_THREADS, smem, stream>>>(p, rig, eye, rec_sel, rec_count);
+    else if (eye) k_refine_rig_rgbd_tab[cam]<<<jobs, K4_THREADS, smem, stream>>>(p, rig, eye);
+    else if (rec_sel) k_refine_rig_rec_tab[cam]<<<jobs, K4_THREADS, 0, stream>>>(p, rig, rec_sel, rec_count);
+    else k_refine_rig_tab[cam]<<<jobs, K4_THREADS, 0, stream>>>(p, rig);
 }
 
 }  // namespace dsac

@@ -42,10 +42,11 @@ constexpr int UNC_THREADS = 64, UNC_WARPS = UNC_THREADS / 32;
 // entries cam << 11 | cell at a stride of C K4_MAX_INLIERS (k_refine_rig_rec).  A cell is set up in its own camera frame at
 // the composed pose and mapped to the rig frame (ift_point_to_rig), as k_refine_ift_rig does; the support counts the cells
 // of every camera under its composed pose.  A rig with DSAC_ST_BAD_RIG or DSAC_ST_BAD_PRIOR in rig_status gets zeros.
+// RIG with RGBD (k_pose_uncertainty_rig_rgbd, RGB-D rigs): the residual is the cell's 3-vector in its own camera frame
+// against its eye point (mm), sigma2 over 3m - 6; the support is the reprojection count, with or without depth.
 template <bool PER_FRAME, bool RGBD, bool RIG = false>
 __device__ __forceinline__ void k_pose_uncertainty_body(const UncParams& p, RigRefine rig = RigRefine{},
                                                         const uint32_t* rig_status = nullptr) {
-    static_assert(!(RIG && RGBD), "a rig refines RGB frames");
     __shared__ double s_red[UNC_WARPS][32];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int job = blockIdx.x;
@@ -82,13 +83,18 @@ __device__ __forceinline__ void k_pose_uncertainty_body(const UncParams& p, RigR
             const int code = sel[i], fr = job * n_cams + (code >> 11), cell = code & 2047;
             const int16_t* co = p.coords + ((size_t)fr * DSAC_N_CONST + cell) * 3;
             const int32_t* px = p.pix + (size_t)fr * p.pix_stride + cell * 2;
-            const double Y[3] = {(double)co[0], (double)co[1], (double)co[2]}, e[3] = {(double)px[0], (double)px[1], 0};
+            const double Y[3] = {(double)co[0], (double)co[1], (double)co[2]};
+            double e[3] = {(double)px[0], (double)px[1], 0};
+            if constexpr (RGBD) {
+                const double* ey = p.eye + ((size_t)fr * DSAC_N_CONST + cell) * 3;
+                e[0] = ey[0]; e[1] = ey[1]; e[2] = ey[2];
+            }
             const double* E = rig.ext + (size_t)fr * 12;
             double Rk[9], tk[3];
             rig_compose(E, E + 9, R, pose + 3, Rk, tk);
             const Cam cm = frame_cam<PER_FRAME>(p, fr);
             IftPoint P;
-            ift_point_setup(Rk, tk, Y, e, cm.f, cm.cx, cm.cy, false, P);
+            ift_point_setup(Rk, tk, Y, e, cm.f, cm.cx, cm.cy, RGBD, P);
             ift_point_to_rig(E, P);
             ift_point_gn(P, v);
             continue;
@@ -186,7 +192,15 @@ __global__ void __launch_bounds__(UNC_THREADS) k_pose_uncertainty_rig(UncParams 
 __global__ void __launch_bounds__(UNC_THREADS) k_pose_uncertainty_rig_cam(UncParams p, RigRefine rig, const uint32_t* status) {
     k_pose_uncertainty_body<true, false, true>(p, rig, status);
 }
-constexpr void (*k_pose_uncertainty_rig_tab[2])(UncParams, RigRefine, const uint32_t*) = {k_pose_uncertainty_rig, k_pose_uncertainty_rig_cam};
+__global__ void __launch_bounds__(UNC_THREADS) k_pose_uncertainty_rig_rgbd(UncParams p, RigRefine rig, const uint32_t* status) {
+    k_pose_uncertainty_body<false, true, true>(p, rig, status);
+}
+__global__ void __launch_bounds__(UNC_THREADS) k_pose_uncertainty_rig_rgbd_cam(UncParams p, RigRefine rig, const uint32_t* status) {
+    k_pose_uncertainty_body<true, true, true>(p, rig, status);
+}
+// [per-frame camera][RGB-D]
+constexpr void (*k_pose_uncertainty_rig_tab[2][2])(UncParams, RigRefine, const uint32_t*) = {
+    {k_pose_uncertainty_rig, k_pose_uncertainty_rig_rgbd}, {k_pose_uncertainty_rig_cam, k_pose_uncertainty_rig_rgbd_cam}};
 
 inline void launch_pose_uncertainty(const UncParams& p, unsigned jobs, cudaStream_t stream) {
     // [per-frame camera][RGB-D]

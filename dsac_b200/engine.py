@@ -35,7 +35,7 @@ EXPORTS = [
     "dsac_sampling_log_prob_backward_device", "dsac_set_coord_derivatives", "dsac_pose_uncertainty_device",
     "dsac_last_pass", "dsac_set_pose_priors_device", "dsac_pose_modes_device", "dsac_forward_rig_device",
     "dsac_backward_rig_device", "dsac_backward_rig_pose_device", "dsac_rig_refined_jp6_device",
-    "dsac_rig_pose_uncertainty_device", "dsac_set_rig_pose_priors_device",
+    "dsac_rig_pose_uncertainty_device", "dsac_set_rig_pose_priors_device", "dsac_set_rig_cell_depth_device",
 ]
 
 ST_OBJ_DRAW_EXHAUSTED = 8    # DSAC_ST_OBJ_DRAW_EXHAUSTED
@@ -246,6 +246,7 @@ def load(build_if_missing=True):
     lib.dsac_rig_pose_uncertainty_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(PoseUncertaintyOut), C.c_void_p]
     lib.dsac_set_rig_pose_priors_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_double,
                                                     C.c_void_p]
+    lib.dsac_set_rig_cell_depth_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
     lib.dsac_backward_pose_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]
     lib.dsac_backward_dsac_pose_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(BackwardDsacOut),
                                                    C.c_void_p, C.c_float, C.c_void_p]
@@ -728,6 +729,14 @@ class Engine:
                                                              k if d_poses else 0, C.c_void_p(d_poses) if d_poses else None,
                                                              C.c_void_p(d_info) if d_info else None, float(gate),
                                                              C.c_void_p(stream) if stream else None))
+
+    def set_rig_cell_depth_device(self, n, n_cameras, d_depth, stream=None):
+        """dsac_set_rig_cell_depth_device: float32 [n][1600] depth in mm per cell of every camera frame on the device (raw
+        pointer as int) makes the following forward_rig_device passes over n frames of n_cameras cameras RGB-D rigs
+        (INTEGRATION.md, "RGB-D rigs").  d_depth None / 0 clears it."""
+        self._check(self.lib.dsac_set_rig_cell_depth_device(self.h, n if d_depth else 0, n_cameras if d_depth else 0,
+                                                            C.c_void_p(d_depth) if d_depth else None,
+                                                            C.c_void_p(stream) if stream else None))
 
     def rig_pose_uncertainty_device(self, n, n_cameras, stream=None, **ptrs):
         """dsac_rig_pose_uncertainty_device (raw device pointers as ints): the covariance of each refined rig pose of the

@@ -585,6 +585,31 @@ int dsac_rig_pose_uncertainty_device(dsac_engine* e, int32_t n_frames, int32_t n
  * awaited. */
 int dsac_set_rig_pose_priors_device(dsac_engine* e, int32_t n_frames, int32_t n_cameras, int32_t k, const double* d_poses,
                                     const double* d_info, double gate, void* stream);
+/* RGB-D rigs (INTEGRATION.md, "RGB-D rigs"): dsac_set_rig_cell_depth_device makes the following dsac_forward_rig_device
+ * passes over n_frames frames of n_cameras = C cameras RGB-D passes.  d_depth: DEVICE float32 [n_frames][1600], the depth in
+ * mm at each cell of camera frame f = r C + c, with the rules of dsac_set_cell_depth_device (a cell has depth iff its value
+ * is finite and > 0).  Copied on `stream` into an engine-owned buffer of its own (sized once for max_frames), so neither
+ * depth setting changes the other's values.  With it:
+ *   sample: every camera frame samples exactly as an RGB-D dsac_forward_device samples it (Kabsch minimal sets,
+ *           DSAC_ST_NO_DEPTH and no hypotheses for a frame with fewer than 4 cells with depth, rig pose priors composed as
+ *           before); a NO_DEPTH frame's H zero hypotheses are lifted and scored as any other, and the rig status ORs in
+ *           DSAC_ST_NO_DEPTH without spoiling the rig;
+ *   score:  unchanged (reprojection);
+ *   refine: per camera in order its first <= inlier_count cells of the step's permutation with reprojection error < thr2d
+ *           under its composed pose AND depth in its own frame (fewer than 50 in all stop, DSAC_ST_REFINE_ABORTED), then the
+ *           Kabsch fit of the rig pose from their scene coordinates to their rig-frame eye points R_c^T (e - t_c), the
+ *           minimiser of sum |R_c (R Y + t) + t_c - e|^2 (e - t_c exactly for an extrinsic whose rotation is exactly I).
+ * The rig backward differentiates it with the Kabsch refinement's replays, the IFT of the RGB-D residual for the direct
+ * term and the Kabsch dPNP per frame (depth is not differentiated); dsac_rig_pose_uncertainty_device uses the 3-vector
+ * residual in mm and sigma2 = sum |r|^2 / (3m - 6), the support still counting reprojection inliers.  C = 1 with a zero
+ * extrinsic gives an RGB-D dsac_forward_device's results and its covariance bit for bit (the backward's direct term to
+ * rounding).  Sticky; d_depth == NULL (other arguments ignored)
+ * clears it.  A rig pass over other n_frames or C refuses; while per-frame cell depth (dsac_set_cell_depth_device) is set
+ * the rig pass still refuses.  Every other forward entry point refuses while the setting is on.  The rig backward,
+ * dsac_rig_refined_jp6_device, dsac_rig_pose_uncertainty_device and dsac_sampling_log_prob*_device refuse a rig pass after
+ * which the setting changed.  DSAC_ERR_ARG, with the engine left as it was: n_frames outside [1, max_frames] or not a
+ * multiple of C, C outside [1, DSAC_MAX_RIG_CAMERAS], or a submitted pass that has not been awaited. */
+int dsac_set_rig_cell_depth_device(dsac_engine* e, int32_t n_frames, int32_t n_cameras, const float* d_depth, void* stream);
 
 /* Soft-argmax backward seeded by d_grad_ref [n][6] = dOuter/d(refined jp6) instead of dLossMax.
  * No ground truth needed. dloss_dobj / dloss_dpred / clamp as in dsac_backward_device; clamp applies to the total. */
