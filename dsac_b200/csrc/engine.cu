@@ -65,7 +65,8 @@ static constexpr void (*k1_cells_tab[2])(K1SplitParams, int, int) = {k1_cells, k
 static constexpr void (*k_rgbd_eye_tab[2])(const float*, const int32_t*, int, Cam, const Cam*, const uint32_t*, double*, uint32_t*) = {
     k_rgbd_eye_t<false>, k_rgbd_eye_t<true>};
 static constexpr void (*k_score_tab[2][2])(ScoreParams) = {{k_score<false>, k_score<true>}, {k_score_cam<false>, k_score_cam<true>}};
-static constexpr void (*k_score_rig_tab[2])(ScoreParams) = {k_score_rig<false>, k_score_rig<true>};
+static constexpr void (*k_score_rig_tab[2][2])(ScoreParams) = {{k_score_rig<false, false>, k_score_rig<true, false>},
+                                                                {k_score_rig<false, true>, k_score_rig<true, true>}};
 
 // Owners of the engine's CUDA resources, the only code here that frees any.  Each releases what it holds in its
 // destructor, is move-only, and converts to the raw pointer or handle for use at call sites.
@@ -169,6 +170,11 @@ struct Pass {
     // null: an RGB pass
     const float* depth = nullptr;
     bool rgbd() const { return depth != nullptr; }
+    // a rig pass scored by the rig score hooks (dsac_set_rig_score_hooks): the pair and user it called, which the rig
+    // backward must find registered still; all null: scored in closed form
+    dsac_score_hook rig_hook = nullptr;
+    dsac_score_backward_hook rig_bw_hook = nullptr;
+    void* rig_hook_user = nullptr;
 };
 
 struct dsac_engine {
@@ -181,6 +187,10 @@ struct dsac_engine {
     dsac_score_backward_hook bw_hook = nullptr;
     void* bw_hook_user = nullptr;
     DevMem<double> d_ext_g;         // [n][H][N] dScore/dDiffMap from the backward hook, then its clamped input [n][H] (grow-only)
+    // the rig score hooks (dsac_set_rig_score_hooks), read by the rig passes and the rig backward only
+    dsac_score_hook rig_hook = nullptr;
+    dsac_score_backward_hook rig_bw_hook = nullptr;
+    void* rig_hook_user = nullptr;
     Event ev_fwd;                   // recorded after the last forward launch: the backward waits on it
     DevMem<double> d_kabsch;        // dsac_kabsch: inputs and outputs in one grow-only block
     DevMem<uint64_t> d_reg_keys;    // dsac_register_depth_device: per-pixel scatter keys, grow-only
@@ -294,14 +304,17 @@ struct dsac_engine {
         double* prior_pose;         // [n][k][6] the rig pose priors composed per frame (k_rig_prior_prep), k of the setting
         PriorGate* prior_tab;       // [n][k]
         uint32_t* prior_bad;        // [n]
+        float* dm;                  // [n][P][N] the error images of a hooked rig pass (rig_dm_buf)
     } rig = {};
     DevMem<char> rig_buf;
+    DevMem<char> rig_dm_buf;        // grow-only, sized for the n frames and the pool of the largest hooked rig pass
     // dsac_backward_rig(_pose)_device: the soft-argmax backward's arrays over rigs and pools, the recording replay, the
     // composed poses, w and the support vectors, in one grow-only block that no other call writes, ordered by ev_rig_bw as
     // the uncertainty scratch is by ev_unc
     struct {
         BackwardScratch b;
         double *rec_pose, *w, *u, *frame_grad;
+        double *ext_g, *hook_sog;   // a hooked rig pass: [n][P][N] dScore/dDiffMap from the backward hook, [n][P] its input
         uint16_t* rec_sel;
         int32_t *rec_count, *n_perm;
         uint32_t* status;
@@ -782,9 +795,12 @@ static const struct {
 // The start every forward entry point shares: the batch matches each setting in force, each of `streams` waits for the
 // settings' updates, and the record of the pass takes its inputs and the settings' snapshot.  A pipeline's entry point
 // sets the record's kind once the engine holds a pass of it.  rig: the rig pass, the only one that reads the rig pose
-// priors and the rig cell depth; any other refuses while one of them is set rather than ignore it.
+// priors, the rig cell depth and the rig score hooks; any other refuses while one of them is set rather than ignore it.
 static int pass_begin(dsac_engine* e, int32_t kind, int32_t n, int64_t frame0, const int16_t* coords, const int32_t* pix,
                       int32_t pix_shared, const double* gt, std::initializer_list<cudaStream_t> streams, bool rig = false) {
+    if (e->rig_hook && !rig)
+        return fail(e, DSAC_ERR_ARG,
+                    "rig score hooks are registered (dsac_set_rig_score_hooks), which only dsac_forward_rig_device calls: clear them first");
     Pass p;
     for (int i = 0; i < SET_COUNT; i++) {
         const Setting& s = e->set[i];
@@ -1065,6 +1081,21 @@ int dsac_set_score_backward_hook(dsac_engine* e, dsac_score_backward_hook fn, vo
     if (!e) return DSAC_ERR_ARG;
     e->bw_hook = fn;
     e->bw_hook_user = user;
+    return DSAC_OK;
+}
+
+// The rig passes' twin of the score seam: both hooks or neither; a rig pass reads them, every other forward refuses while
+// they are registered (pass_begin), and the rig backward needs the pair its pass called.
+int dsac_set_rig_score_hooks(dsac_engine* e, dsac_score_hook fn, dsac_score_backward_hook bw_fn, void* user) {
+    static const char* who = "dsac_set_rig_score_hooks";
+    if (!e) return DSAC_ERR_ARG;
+    if (e->pending_chunks) return fail(e, DSAC_ERR_ARG, "%s: a submitted pass has not been awaited (dsac_forward_wait)", who);
+    if (!fn != !bw_fn)
+        return fail(e, DSAC_ERR_ARG, "%s: the forward and the backward hook are set together (both NULL clears them), %s is NULL", who,
+                    fn ? "the backward hook" : "the forward hook");
+    e->rig_hook = fn;
+    e->rig_bw_hook = bw_fn;
+    e->rig_hook_user = fn ? user : nullptr;
     return DSAC_OK;
 }
 

@@ -991,8 +991,9 @@ __global__ void __launch_bounds__(K2_THREADS, K2_MIN_BLOCKS) k_score(ScoreParams
 // the same with the per-frame principal points (ScoreParams::cams)
 template <bool WRITE_DM>
 __global__ void __launch_bounds__(K2_THREADS, K2_MIN_BLOCKS) k_score_cam(ScoreParams p) { k_score_body<WRITE_DM, true>(p); }
-// scores only (no diffmaps, no tail), with or without the per-frame principal points: the cameras of a multi-camera rig
-template <bool PER_FRAME>
-__global__ void __launch_bounds__(K2_THREADS, K2_MIN_BLOCKS) k_score_rig(ScoreParams p) { k_score_body<false, PER_FRAME, false>(p); }
+// scores only (no tail), with or without the per-frame principal points: the cameras of a multi-camera rig.  WRITE_DM: also
+// the error images [n][P][N] of every camera frame against its rig's pool, which the rig score hooks read
+template <bool WRITE_DM, bool PER_FRAME>
+__global__ void __launch_bounds__(K2_THREADS, K2_MIN_BLOCKS) k_score_rig(ScoreParams p) { k_score_body<WRITE_DM, PER_FRAME, false>(p); }
 
 }  // namespace dsac

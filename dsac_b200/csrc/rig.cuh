@@ -5,14 +5,16 @@
 // X_cam = Rc X_rig + tc.  The sampler runs on the frames as in an ordinary pass.  Then:
 //   k_rig_lift   the extrinsics (Rc, tc), the rig status, the pool -- slot j = c H + h of rig r is camera c's hypothesis h
 //                lifted to the rig frame -- and the fp32 rows of every pool pose in every camera of its rig;
-//   k_score_rig  (k_score without its softmax tail) every camera frame against its rig's pool of P = C H poses;
+//   k_score_rig  (k_score without its softmax tail) every camera frame against its rig's pool of P = C H poses; with the
+//                rig score hooks it writes the error images [n][P][N] too and the forward hook replaces its scores;
 //   k_rig_tail   the rig's score of slot j is the sum of its cameras' scores in camera order, then softargmax_tail;
 //   k_refine_rig the refinement of the soft-argmax rig pose over all cameras' cells (refine.cuh).
 // The rig backward (dsac_backward_rig_device, rig_backward_host.inc) is the soft-argmax backward's implicit chain over the
 // pool: k_bw_prep_implicit, k_refine_rig_rec and the 12 dRefineHyp jobs of k_refine_rig, k_bw_combine_implicit and
 // k_refine_ift_rig per rig; k_dpnp_ift per frame; then
 //   k_rig_bw_hypjp    the composed pose T_c o T_j of every (frame, slot) in jp with its Rodrigues Jacobian;
-//   k_dscore_rig      every camera frame against its rig's pool: the direct part into the frame's row, w per (frame, slot);
+//   k_dscore_rig      every camera frame against its rig's pool: the direct part into the frame's row, w per (frame, slot)
+//                     (after a hooked pass k_rig_clamp_broadcast and the backward hook first, whose dScore/dDiffMap it reads);
 //   k_rig_bw_support  per (frame, hypothesis) the 1x6 of path I (dLdAvg L_j) and of path II (sum_c w K_c,j);
 //   k_rig_bw_scatter  per frame, hypotheses in order: both through dPNP onto the minimal set's cells.
 #pragma once
@@ -262,6 +264,18 @@ __global__ void __launch_bounds__(32) k_rig_bw_scatter(RigBwParams p) {
         }
         __syncwarp(0xfff);
     }
+}
+
+// A hooked rig pass (dsac_set_rig_score_hooks): the rig's score output gradients sog [R][P] clamped to +-clamp, as
+// k_clamp_copy clamps an ordinary pass's, and given to every camera frame of the rig [n][P] -- the rig score is the sum of
+// its cameras' scores, so d(rig score) / d(camera score) = 1 -- the input of the rig score backward hook
+__global__ void k_rig_clamp_broadcast(const double* __restrict__ sog, int C, int P, size_t count, double clamp, double* __restrict__ out) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    const size_t f = i / P, j = i - f * P;
+    double v = sog[(f / C) * P + j];
+    if (clamp > 0) v = fmax(-clamp, fmin(clamp, v));
+    out[i] = v;
 }
 
 // the per-rig loss gradient [R] read per frame [n], as k_e2e_grad indexes it

@@ -36,6 +36,7 @@ EXPORTS = [
     "dsac_last_pass", "dsac_set_pose_priors_device", "dsac_pose_modes_device", "dsac_forward_rig_device",
     "dsac_backward_rig_device", "dsac_backward_rig_pose_device", "dsac_rig_refined_jp6_device",
     "dsac_rig_pose_uncertainty_device", "dsac_set_rig_pose_priors_device", "dsac_set_rig_cell_depth_device",
+    "dsac_set_rig_score_hooks",
 ]
 
 ST_OBJ_DRAW_EXHAUSTED = 8    # DSAC_ST_OBJ_DRAW_EXHAUSTED
@@ -247,6 +248,7 @@ def load(build_if_missing=True):
     lib.dsac_set_rig_pose_priors_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_double,
                                                     C.c_void_p]
     lib.dsac_set_rig_cell_depth_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.dsac_set_rig_score_hooks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.dsac_backward_pose_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]
     lib.dsac_backward_dsac_pose_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(BackwardDsacOut),
                                                    C.c_void_p, C.c_float, C.c_void_p]
@@ -401,6 +403,7 @@ class Engine:
             raise RuntimeError("dsac_engine_create failed (%d): %s" % (rc, self.lib.dsac_last_error(None).decode()))
         self.h = h
         self._hook = None
+        self._rig_hooks = None   # the trampolines of set_rig_score_hooks
         self._dataset_cameras = None   # bytes of the dataset camera table installed by set_dataset_cameras, or None
         self.passes = 0   # forward passes started on this engine: the engine holds one pass, autograd.py checks it is still its own
 
@@ -737,6 +740,27 @@ class Engine:
         self._check(self.lib.dsac_set_rig_cell_depth_device(self.h, n if d_depth else 0, n_cameras if d_depth else 0,
                                                             C.c_void_p(d_depth) if d_depth else None,
                                                             C.c_void_p(stream) if stream else None))
+
+    def set_rig_score_hooks(self, fn, bw_fn):
+        """dsac_set_rig_score_hooks: score every rig pass's pool with fn and differentiate it with bw_fn (INTEGRATION.md,
+        "Rig score hooks"); the callables of set_score_hook and set_score_backward_hook, called with n camera frames and
+        P = n_cameras * n_hyps pool slots (ScoreCNN and its backward as they are).  (None, None) clears them."""
+        if fn is None and bw_fn is None:
+            self._check(self.lib.dsac_set_rig_score_hooks(self.h, None, None, None))
+            self._rig_hooks = None
+            return
+        if fn is None or bw_fn is None:
+            raise ValueError("set_rig_score_hooks: the forward and the backward hook are set together; (None, None) clears them")
+
+        def tramp(dm, n, P, sc, stream, user):
+            return int(fn(dm or 0, n, P, sc or 0, stream or 0))
+
+        def bw_tramp(dm, sg, n, P, out, stream, user):
+            return int(bw_fn(dm or 0, sg or 0, n, P, out or 0, stream or 0))
+
+        hooks = (SCORE_HOOK(tramp), SCORE_BACKWARD_HOOK(bw_tramp))
+        self._check(self.lib.dsac_set_rig_score_hooks(self.h, C.cast(hooks[0], C.c_void_p), C.cast(hooks[1], C.c_void_p), None))
+        self._rig_hooks = hooks   # the engine calls them until they are replaced or cleared
 
     def rig_pose_uncertainty_device(self, n, n_cameras, stream=None, **ptrs):
         """dsac_rig_pose_uncertainty_device (raw device pointers as ints): the covariance of each refined rig pose of the

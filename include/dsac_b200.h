@@ -610,6 +610,26 @@ int dsac_set_rig_pose_priors_device(dsac_engine* e, int32_t n_frames, int32_t n_
  * which the setting changed.  DSAC_ERR_ARG, with the engine left as it was: n_frames outside [1, max_frames] or not a
  * multiple of C, C outside [1, DSAC_MAX_RIG_CAMERAS], or a submitted pass that has not been awaited. */
 int dsac_set_rig_cell_depth_device(dsac_engine* e, int32_t n_frames, int32_t n_cameras, const float* d_depth, void* stream);
+/* Rig score hooks (INTEGRATION.md, "Rig score hooks"): the score seam for the rig passes.  With fwd and bwd registered, each
+ * dsac_forward_rig_device over n frames of C cameras, P = C * n_hyps:
+ *   score:  k_score_rig also writes the error image of camera frame f = r C + c against slot j of its rig's pool at the
+ *           composed pose T_c o T_j, diffmaps [n][P][N] float (k_score's arithmetic, clamped at 100; in an engine-owned
+ *           buffer, so write_diffmaps is not needed), then calls fwd(diffmaps, n, P, cam_scores, stream, user), which
+ *           overwrites the camera scores [n][P] double; the rig score of slot j is still their fp64 sum in camera order,
+ *           followed by the softmax, entropy and soft-argmax over the pool.  A nonzero return gives DSAC_ERR_ARG and the
+ *           engine then holds no pass.
+ *   backward: dsac_backward_rig_device and dsac_backward_rig_pose_device clamp the rig's score output gradients [R][P] to
+ *           +-grad_clamp, give them to each of its camera frames (d rig score / d camera score = 1) and call
+ *           bwd(diffmaps, score_grads [n][P], n, P, diffmap_grads [n][P][N] double, stream, user); the score term then reads
+ *           diffmap_grads in place of the closed-form soft-inlier derivative.  A nonzero return gives DSAC_ERR_ARG.  Both
+ *           refuse a rig pass that called other hooks, or none, than those registered now.
+ * dsac_rig_refined_jp6_device and dsac_rig_pose_uncertainty_device do not read the score and keep working after the hooks
+ * change; the covariance's support stays the closed-form reprojection count.  fwd and bwd are set together; both NULL clears
+ * them.  Sticky.  While they are registered every other forward entry point (dsac_forward, _submit, _device,
+ * dsac_forward_dsac, _device) refuses, naming this setter; the per-frame score hook (dsac_set_score_hook) still makes the rig
+ * pass refuse.  DSAC_ERR_ARG, with the engine left as it was: exactly one of fwd and bwd NULL, or a submitted pass that has
+ * not been awaited. */
+int dsac_set_rig_score_hooks(dsac_engine* e, dsac_score_hook fwd, dsac_score_backward_hook bwd, void* user);
 
 /* Soft-argmax backward seeded by d_grad_ref [n][6] = dOuter/d(refined jp6) instead of dLossMax.
  * No ground truth needed. dloss_dobj / dloss_dpred / clamp as in dsac_backward_device; clamp applies to the total. */
