@@ -11,6 +11,7 @@
     modes = pose_modes(engine, n, 4, 0.17, 100.0)                   # up to 4 distinct refined poses per frame
     loss = rig_softam_loss(engine, prediction, pix, ext, C, gt_rig)  # one loss per rig of C cameras, [n / C]
     pose = rig_softam_pose(engine, prediction, pix, ext, C)          # refined jp 6-vector per rig, [n / C][6]
+    modes = rig_pose_modes(engine, n, C, 4, 0.17, 100.0)             # up to 4 distinct refined poses per rig
 
 `prediction` is the coordinate CNN's output: float32 [n][1600][3] scene coordinates in metres on the engine's device,
 cell y*40+x.  It is the only input that receives a gradient.  The gradient is the one the reference hands to
@@ -405,6 +406,28 @@ def rig_pose_uncertainty(engine, n, n_cameras):
         out[k] = torch.empty((R,), dtype=torch.int32, device=dev)
     engine.rig_pose_uncertainty_device(n, int(n_cameras), torch.cuda.current_stream(dev).cuda_stream,
                                        **{k: v.data_ptr() for k, v in out.items()})
+    return out
+
+
+def rig_pose_modes(engine, n, n_cameras, max_modes, rot_rad, trans_mm):
+    """The distinct refined rig poses of each rig's pool after the engine's last rig pass over n frames of n_cameras
+    cameras (INTEGRATION.md, "Rig pose modes"), a dict of device tensors on torch.cuda.current_stream() shaped as
+    pose_modes shapes them, one row per rig (R = n / n_cameras): n_modes int32 [R]; hyp, members, steps_done, n_fit,
+    support and ok int32 [R][M]; score, mass and sigma2 float64 [R][M]; pose float64 [R][M][6] (cv rig poses, as the
+    poses of rig_priors= take them); cov_xi float64 [R][M][6][6] in the rig chart, M = max_modes.  hyp is the pool slot
+    c * n_hyps + h of the mode's seed (an index into rig_pose's rig_hyp, scores and sf), -1 for an unused entry.  These
+    outputs carry no autograd history."""
+    dev = torch.device("cuda", engine.cfg.device)
+    R, M = n // int(n_cameras), int(max_modes)
+    out = {"n_modes": torch.empty((R,), dtype=torch.int32, device=dev),
+           "pose": torch.empty((R, M, 6), dtype=torch.float64, device=dev),
+           "cov_xi": torch.empty((R, M, 6, 6), dtype=torch.float64, device=dev)}
+    for k in ("score", "mass", "sigma2"):
+        out[k] = torch.empty((R, M), dtype=torch.float64, device=dev)
+    for k in ("hyp", "members", "steps_done", "n_fit", "support", "ok"):
+        out[k] = torch.empty((R, M), dtype=torch.int32, device=dev)
+    engine.rig_pose_modes_device(n, int(n_cameras), M, rot_rad, trans_mm, torch.cuda.current_stream(dev).cuda_stream,
+                                 **{k: v.data_ptr() for k, v in out.items()})
     return out
 
 

@@ -290,8 +290,8 @@ struct dsac_engine {
     uint32_t* unc_status = nullptr;   // [R] dsac_rig_pose_uncertainty_device: the rig status its replay ORs the abort bit into
     DevMem<char> unc_buf;
     Event ev_unc;
-    // dsac_pose_modes_device: its seeds, recording replay and covariances in one grow-only block of its own, ordered by
-    // ev_modes as the uncertainty scratch is by ev_unc
+    // dsac_pose_modes_device and dsac_rig_pose_modes_device: their seeds, recording replay and covariances in one grow-only
+    // block of their own, ordered by ev_modes as the uncertainty scratch is by ev_unc
     DevMem<char> modes_buf;
     Event ev_modes;
     // dsac_forward_rig_device: the extrinsics, the pool, its rows and scores and the per-rig results, views into rig_buf
@@ -2226,3 +2226,4 @@ static int carve_scratch(dsac_engine* e, DevMem<char>& buf, std::initializer_lis
 #include "rig_host.inc"
 #include "rig_backward_host.inc"
 #include "rig_tracking_host.inc"
+#include "rig_modes_host.inc"

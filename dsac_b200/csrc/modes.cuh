@@ -4,7 +4,8 @@
 //   mode_dist        the distance between two translations
 //   mode_near        the nearness test: angle <= rot and distance <= trans
 //   k_mode_select    one CTA per frame: rank the occupied slots by score, walk them greedily into at most M seeds with
-//                    their mass and member count, and write the seeds' refinement jobs
+//                    their mass and member count, and write the seeds' refinement jobs; k_mode_select<true> does the
+//                    same for each rig's pool of C H lifted poses (dsac_rig_pose_modes_device)
 //   k_mode_merge     one warp per frame, after the refinement and the uncertainty of the seeds: merge seeds whose refined
 //                    poses are near an earlier survivor, compact, and gather the outputs
 //
@@ -16,6 +17,9 @@
 
 #include "pose_math.cuh"
 #include "prior.cuh"
+#if defined(__CUDACC__) && !defined(DSAC_HOST_ONLY)
+#include "refine.cuh"   // RIG_ST_SPOILED
+#endif
 
 namespace dsac {
 
@@ -58,12 +62,13 @@ DSAC_HD uint64_t mode_rank_key(bool occupied, double score) {
 #if defined(__CUDACC__) && !defined(DSAC_HOST_ONLY)
 
 struct ModeSelectParams {
-    const double* hyp_pose;    // [n][H][6]
-    const int32_t* img_idx;    // [n][H][4]
-    const double* scores;      // [n][H]
-    const double* sf;          // [n][H]
-    const uint32_t* status;    // [n]
+    const double* hyp_pose;    // [n][H][6]  (RIG: the pools [R][C H][6])
+    const int32_t* img_idx;    // [n][H][4]  (RIG: of the n = R C camera frames)
+    const double* scores;      // [n][H]     (RIG: [R][C H])
+    const double* sf;          // [n][H]     (RIG: [R][C H])
+    const uint32_t* status;    // [n]        (RIG: the rig status [R])
     int H, M, prior_k;         // slots per frame, modes per frame, priors of the pass (0: none)
+    int C;                     // RIG: cameras per rig
     double rot, trans;         // nearness radii (rad, mm)
     // per job j = f * M + m, seed m of frame f
     int32_t* job_frame;        // f, or -1 for no seed
@@ -83,21 +88,32 @@ constexpr int MODE_SELECT_THREADS = 256;
 // the ranking 32 slots at a time: each lane tests its slot against the existing seeds in seed order; the lowest-ranked
 // slot near none becomes the next seed (while fewer than M exist), and the slots after it are tested against that seed,
 // until no candidate is left.  Every slot's rotation is formed once, when its chunk is walked.
+// RIG (dsac_rig_pose_modes_device): CTA f is rig f and its slots are the S = C H slots of its pool, slot j = c H + h being
+// camera c's hypothesis h lifted to the rig frame (k_rig_lift).  Slot j is occupied when frame f C + c sampled h, or when
+// the pass had rig priors and h >= H - prior_k; a rig with DSAC_ST_BAD_RIG or DSAC_ST_BAD_PRIOR has none.  The walk, the
+// nearness and the mass are those of a frame, over the rig poses and the pool's sf.
+template <bool RIG = false>
 __global__ void __launch_bounds__(MODE_SELECT_THREADS, 1) k_mode_select(ModeSelectParams p) {
     __shared__ uint64_t s_key[1024];
     __shared__ uint16_t s_slot[1024];
     __shared__ double s_R[MODE_MAX][9], s_t[MODE_MAX][3];
     __shared__ int s_seed_slot[MODE_MAX];
     const int f = blockIdx.x, tid = threadIdx.x;
-    const int H = p.H;
+    const int H = RIG ? p.C * p.H : p.H;   // slots per pool
     int P = 1;
     while (P < H) P <<= 1;
-    const bool prior_ok = p.prior_k > 0 && !(p.status[f] & PRIOR_ST_BAD);
+    const bool prior_ok = RIG ? !(p.status[f] & RIG_ST_SPOILED) : p.prior_k > 0 && !(p.status[f] & PRIOR_ST_BAD);
     for (int i = tid; i < P; i += MODE_SELECT_THREADS) {
         uint64_t k = 0;
         if (i < H) {
             const size_t hi = (size_t)f * H + i;
-            const bool occupied = p.img_idx[hi * 4] >= 0 || (prior_ok && i >= H - p.prior_k);
+            bool occupied;
+            if constexpr (RIG) {   // prior_ok: the rig is not spoiled
+                const int c = i / p.H, h = i - c * p.H;
+                occupied = prior_ok && (p.img_idx[(((size_t)f * p.C + c) * p.H + h) * 4] >= 0 || (p.prior_k > 0 && h >= p.H - p.prior_k));
+            } else {
+                occupied = p.img_idx[hi * 4] >= 0 || (prior_ok && i >= H - p.prior_k);
+            }
             k = mode_rank_key(occupied, p.scores[hi]);
         }
         s_key[i] = k;

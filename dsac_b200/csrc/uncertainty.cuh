@@ -19,6 +19,7 @@ struct UncParams {
     const Cam* cams;            // [n] or null
     const double* eye;          // [n][N][3] (RGB-D) or null
     int jobs_per_frame;         // 1 (soft-argmax) or H (DSAC variant): job j belongs to frame j / jobs_per_frame
+                                // (RIG: to rig j / jobs_per_frame; M for the modes of a rig's pool)
     float thr;                  // thr2d, k_score's inlier threshold
     const double* pose;         // [jobs][6] cv pose of the recording replay
     const uint16_t* sel;        // [jobs][K4_MAX_INLIERS] cells of its last accepted step
@@ -38,8 +39,9 @@ constexpr int UNC_THREADS = 64, UNC_WARPS = UNC_THREADS / 32;
 // (score_pair_error on the pose's fp32 projection rows, built as k1_write_hyp builds them) below thr2d, every cell with
 // or without depth.  The 23 sums are reduced with the transposed butterfly, then the warps in order; one lane does the 6x6
 // work in fp64.
-// RIG (k_pose_uncertainty_rig, dsac_rig_pose_uncertainty_device): job r is rig r of rig.C cameras, pose the rig's, sel
-// entries cam << 11 | cell at a stride of C K4_MAX_INLIERS (k_refine_rig_rec).  A cell is set up in its own camera frame at
+// RIG (k_pose_uncertainty_rig, dsac_rig_pose_uncertainty_device and dsac_rig_pose_modes_device): job j belongs to rig
+// r = j / jobs_per_frame of rig.C cameras, pose a pose of the rig, sel entries cam << 11 | cell at a stride of
+// C K4_MAX_INLIERS per job (k_refine_rig_rec).  A cell is set up in its own camera frame at
 // the composed pose and mapped to the rig frame (ift_point_to_rig), as k_refine_ift_rig does; the support counts the cells
 // of every camera under its composed pose.  A rig with DSAC_ST_BAD_RIG or DSAC_ST_BAD_PRIOR in rig_status gets zeros.
 // RIG with RGBD (k_pose_uncertainty_rig_rgbd, RGB-D rigs): the residual is the cell's 3-vector in its own camera frame
@@ -58,7 +60,7 @@ __device__ __forceinline__ void k_pose_uncertainty_body(const UncParams& p, RigR
     const int16_t* coords = p.coords + (size_t)frame * DSAC_N_CONST * 3;
     const int32_t* pix = p.pix + (size_t)frame * p.pix_stride;
     if constexpr (RIG) {
-        if (rig_status[job] & RIG_ST_SPOILED) {   // (uniform over the CTA)
+        if (rig_status[frame] & RIG_ST_SPOILED) {   // (uniform over the CTA)
             if (tid < 36) {
                 if (p.cov_xi) p.cov_xi[(size_t)job * 36 + tid] = 0.0;
                 if (p.cov_jp6) p.cov_jp6[(size_t)job * 36 + tid] = 0.0;
@@ -80,7 +82,7 @@ __device__ __forceinline__ void k_pose_uncertainty_body(const UncParams& p, RigR
     for (int k = 0; k < 32; k++) v[k] = 0;
     for (int i = tid; i < cnt; i += UNC_THREADS) {
         if constexpr (RIG) {
-            const int code = sel[i], fr = job * n_cams + (code >> 11), cell = code & 2047;
+            const int code = sel[i], fr = frame * n_cams + (code >> 11), cell = code & 2047;
             const int16_t* co = p.coords + ((size_t)fr * DSAC_N_CONST + cell) * 3;
             const int32_t* px = p.pix + (size_t)fr * p.pix_stride + cell * 2;
             const double Y[3] = {(double)co[0], (double)co[1], (double)co[2]};
@@ -115,7 +117,7 @@ __device__ __forceinline__ void k_pose_uncertainty_body(const UncParams& p, RigR
     if constexpr (RIG) {   // support over every camera, under its composed pose (the rows k_rig_lift gives k_score)
         int sup = 0;
         for (int c2 = 0; c2 < n_cams; c2++) {
-            const int fr = job * n_cams + c2;
+            const int fr = frame * n_cams + c2;
             const double* E = rig.ext + (size_t)fr * 12;
             double Rk[9], tk[3];
             rig_compose(E, E + 9, R, pose + 3, Rk, tk);

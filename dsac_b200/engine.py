@@ -36,7 +36,7 @@ EXPORTS = [
     "dsac_last_pass", "dsac_set_pose_priors_device", "dsac_pose_modes_device", "dsac_forward_rig_device",
     "dsac_backward_rig_device", "dsac_backward_rig_pose_device", "dsac_rig_refined_jp6_device",
     "dsac_rig_pose_uncertainty_device", "dsac_set_rig_pose_priors_device", "dsac_set_rig_cell_depth_device",
-    "dsac_set_rig_score_hooks",
+    "dsac_set_rig_score_hooks", "dsac_rig_pose_modes_device",
 ]
 
 ST_OBJ_DRAW_EXHAUSTED = 8    # DSAC_ST_OBJ_DRAW_EXHAUSTED
@@ -245,6 +245,8 @@ def load(build_if_missing=True):
     lib.dsac_backward_rig_pose_device.argtypes = lib.dsac_backward_rig_device.argtypes
     lib.dsac_rig_refined_jp6_device.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.dsac_rig_pose_uncertainty_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(PoseUncertaintyOut), C.c_void_p]
+    lib.dsac_rig_pose_modes_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double,
+                                               C.POINTER(PoseModesOut), C.c_void_p]
     lib.dsac_set_rig_pose_priors_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_double,
                                                     C.c_void_p]
     lib.dsac_set_rig_cell_depth_device.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
@@ -772,6 +774,19 @@ class Engine:
                 raise KeyError(k)
             setattr(raw, k, v)
         self._check(self.lib.dsac_rig_pose_uncertainty_device(self.h, n, n_cameras, C.byref(raw), C.c_void_p(stream) if stream else None))
+
+    def rig_pose_modes_device(self, n, n_cameras, max_modes, rot_rad, trans_mm, stream=None, **ptrs):
+        """dsac_rig_pose_modes_device (raw device pointers as ints): the distinct refined rig poses of each rig's pool after
+        the preceding forward_rig_device over n frames of n_cameras cameras (INTEGRATION.md, "Rig pose modes"); ptrs: device
+        destinations of the fields of dsac_pose_modes_out, per rig (n_modes [R]; the others [R][max_modes](...),
+        R = n / n_cameras; hyp is the pool slot c * n_hyps + h)."""
+        raw = PoseModesOut()
+        for k, v in ptrs.items():
+            if k not in _MODES_FIELDS:
+                raise KeyError(k)
+            setattr(raw, k, v)
+        self._check(self.lib.dsac_rig_pose_modes_device(self.h, n, n_cameras, max_modes, float(rot_rad), float(trans_mm),
+                                                        C.byref(raw), C.c_void_p(stream) if stream else None))
 
     def last_pass(self, n):
         """dsac_last_pass: "softam", "dsac" or "rig", the kind of the pass over n frames the engine holds (what

@@ -561,6 +561,29 @@ int dsac_rig_refined_jp6_device(dsac_engine* e, int32_t n_frames, double* d_jp6,
  * NULL.  The outputs are not differentiated. */
 int dsac_rig_pose_uncertainty_device(dsac_engine* e, int32_t n_frames, int32_t n_cameras, const dsac_pose_uncertainty_out* d_out,
                                      void* stream);
+/* dsac_rig_pose_modes_device (INTEGRATION.md, "Rig pose modes"): dsac_pose_modes_device lifted to each rig's pool of
+ * P = C * n_hyps slots after a dsac_forward_rig_device over the same n_frames and n_cameras = C.  Every field of d_out is
+ * per rig: n_modes [R], the others [R][M](...), R = n_frames / C, M = max_modes.
+ *   1. slot j = c*H + h of rig r is occupied when frame r*C + c sampled hypothesis h (img_idx[f][h][0] >= 0), or when the
+ *      pass had rig pose priors (k of them) and h >= H - k; a rig with DSAC_ST_BAD_RIG or DSAC_ST_BAD_PRIOR has none and
+ *      gets n_modes 0;
+ *   2. the slots are ranked by the rig's scores (dsac_rig_out.scores: the hooks' with rig score hooks), descending, ties
+ *      to the lower slot, NaN after every score;
+ *   3. the walk, the nearness and the mass of dsac_pose_modes_device over the rig poses rig_hyp (rig frame) and the
+ *      pool's sf; hyp is the pool slot j of the seed (the index into rig_hyp, scores and sf), -1 unused;
+ *   4. each seed is refined from its rig pose as the rig pass refines its soft-argmax rig pose (pose, steps_done), over all
+ *      C cameras' cells (with rig cell depth, the Kabsch refinement of RGB-D rigs), and has the covariance that
+ *      dsac_rig_pose_uncertainty_device computes for a rig pose refined from there (cov_xi .. ok);
+ *   5. the merge of dsac_pose_modes_device.
+ * C = 1 with a zero extrinsic gives dsac_pose_modes_device's outputs after the ordinary pass bit for bit.  The score hooks
+ * are not read: the call keeps working after they change.  Ordered after the pass by an event, own scratch: it changes no
+ * output of the pass and no later result.  DSAC_ERR_ARG, with the engine left as it was: not after a
+ * dsac_forward_rig_device over n_frames, n_cameras not the pass's C, cameras, cell depth, pose priors, rig pose priors or rig
+ * cell depth changed since the pass, a submitted pass that has not been awaited, max_modes outside
+ * [1, min(n_hyps, DSAC_MAX_MODES)] (a rig's modes fit one rig pose priors setting), rot_rad or trans_mm not finite or
+ * negative, or d_out NULL.  The outputs are not differentiated. */
+int dsac_rig_pose_modes_device(dsac_engine* e, int32_t n_frames, int32_t n_cameras, int32_t max_modes, double rot_rad,
+                               double trans_mm, const dsac_pose_modes_out* d_out, void* stream);
 /* dsac_set_rig_pose_priors_device: k rig poses per rig join the pools of the following dsac_forward_rig_device passes over
  * n_frames frames of n_cameras = C cameras.  d_poses: DEVICE float64 [R][k][6] cv rig poses (X_cam = R_c (R_j Y + t_j) +
  * t_c); d_info: DEVICE float64 [R][k][6][6] information matrices in the rig chart R = exp([w]x) R_j, t = t_j + tau
